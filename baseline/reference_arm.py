@@ -4,7 +4,7 @@ Runs the UNMODIFIED reference package installed at ``baseline/_ref`` (``pip inst
 --target`` of /root/reference) through its own public API and stock code path:
 
 * one ``ArraysToArraysService(wrap_logp_grad_func(f))`` gRPC worker PROCESS per data shard
-  (the reference's deployment model, ``/root/reference/demo_node.py:98-108``), placed on the
+  (the reference's deployment model, ``demo_node.py:98-108``), placed on the
   GPU that owns the shard; ``f`` is plain PyTorch (two bf16 matmuls + elementwise) — none of
   this repository's kernels, models or engine;
 * the client is the reference's ``LogpGradServiceClient`` per worker, fanned out with

@@ -2,7 +2,7 @@
 
 Config (BASELINE.json): 8 shards x 10M rows x 256 features, bf16 design matrix, one theta per
 evaluation; shards are spread over the N GPUs (8/N per GPU => strong scaling).  Synthetic data,
-random parameters.  Contract: see the driver's instructions (one JSON line on rank 0).
+random parameters.  Output: one JSON line on rank 0.
 
     python bench.py                       # N=1, default steps
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -42,13 +42,14 @@ def parse_args():
                    help="BASELINE.json configuration (glm = the headline; --kernel fp8 is an alias of --config fp8)")
     p.add_argument("--series", type=int, default=20_000, help="ode: time series per shard")
     p.add_argument("--timepoints", type=int, default=32, help="ode: observations per series")
-    p.add_argument("--min-seconds", type=float, default=0.5,
-                   help="the S-step block is repeated until the timed region lasts this long; the median block counts")
     p.add_argument("--speculative-us", type=float, default=1000.0,
                    help="e2e region: FederatedEngine.set_speculative(wait_us) — the next evaluation's kernel is enqueued "
                         "before theta exists (0 = one launch per evaluation only)")
     p.add_argument("--nuts-draws", type=int, default=200, help="linreg: draws (= tune) of the NUTS run")
     p.add_argument("--out", default=None, help="also append the JSON line to this file")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="write what the last timed step computed ([logp, gradients...] as a caller receives them) "
+                        "to DIR/<name>.npy (float64)")
     return p.parse_args()
 
 
@@ -218,7 +219,7 @@ def build_workload(args, world, rank, dev):
             return ic, beta
 
         keys = {"rows_per_shard": args.rows, "features": P, "global_batch": args.shards * args.rows, "seq_len": P,
-                "l2_policy": "inputs (>= 2.5 GB per GPU) are larger than the 126 MB L2; no flush needed"}
+                "l2_policy": "inputs (>= 2.5 GB per GPU) are larger than the 50 MB L2; no flush needed"}
     elif args.config == "ode":
         shards = [synth_lv_shard(args.series, args.timepoints, seed=s, device=dev) for s in my_shards]
         model = OdeShards([s[0] for s in shards], [s[1] for s in shards], [s[2] for s in shards], [s[3] for s in shards])
@@ -327,49 +328,41 @@ def run_b200(args):
             print(json.dumps({"error": "verification failed", "max_rel_err": max_rel, "tolerance": tol, "n_gpus": world}),
                   flush=True)
         thetas = [draw_theta() for _ in range(W + S)]
-        # ---- warm-up through the public API, and a first estimate of the step time --------------------------
+        # ---- warm-up through the public API --------------------------
         share(W)
-        t0 = time.perf_counter()
         for i in range(W):
             eng.evaluate(*thetas[i])
-        est = max((time.perf_counter() - t0) / max(W, 1), 1e-6)
         barrier()
-        # the timed regions last at least --min-seconds: the S-step block is repeated, the MEDIAN block is reported
-        blocks = max(1, int(np.ceil(args.min_seconds / (est * S)))) if args.min_seconds > 0 else 1
-        blocks = min(blocks, 2000)
-        share(blocks * S)
+        share(S)
         sampler = ClockSampler(local_rank).start()
-        # ---- device-timed region: `blocks` x S back-to-back fused evaluations --------------------------------
-        block_ms = []
+        # ---- device-timed region: exactly S back-to-back evaluations ------------------------------------------
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         if backend == "fused":
             stream = eng.torch_stream()
             eng.set_device_theta(thetas[W], enable=True)
             launches0 = eng.kernel_launches
-            events = [torch.cuda.Event(enable_timing=True) for _ in range(blocks + 1)]
-            events[0].record(stream)
+            start.record(stream)
             last = 0
-            for bi in range(blocks):
-                for _ in range(S):
-                    last = eng.launch()
-                events[bi + 1].record(stream)
-            eng.wait(last)
-            events[-1].synchronize()
-            block_ms = [events[i].elapsed_time(events[i + 1]) for i in range(blocks)]
-            launches = (eng.kernel_launches - launches0) // blocks
+            for _ in range(S):
+                last = eng.launch()
+            end.record(stream)
+            last_vals = np.array(eng.wait(last), dtype=np.float64, copy=True)
+            end.synchronize()
+            launches = eng.kernel_launches - launches0
             eng.set_device_theta(thetas[W], enable=False)
         else:
-            events = [torch.cuda.Event(enable_timing=True) for _ in range(blocks + 1)]
-            events[0].record()
-            for bi in range(blocks):
-                for i in range(S):
-                    eng.evaluate_raw(thetas[W + i])
-                events[bi + 1].record()
-            events[-1].synchronize()
-            block_ms = [events[i].elapsed_time(events[i + 1]) for i in range(blocks)]
+            start.record()
+            for i in range(S):
+                last_vals = eng.evaluate_raw(thetas[W + i])
+            end.record()
+            end.synchronize()
             launches = 0
+        timed_ms = start.elapsed_time(end)
         barrier()
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, model.unpack_result(last_vals))
         # ---- end-to-end region: public API, pinned H2D of theta + D2H of the result each step -----------------
-        e2e_steps = share(blocks * S)
+        e2e_steps = share(S)
 
         evaluated = [0]   # evaluations of the current phase (the peers serve exactly as many as the root announced)
 
@@ -422,8 +415,8 @@ def run_b200(args):
             else:
                 spec_on = False
         clocks = sampler.stop()
-        result = dict(block_ms=block_ms, e2e_s=e2e_s, e2e_steps=e2e_steps, launches=launches, checksum=checksum,
-                      clocks=clocks, verified=verified, max_rel_err=max_rel, blocks=blocks, e2e_plain_s=e2e_plain_s,
+        result = dict(timed_ms=timed_ms, e2e_s=e2e_s, e2e_steps=e2e_steps, launches=launches, checksum=checksum,
+                      clocks=clocks, verified=verified, max_rel_err=max_rel, e2e_plain_s=e2e_plain_s,
                       e2e_speculative=spec_on, e2e_spec_s=locals().get("e2e_spec_s"))
     else:
         # peers: each phase serves exactly as many epochs as the root evaluates; their kernels wait on the
@@ -462,9 +455,7 @@ def run_b200(args):
     if rank != 0:
         return
 
-    block_ms = sorted(result["block_ms"])
-    med_ms = block_ms[len(block_ms) // 2]
-    ms_per_step = med_ms / S
+    ms_per_step = result["timed_ms"] / S
     value = 1000.0 / ms_per_step * K
     e2e_value = result["e2e_steps"] / result["e2e_s"] * K
     peaks = {}
@@ -472,7 +463,7 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet (HBM3)
     metric, model_name = CONFIGS[args.config]
     config = {
         "model": model_name,
@@ -483,9 +474,7 @@ def run_b200(args):
         "kernel": args.kernel if args.config == "glm" else args.config,
         "backend": backend,
         "comm": comm_mode,
-        "timed_blocks": result["blocks"],
-        "timed_seconds": sum(result["block_ms"]) / 1e3,
-        "block_ms_min_med_max": [block_ms[0], med_ms, block_ms[-1]],
+        "timed_seconds": result["timed_ms"] / 1e3,
         "hbm_bytes_per_eval_per_gpu": bytes_per_eval,
     }
     if bytes_per_eval:
@@ -493,11 +482,11 @@ def run_b200(args):
     if args.config in ("glm", "fp8"):
         # three-term roofline of the fused broadcast->compute->reduce kernel (seconds per eval per GPU):
         # HBM stream of the shard, tensor-core time of the two skinny GEMMs (N padded to 16 columns each),
-        # NVLink bytes (theta in, partial out) at the measured 770 GB/s peer bandwidth
+        # NVLink bytes (theta in, partial out) at 450 GB/s per direction (H100 SXM data sheet)
         config["roofline_s"] = {
             "hbm": bytes_per_eval / (hbm * 1e9),
-            "tensor": flops_per_eval * (32.0 / max(1, 4 * K)) / (peaks.get("bf16_tflops", 1590.0) * 1e12),
-            "nvlink": (n_theta_words * 4 + n_vals * 8) / 770e9,
+            "tensor": flops_per_eval * (32.0 / max(1, 4 * K)) / (peaks.get("bf16_tflops", 989.0) * 1e12),
+            "nvlink": (n_theta_words * 4 + n_vals * 8) / 450e9,
             "bound": "hbm",
         }
     line = {
@@ -542,6 +531,26 @@ def run_b200(args):
     if not result["verified"]:
         raise SystemExit(3)
     return line
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """``out_dir/<name>.npy`` (float64) per output of the last timed step: ``logp``, then ``grad_0``, ``grad_1``, ...
+    Above 64 MB in all, every output is replaced by the same fixed, seeded sample of its flattened entries
+    (sorted indices, ``numpy.random.default_rng(0)``), so two builds can still be compared entry for entry."""
+    import numpy as np
+
+    arrays = [np.asarray(a, dtype=np.float64) for a in arrays]
+    total = sum(a.nbytes for a in arrays)
+    os.makedirs(out_dir, exist_ok=True)
+    for i, a in enumerate(arrays):
+        if total > DUMP_LIMIT_BYTES:
+            keep = max(1, a.size * DUMP_LIMIT_BYTES // total)
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(keep, a.size), replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, "logp.npy" if i == 0 else f"grad_{i - 1}.npy"), a)
 
 
 def linreg_nuts(eng, args):
@@ -612,6 +621,8 @@ def run_reference(args):
 
 if __name__ == "__main__":
     a = parse_args()
+    if a.impl == "reference" and a.dump_outputs:
+        raise SystemExit("--dump-outputs needs the fused or the NCCL implementation (--impl b200 / nccl)")
     if a.impl == "reference":
         run_reference(a)
     else:

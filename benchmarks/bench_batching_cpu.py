@@ -3,9 +3,9 @@
 A node whose evaluator costs ``--launch-ms`` per launch *regardless of how many chains ride in it* — the
 cost model of the multi-chain tensor-core kernel, where the design matrix is streamed once per launch —
 is driven by C concurrent clients, with and without :class:`DynamicBatcher`.  This isolates what the
-batcher and the gRPC path add; the real kernel numbers come from ``examples/batched_serving.py`` on a B200.
+batcher and the gRPC path add; the real kernel numbers come from ``examples/batched_serving.py`` on an H100.
 
-    python benchmarks/bench_batching_cpu.py [--chains 8] [--launch-ms 2.0] [--out profiles/batching_cpu_r1.jsonl]
+    python benchmarks/bench_batching_cpu.py [--chains 8] [--launch-ms 2.0] [--out results.jsonl]
 """
 import argparse
 import asyncio

@@ -1,11 +1,11 @@
 """Chains in separate PROCESSES -> gRPC -> one GPU node, with and without dynamic batching.
 
 The reference's deployment: every chain of a sampler is a process with its own connection to the node
-(``/root/reference/pytensor_federated/service.py:266-275``, ``test_wrapper_ops.py:305-317``), and the node
+(``pytensor_federated/service.py:266-275``, ``test_wrapper_ops.py:305-317``), and the node
 answers the requests one after the other.  Here the node puts the requests that are waiting into ONE
 multi-chain launch of the tensor-core GLM kernel (``DynamicBatcher`` + ``GlmShards(n_chains=K)``).
 
-    python benchmarks/bench_batching_gpu.py --chains 8 16 --evals 300 --out profiles/batching_gpu_r2.jsonl
+    python benchmarks/bench_batching_gpu.py --chains 8 16 --evals 300 --out results.jsonl
 
 One JSON line per (chains, mode): aggregate chain-evaluations per second measured in the client processes
 (start barrier -> last client done), launches used, mean batch size.

@@ -1,7 +1,7 @@
 """Secondary benchmarks for the other BASELINE.json configurations (single process, GPU 0..N-1 via
 the in-process launcher is not used here: these are per-GPU numbers at N = 1 unless torchrun is used).
 
-    python benchmarks/bench_configs.py --out gpurun_out/configs.jsonl
+    python benchmarks/bench_configs.py --out configs.jsonl
 
 Each line: config name, backend (fused | collective = stock PyTorch eager + (no-op) collectives),
 evals/s measured end to end through ``FederatedEngine.evaluate`` (pinned H2D theta, D2H result),
@@ -101,7 +101,7 @@ def main():
         emit(config=f"hierarchical logistic GLM, 8 groups x {args.fp8_rows} x 256, fp8 block-scaled, 1 GPU", backend="fused",
              evals_per_s=rate, latency_us=lat, hbm_bytes_per_eval=model.bytes_per_eval(),
              hbm_tb_per_s=model.bytes_per_eval() * rate / 1e12)
-    # 5) sampling throughput: lock-step HMC, K chains per fused launch (tcgen05 kernel) vs K = 1
+    # 5) sampling throughput: lock-step HMC, K chains per fused launch (tensor-core kernel) vs K = 1
     from pytensor_federated_b200.models import GlmShards, synth_logistic_shard
     from pytensor_federated_b200.sampling import glm_batch_fn, hmc_sample_batched
 

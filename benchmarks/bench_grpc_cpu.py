@@ -4,7 +4,7 @@ Runs the SAME numpy model behind (a) the unmodified reference's ArraysToArraysSe
 + dependency shims) and (b) this package's service, and times the reference-style client calls:
 sequential ``evaluate`` and the ``asyncio.gather`` fan-out of a fused graph node.  CPU only.
 
-    python benchmarks/bench_grpc_cpu.py [--out profiles/grpc_cpu_r1.jsonl]
+    python benchmarks/bench_grpc_cpu.py [--out results.jsonl]
 """
 import argparse
 import asyncio

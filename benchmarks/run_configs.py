@@ -5,7 +5,7 @@ eight-fold.  This runner initialises NCCL once and then calls `bench.run_b200` f
 (every run still prints its own JSON line and verifies against the fp64 oracle first).
 
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29600 \
-        benchmarks/run_configs.py --gpus 8 --out profiles/configs_r2.jsonl glm trace fp8 linreg nccl
+        benchmarks/run_configs.py --gpus 8 --out results.jsonl glm trace fp8 linreg nccl
 """
 import argparse
 import os

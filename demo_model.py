@@ -1,6 +1,6 @@
 """Client-side demo: a hierarchical linear model over N federated nodes, MAP + NUTS.
 
-Same model as the reference's ``demo_model.py`` (``/root/reference/demo_model.py:24-44``):
+Same model as the reference's ``demo_model.py`` (``demo_model.py:24-44``):
 ``intercept_mu ~ N(0,1)``, ``intercept[i] ~ N(intercept_mu, 0.1)``, ``slope ~ N(0,1)`` and one
 remote log-likelihood per node with offset intercepts, each entering as a potential.
 
@@ -62,7 +62,7 @@ def run_model(remote_ops, n: int, tune: int, draws: int, chains: int = 1):
 def run_model_pymc(remote_ops, n: int, tune: int, draws: int):
     """The same model through PyMC (needs PyMC + PyTensor; the Ops are then genuine PyTensor Ops).
 
-    Mirrors ``/root/reference/demo_model.py:28-44``; not executable in the offline B200 image.
+    Mirrors ``demo_model.py:28-44``; not executable in the offline image.
     """
     import arviz
     import pymc as pm

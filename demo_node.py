@@ -1,9 +1,9 @@
 """Worker-node launcher: serves the demo linear model behind the ArraysToArrays gRPC schema.
 
 CLI-compatible with the reference's ``demo_node.py`` (``--bind --ports --delay``, one OS process
-per port, ``/root/reference/demo_node.py:98-134``); any pytensor-federated client can connect.
+per port, ``demo_node.py:98-134``); any pytensor-federated client can connect.
 The node's private dataset lives on the GPU when one is visible (``--device cuda``) and each
-evaluation is one fused sm_100a kernel launch; ``--device cpu`` uses the eager oracle.
+evaluation is one fused sm_90a kernel launch; ``--device cpu`` uses the eager oracle.
 
 For the on-box data plane (no sockets at all) see ``demo_model.py --fused``.
 """

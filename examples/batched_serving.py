@@ -5,7 +5,7 @@
 Starts a gRPC node whose compute function is a K-chain `FederatedEngine(GlmShards(..., n_chains=K))`
 behind a `DynamicBatcher`, then drives it with `--chains` concurrent clients the way independent chains of
 a sampler would.  Requests that arrive together ride in ONE fused launch (chains sit on the MMA N axis of
-the tcgen05 kernel), so the node's throughput grows with the number of chains instead of being divided
+the tensor-core kernel), so the node's throughput grows with the number of chains instead of being divided
 by it.  `--no-batching` serves the same clients one request per launch for comparison.  Runs on CPU too
 (eager baseline kernel), where it only demonstrates the plumbing.
 """

@@ -1,5 +1,5 @@
 """Federated parameter estimation for YOUR ODE — the use case the reference's README sketches
-(`/root/reference/README.md:39-52`: the data and the solver stay on the node, only theta and [LL, dLL/dtheta] travel).
+(`README.md:39-52`: the data and the solver stay on the node, only theta and [LL, dLL/dtheta] travel).
 
     python examples/custom_ode.py [--series 2000] [--nodes 3]
 

@@ -4,8 +4,8 @@
     torchrun --nproc-per-node 4 --master-addr 127.0.0.1 examples/federated_glm.py --chains 8
 
 Every rank builds its *private* shard; rank 0 is the client and runs lock-step HMC with `--chains`
-chains per fused evaluation; the other ranks serve.  On GPUs the evaluation is the fused sm_100a
-kernel (θ multicast over NVSwitch → tcgen05 GEMMs → NVLink reduce); on CPU it is the gloo/eager
+chains per fused evaluation; the other ranks serve.  On GPUs the evaluation is the fused sm_90a
+kernel (θ multicast over NVSwitch → wgmma GEMMs → NVLink reduce); on CPU it is the gloo/eager
 baseline with the same API.
 """
 import argparse

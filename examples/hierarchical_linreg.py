@@ -3,7 +3,7 @@ written the two ways this package offers, on N nodes (GPUs, or CPU processes for
 
     python examples/hierarchical_linreg.py --nodes 8 --draws 300
 
-1. one `FederatedLogpGradOp` per node, as in the reference (`/root/reference/demo_model.py:28-36`): the
+1. one `FederatedLogpGradOp` per node, as in the reference (`demo_model.py:28-36`): the
    `fuse_asyncs` rewrite answers all of them with ONE fused launch per model evaluation;
 2. ONE Op for the whole federation (`NodeFederation.all_nodes_op`): vector of node intercepts in, summed
    log-likelihood and per-node gradients out — the graph no longer grows with the number of nodes.

@@ -1,7 +1,7 @@
 """Checks that the .proto sources, the runtime descriptors and the hand-written
 codec agree, and (when ``protoc`` exists) regenerates stock ``*_pb2.py`` files.
 
-Counterpart of ``/root/reference/protobufs/generate.py`` — but the package does
+Counterpart of ``protobufs/generate.py`` — but the package does
 not depend on generated code, so this is a verification tool, not a build step.
 """
 import pathlib

@@ -1,7 +1,7 @@
-"""B200-native federated log-probability / gradient engine.
+"""GPU-native federated log-probability / gradient engine.
 
 The top level offers the names a user of the reference imports from ``pytensor_federated``
-(``/root/reference/pytensor_federated/__init__.py:1-22``) plus, lazily, the engine-side entry points
+(``pytensor_federated/__init__.py:1-22``) plus, lazily, the engine-side entry points
 (``FederatedEngine``, ``NodeFederation``, ``launch_federation``, ``DynamicBatcher``).  Nodes need neither
 PyTensor nor torch to import this package: the graph Ops come from the backend shim
 (:mod:`._graph_backend`) and everything GPU-related is imported on first use.

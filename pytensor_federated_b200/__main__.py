@@ -1,7 +1,7 @@
 """``python -m pytensor_federated_b200 [info|build|serve-demo]`` — small operator CLI.
 
 * ``info``  — version, native library, graph backend, visible GPUs, TLS / metrics configuration.
-* ``build`` — compile ``libb200fed.so`` for sm_100a (same as ``python -m pytensor_federated_b200.build``).
+* ``build`` — compile ``libb200fed.so`` for sm_90a (same as ``python -m pytensor_federated_b200.build``).
 """
 from __future__ import annotations
 
@@ -46,7 +46,7 @@ def main(argv=None) -> int:
     parser = argparse.ArgumentParser(prog="python -m pytensor_federated_b200")
     sub = parser.add_subparsers(dest="command")
     sub.add_parser("info", help="print the installation / configuration summary as JSON")
-    b = sub.add_parser("build", help="compile the native library for sm_100a")
+    b = sub.add_parser("build", help="compile the native library for sm_90a")
     b.add_argument("--force", action="store_true")
     args = parser.parse_args(argv)
     if args.command == "build":

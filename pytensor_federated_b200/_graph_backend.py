@@ -1,9 +1,9 @@
 """Selects the symbolic-graph backend of the Op layer.
 
 * PyTensor installed → the Ops are genuine PyTensor Ops (drop-in for models written against the
-  reference; import list mirrors ``/root/reference/pytensor_federated/op_async.py:4-11`` and
+  reference; import list mirrors ``pytensor_federated/op_async.py:4-11`` and
   ``wrapper_ops.py:4-8``).
-* PyTensor missing (the B200 image) → the in-repo IR :mod:`pytensor_federated_b200.graph`, which
+* PyTensor missing (the offline image) → the in-repo IR :mod:`pytensor_federated_b200.graph`, which
   implements the same names.  Set ``B200FED_GRAPH_BACKEND=builtin`` to force it.
 """
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """Minimal proto3 wire-format primitives (no protoc, no generated code).
 
 The reference generates its message classes with ``protoc`` + the betterproto
-plugin (``/root/reference/protobufs/generate.py:15-27``).  Neither tool exists in
+plugin (``protobufs/generate.py:15-27``).  Neither tool exists in
 this image, and the schema is five tiny messages, so the wire format is written
 out by hand here: varints, length-delimited fields and fixed32 floats.  The byte
 layout is the proto3 standard one, so these messages interoperate with a stock

@@ -1,8 +1,8 @@
 """Dynamic batching of concurrent requests on a serving node.
 
 The reference serves every request of every client one after the other
-(``/root/reference/pytensor_federated/service.py:104-112``): four MCMC chains that share a node cost four
-evaluations.  On a B200 node the tensor-core GLM kernel evaluates up to 16 chains in ONE launch for
+(``pytensor_federated/service.py:104-112``): four MCMC chains that share a node cost four
+evaluations.  On a GPU node the tensor-core GLM kernel evaluates up to 16 chains in ONE launch for
 roughly the price of one (the design matrix is streamed once, chains ride along the MMA N dimension —
 ``csrc/glm_tc.cu``).  :class:`DynamicBatcher` is the piece that lets a gRPC node exploit this: requests
 that arrive within a short window are stacked, evaluated by one batched call, and un-stacked into their

@@ -1,4 +1,4 @@
-"""In-tree build of the native library (``libb200fed.so``) for sm_100a.
+"""In-tree build of the native library (``libb200fed.so``) for sm_90a.
 
 No torch headers and no pybind: the library is plain CUDA runtime + a C ABI, loaded with
 ``ctypes`` (see :mod:`pytensor_federated_b200.ops.native`).  That keeps a full rebuild at a
@@ -21,7 +21,7 @@ BUILD = CSRC / "build"
 LIB = PKG / "libb200fed.so"
 
 SOURCES = ["runtime.cu", "linreg.cu", "glm_simt.cu", "glm_tc.cu", "glm_fp8.cu", "glm_generic.cu", "ode.cu", "ode_generic.cu", "codec.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -61,7 +61,7 @@ def is_current() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) -> Path:
-    """Compiles every ``.cu`` under ``csrc/`` for sm_100a and links ``libb200fed.so``."""
+    """Compiles every ``.cu`` under ``csrc/`` for sm_90a and links ``libb200fed.so``."""
     if not force and is_current():
         return LIB
     nvcc = nvcc_path()
@@ -93,8 +93,8 @@ def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) 
 
 
 def dump_sass(out_dir: Optional[Path] = None) -> Path:
-    """Writes ``cuobjdump -sass`` of the library (evidence for UTC*MMA / UTMALDG / multimem)."""
-    out_dir = Path(out_dir or PKG.parent / "profiles")
+    """Writes ``cuobjdump -sass`` of the library (HGMMA / UTMALDG / multimem instructions) to ``out_dir``."""
+    out_dir = Path(out_dir or BUILD)
     out_dir.mkdir(parents=True, exist_ok=True)
     out = out_dir / "libb200fed.sass"
     res = subprocess.run(["cuobjdump", "-sass", str(LIB)], capture_output=True, text=True, check=True)

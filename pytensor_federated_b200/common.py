@@ -1,6 +1,6 @@
 """Bayesian-flavoured adapters around the ArraysToArrays transport.
 
-Reference: ``/root/reference/pytensor_federated/common.py:12-161``.  Server side:
+Reference: ``pytensor_federated/common.py:12-161``.  Server side:
 ``wrap_logp_func`` / ``wrap_logp_grad_func`` turn a log-probability function into a
 ``ComputeFunc`` and validate what it returns (same exception types and messages as
 the reference, ``:17-21`` and ``:31-46``).  Client side: ``LogpServiceClient`` /

@@ -92,7 +92,7 @@ class TlsConfigError(ValueError):
 @dataclasses.dataclass(frozen=True)
 class TlsConfig:
     """TLS material of the gRPC path (PEM bytes).  The reference only speaks plaintext
-    (``grpclib.client.Channel(host, port)``, ``/root/reference/pytensor_federated/service.py:230``); nodes
+    (``grpclib.client.Channel(host, port)``, ``pytensor_federated/service.py:230``); nodes
     that hold private data usually sit behind TLS, optionally with client certificates.
 
     Server: ``cert`` + ``key`` (its identity); ``ca`` + ``mutual=True`` additionally demands client certs.

@@ -3,7 +3,7 @@
 // InputArrays / OutputArrays = { repeated npproto.ndarray items = 1; string uuid = 2; }
 // npproto.ndarray            = { bytes data = 1; string dtype = 2; repeated int64 shape = 3 [packed];
 //                                repeated int64 strides = 4 [packed]; }
-// Schema: /root/reference/protobufs/service.proto:6-19, npproto/ndarray.proto:7-12.  The Python
+// Schema: protobufs/service.proto:6-19, npproto/ndarray.proto:7-12.  The Python
 // implementation (pytensor_federated_b200/_pb.py, rpc.py) is the fallback and the oracle: both must
 // produce identical bytes (tests/test_native_codec.py).  One call encodes a whole message into a
 // caller-provided buffer with a single memcpy per array; decoding returns offsets so that NumPy can

@@ -1,4 +1,4 @@
-// Device-side federation protocol shared by every model kernel (sm_100a).
+// Device-side federation protocol shared by every model kernel (sm_90a).
 //
 // One evaluation ("epoch") of a federated log-likelihood is ONE kernel per GPU:
 //
@@ -16,7 +16,7 @@
 //
 // This replaces the reference's per-evaluation path of
 //   npproto encode -> HTTP/2 send -> decode -> compute -> encode -> recv -> decode
-// (/root/reference/pytensor_federated/service.py:150-158, :45-72) and the
+// (pytensor_federated/service.py:150-158, :45-72) and the
 // client-side graph sum over nodes, with zero host involvement on the nodes.
 //
 // Memory-model notes: data is written with weak stores, then

@@ -1,37 +1,28 @@
-// Federated logistic GLM on a BLOCK-SCALED FP8 design matrix (tcgen05.mma kind::mxf8f6f4.block_scale).
+// Federated logistic GLM on a BLOCK-SCALED FP8 design matrix (Hopper: wgmma e4m3 + TMA + mbarrier).
 //
 // Storage: X as e4m3 bytes + one UE8M0 scale per 32 x 32 block (32 rows x 32 features):
 //     x[r, f] = e4m3(Xq[r, f]) * 2^(S[r/32, f/32] - 127)
-// The kernel receives the scales pre-packed per 128-row tile in the word order of the TMEM
-// scale-factor columns (16 words per tile), so the epilogue warps only move them.
-// i.e. 1.03 bytes per element instead of 2 for bf16 -> the HBM-bound evaluation gets ~2x faster.
+// i.e. 1.03 bytes per element instead of 2 for bf16 -> the HBM-bound evaluation reads half the bytes.
+// The scales come pre-packed per 128-row tile (models/glm.py: pack_tile_scales); this kernel reads byte
+// 32 + 4 fb + q of a tile's 64 = the scale of (row group q, feature block fb).
 //
-// Both GEMMs consume the quantised tile directly; the dequantisation is done by the tensor core.
-// TMEM scale-factor layout (cta_group::1, M = 128, 32-element blocks): the scale of operand row m
-// for K-block j sits in lane m % 32 (replicated in all four 32-lane subpartitions), 32-bit column
-// base + 4*(j/4) + m/32, byte j % 4 — the byte is selected by the instruction descriptor's sf_id.
-// With 32-row x 32-feature blocks every lane holds the same word, so the epilogue warps can
-// write the scale words with plain tcgen05.st:
-//   MMA #1  eta[128 x 16] += Xq_tile[:, feature block fb] . Theta^T     rows m -> row group m/32:
-//           column 4*(fb/4) + q holds the scales of (row group q, feature blocks 4*(fb/4)..+3),
-//           sf_id = fb % 4.
-//   MMA #2  G[128 feat x 16] += Xq_tile^T[:, row group q] . R           rows m -> feature block
-//           4h + m/32: column 4h + qq holds the scales of (row groups 0..3, feature block 4h+qq),
-//           sf_id = q.
-//   Scale-factor-B is the constant 2^0 for MMA #1 and for the logistic family (|r| <= 1).
-//   Poisson / Gaussian residuals are unbounded: there (template DYN) every 32-row group of R gets
-//   its own UE8M0 scale — warp max -> exponent, exchanged through shared memory, written to the
-//   scale-factor-B columns of the R buffer by the epilogue warps, byte selected by b_sf_id = row
-//   group — so the radix-16 expansion is relative to the block maximum, which is what the
-//   block-scaled MMA is for.
-// Theta and the residuals are themselves e4m3: theta is a 5-term, r a 4-term radix-16 expansion
-// (term k carries weight 16^-k), the terms sit in separate N columns and are recombined in the
-// epilogue in fp32, so the low precision of the operands does not leak into the result.
+// Hopper has no block-scaled MMA:
+//   MMA #1  eta[64 rows x 24] = Xd_rows . Theta^T   on a dequantised bf16 copy of the consumer's rows: an e4m3
+//           value times its power-of-two block scale is exact in bf16, so the copy IS the design matrix and
+//           the MMA runs as one chain.  Theta is a 3-way bf16 split as in glm_tc.cu (the fp8 wgmma accumulates
+//           with fewer mantissa bits than fp32, which eta, a long dot product with cancellation, cannot afford).
+//   MMA #2  G[64 feat x 32] += sum_rg S[rg, fb] * s_r[rg] * (Xq^T[feat, rg] . R[rg])   in e4m3, the block scales
+//           applied in fp32 registers after each 32-row K step; 8-bit wgmma operands must be K-major, so it reads
+//           a transposed copy of the tile that each consumer warpgroup writes for its feature half.
+// The residuals are a 4-term radix-16 e4m3 expansion (term k carries weight 16^-k) in separate N columns,
+// recombined in fp32/fp64, so the low precision of the operand does not leak into the gradient.
+// Poisson / Gaussian residuals are unbounded: there (template DYN) every 32-row group of R gets its own
+// power-of-two scale s_r (from the group's largest |r|), so the expansion is relative to the block maximum.
 //
-// Pipeline/roles as in glm_tc.cu; scale words are written to TMEM kEG tiles ahead by the
-// epilogue warps (tcgen05.st), 2*kEG-deep ring.  Workload: BASELINE.json "hierarchical GLM, 8
-// partial-pooling groups (one per GPU), fp8 block-scaled design matrix" (groups = intercepts).
+// Roles and pipeline as in glm_tc.cu.  Workload: BASELINE.json "hierarchical GLM, 8 partial-pooling groups
+// (one per GPU), fp8 block-scaled design matrix" (groups = intercepts).
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_fp8.h>
 #include <cuda_runtime.h>
 
@@ -46,42 +37,16 @@ using namespace tc;
 constexpr int kTile = 128;            // rows per tile
 constexpr int kPanelF = 128;          // features per 128-byte swizzle span (1 byte / element)
 constexpr int kPanelB = kTile * 128;  // 16 KB
-constexpr int kEG = 3;                // epilogue groups; tile t belongs to group t % kEG (own eta / R buffers)
-constexpr int kThreadsF = 32 * (3 + 4 * kEG);  // warps: 0 TMA, 1 MMA#1, 2-5 group 0, 6 MMA#2, 7-10 group 1, 11-14 group 2
-constexpr int kMaxChunkF = 30;        // tiles per chunk at most (fp32 accumulation in TMEM), a multiple of kEG
+constexpr int kThreadsF = 384;        // warpgroup 0: TMA producer (warp 0 only), warpgroups 1, 2: consumers
+constexpr int kConsumerWarpsF = 8;
+constexpr int kChunkMultiple = 3;     // tiles per chunk: a multiple of this (chunk table shared with older layouts)
+constexpr int kMaxChunkF = 30;        // tiles per chunk at most (fp32 register accumulation)
 constexpr int kMinChunkF = 6;
 constexpr int kRingF = 16;            // published chunks the consumers may lag behind
-constexpr int kLLRowsF = 4 * kEG;     // epilogue warps: per-warp slots of the warp-level sums
-constexpr int kN = 16;                // MMA N for both GEMMs
-constexpr int kThetaTerms = 5;
+constexpr int kLLRowsF = 12;          // per-warp slot rows of the warp-level sums (>= kConsumerWarpsF)
 constexpr int kResidTerms = 4;
-constexpr int kSfRing = 2 * kEG;      // scale words are written kEG tiles ahead
-
-__device__ __forceinline__ void umma_fp8_block_scaled(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                      uint32_t accumulate, uint32_t tmem_sfa, uint32_t tmem_sfb) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t"
-        "}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb)
-        : "memory");
-}
-// Block-scaled instruction descriptor: e4m3 x e4m3 -> f32, UE8M0 scales, K = 32.
-__host__ __device__ constexpr uint32_t make_idesc_bs(int M, int N, int a_mn_major, int b_mn_major) {
-    return ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | (1u << 23) |
-           ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t (&w)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(w[0]),
-                 "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_x1(uint32_t taddr, uint32_t w) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(w) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+constexpr int kN1 = 24;               // eta columns: bf16 term t (hi, mid, lo) of chain k in column 8 t + k
+constexpr int kN2 = 8 * kResidTerms;  // residual columns: term t of chain k in column 8 t + k
 
 __device__ __forceinline__ uint8_t to_e4m3(float v) {
     return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
@@ -100,9 +65,11 @@ __device__ __forceinline__ void expand16(float v, uint8_t (&terms)[T]) {
         rem = (rem - from_e4m3(terms[k])) * 16.f;
     }
 }
+__device__ __forceinline__ float ue8m0(uint32_t b) { return __uint_as_float(b << 23); }
 
 struct SmemLayoutF {
-    uint32_t stages, stage_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_theta_f, off_ring, off_bars, off_tmem, total;
+    uint32_t stages, stage_bytes, off_xb, xb_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_xt, xt_bytes, off_theta_f,
+        off_ring, off_bars, off_misc, total;
 };
 // doubles per CTA row of the partial array: (hi, lo) pairs of the n_vals outputs, then the per-warp slots
 // [kLLRowsF][KF][1 + G] of the warp-level sums (log-likelihood, intercept gradients) — see csrc/glm_tc.cu
@@ -113,25 +80,29 @@ __host__ __device__ inline SmemLayoutF smem_layout(int P, int n_theta, int n_gro
     SmemLayoutF L;
     const uint32_t panels = P / kPanelF;
     L.stage_bytes = panels * kPanelB;
-    L.theta_b_bytes = panels * kN * 128;
-    L.r_bytes = kTile * kN;  // 1 byte per element
-    const uint32_t fixed = L.theta_b_bytes + kEG * L.r_bytes + ((n_theta * 4 + 15) & ~15) + kRingF * 24 + 512 + 1024;
+    L.xb_bytes = P * 128;             // one consumer warpgroup's 64 rows in bf16: P / 64 panels of 64 rows x 128 bytes
+    L.theta_b_bytes = (P / 64) * kN1 * 128;
+    L.r_bytes = kTile * kN2;   // 1 byte per element
+    L.xt_bytes = (P / 2) * kTile;   // one consumer warpgroup's transposed feature half
+    const uint32_t fixed = 2 * L.xb_bytes + L.theta_b_bytes + 2 * L.r_bytes + 2 * L.xt_bytes + ((n_theta * 4 + 15) & ~15) +
+                           kRingF * 24 + 256 + 768 + 1024;
     uint32_t stages = (227u * 1024u - fixed) / L.stage_bytes;
     if (stages > 6) stages = 6;
     L.stages = stages;
     uint32_t o = stages * L.stage_bytes;
+    L.off_xb = o; o += 2 * L.xb_bytes;
     L.off_theta_b = o; o += L.theta_b_bytes;
-    L.off_r = o; o += kEG * L.r_bytes;
+    L.off_r = o; o += 2 * L.r_bytes;
+    L.off_xt = o; o += 2 * L.xt_bytes;
     L.off_theta_f = o; o += (n_theta * 4 + 15) & ~15;
     L.off_ring = o; o += kRingF * 24;   // published chunks + one mbarrier per ring slot
-    L.off_bars = o; o += 320;
-    L.off_tmem = o; o += 192;  // tmem slot, theta norms, residual-exponent exchange (DYN)
+    L.off_bars = o; o += 256;
+    L.off_misc = o; o += 768;           // per-warp residual maxima, residual scales (DYN)
     L.total = o + 1024;
     return L;
 }
 
-// KF = chains per launch: 1 or 3 (3 x 5 theta terms and 3 x 4 residual terms fit the 16 MMA columns);
-// DYN = per-row-group residual scales (families with unbounded residuals)
+// KF = chains per launch: 1 or 3; DYN = per-row-group residual scales (families with unbounded residuals)
 template <int KF, bool DYN>
 __global__ void __launch_bounds__(kThreadsF, 1)
 fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
@@ -143,59 +114,36 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
 
     const int P = prm.n_features;
     const int G = prm.n_groups;
-    const int NH = P / 128;       // 128-feature panels == UMMA M blocks of MMA #2
-    const int NFB = P / 32;       // 32-feature scale blocks == K steps of MMA #1
+    const int NH = P / 128;       // 128-feature panels
     const SmemLayoutF L = smem_layout(P, comm.n_theta, G);
     const int S = (int)L.stages;
 
     unsigned char* theta_b = smem + L.off_theta_b;
     unsigned char* r_buf = smem + L.off_r;
+    unsigned char* xt_buf = smem + L.off_xt;
     float* theta_f = reinterpret_cast<float*>(smem + L.off_theta_f);
     int4* ring = reinterpret_cast<int4*>(smem + L.off_ring);          // published chunks: (segment or -1, first tile, tiles, -)
     uint64_t* bar_ring = reinterpret_cast<uint64_t*>(smem + L.off_ring + kRingF * 16);   // slot j % kRingF: chunk j published
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L.off_tmem);
-    float* theta_norm = reinterpret_cast<float*>(smem + L.off_tmem + 16);  // c: theta = c * sum_k t_k 16^-k
-    uint8_t* r_expo = smem + L.off_tmem + 64;  // [group][tile parity][chain (3)][row group (4)] UE8M0 bytes
+    unsigned char* xb_buf = smem + L.off_xb;
+    float* r_wmax = reinterpret_cast<float*>(smem + L.off_misc);            // [8 warps][8 chain slots] max |r| over 16 rows
+    float* r_scale = reinterpret_cast<float*>(smem + L.off_misc + 256);     // [2 R buffers][4 row groups][8 chain slots]
     uint64_t* bar_full = bars;            // [6]
-    uint64_t* bar_empty = bars + 6;       // [6]
-    uint64_t* bar_eta_full = bars + 12;             // [kEG]
-    uint64_t* bar_eta_empty = bars + 12 + kEG;      // [kEG]
-    uint64_t* bar_r_full = bars + 12 + 2 * kEG;     // [kEG]
-    uint64_t* bar_r_empty = bars + 12 + 3 * kEG;    // [kEG]
-    uint64_t* bar_g_full = bars + 12 + 4 * kEG;     // [2]
-    uint64_t* bar_g_empty = bars + 14 + 4 * kEG;    // [2]
-    uint64_t* bar_sf_full = bars + 16 + 4 * kEG;    // [kSfRing]   (16 + 6 kEG <= 40 barriers = 320 bytes)
-    static_assert(16 + 4 * kEG + kSfRing <= 40, "barrier block too small");
+    uint64_t* bar_empty = bars + 6;       // [6]   (bars + 128 B: chunk decision)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
     // ---- theta-independent setup: BEFORE the dependency wait inside fed::prologue, so that it overlaps with the
     // tail of the previous evaluation under programmatic dependent launch (see csrc/glm_tc.cu)
-    constexpr uint32_t kTmemCols = 256;
-    for (int i = threadIdx.x; i < (int)(kEG * L.r_bytes / 16); i += blockDim.x)
-        reinterpret_cast<uint4*>(r_buf)[i] = make_uint4(0, 0, 0, 0);
     if (threadIdx.x == 0) {
         *pipeline_fault() = 0;
         for (int i = 0; i < kRingF; ++i) mbar_init(&bar_ring[i], 1);
-        for (int i = 0; i < 6; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < kEG; ++i) {
-            mbar_init(&bar_eta_full[i], 1);
-            mbar_init(&bar_eta_empty[i], 128);
-            mbar_init(&bar_r_full[i], 128);
-            mbar_init(&bar_r_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&bar_g_full[i], 1);
-            mbar_init(&bar_g_empty[i], 128);
-        }
-        for (int i = 0; i < kSfRing; ++i) mbar_init(&bar_sf_full[i], 128);
+        for (int i = 0; i < 6; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 32 * kConsumerWarpsF); }
         fence_barrier_init();
     }
     if (warp == 0 && lane == 0)
         for (int i = 0; i < prm.n_segments; ++i) tma_prefetch_desc(&tmaps[i]);
-    if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
     // Early loads (see csrc/glm_tc.cu): the TMA warp claims the first chunk and fills the stage ring before
     // theta has arrived; theta has its own shared memory here, so every stage can be used.
     unsigned int claim0 = 0;
@@ -220,12 +168,9 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
             __syncwarp();
         }
     }
-    tc_fence_before();
 
     fed::Prologue pro = fed::prologue(comm, theta_f);   // contains __syncthreads()
     const bool active = !pro.stop && !pro.timed_out;
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     constexpr float kResidNorm = 1.f / 256.f;  // r = kResidNorm * sum_k t_k 16^-k, |r| <= 1
 
     const int nch = prm.n_chains < KF ? prm.n_chains : KF;
@@ -240,53 +185,30 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
 
     if (active) {
         for (size_t i = threadIdx.x; i < row_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
-        // ---- theta normalisation per chain: power of two c with max|beta| / c in [128, 256)
-        if (warp < KF) {
-            float m = 0.f;
-            if (warp < nch)
-                for (int f = lane; f < P; f += 32) m = fmaxf(m, fabsf(theta_f[warp * PG + G + f]));
-            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-            if (lane == 0) {
-                int e = 0;
-                if (m > 0.f) {
-                    frexpf(m, &e);      // m = frac * 2^e, frac in [0.5, 1)
-                    e -= 8;             // m / 2^(e-8) in [128, 256)
-                }
-                theta_norm[warp] = ldexpf(1.f, e);
-            }
-        }
-        __syncthreads();
-        float c_theta[KF];
-#pragma unroll
-        for (int k = 0; k < KF; ++k) c_theta[k] = theta_norm[k];
-        // ---- Theta^T as the K-major, 128B-swizzled e4m3 B operand: row n = 5 * chain + term
-        for (int idx = threadIdx.x; idx < NH * kN * 8; idx += blockDim.x) {
-            const int j = idx & 7;                 // 16-byte chunk = 16 features
-            const int n = (idx >> 3) % kN;
-            const int pnl = idx / (8 * kN);
-            const int chain = n / kThetaTerms, term = n % kThetaTerms;
+        // ---- Theta^T as the K-major, 128B-swizzled bf16 B operand of MMA #1: row n = 8 * term + chain
+        for (int idx = threadIdx.x; idx < (P / 64) * kN1 * 8; idx += blockDim.x) {
+            const int j = idx & 7;                 // 16-byte chunk = 8 features
+            const int n = (idx >> 3) % kN1;
+            const int pnl = idx / (8 * kN1);
+            const int chain = n % 8, term = n / 8;
             uint32_t packed[4] = {0, 0, 0, 0};
             if (chain < nch) {
-                const float inv_c = 1.f / theta_norm[chain];
 #pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                    uint8_t terms[kThetaTerms];
-                    expand16<kThetaTerms>(theta_f[chain * PG + G + pnl * kPanelF + j * 16 + e] * inv_c, terms);
-                    packed[e >> 2] |= (uint32_t)terms[term] << ((e & 3) * 8);
+                for (int e = 0; e < 8; ++e) {
+                    const float v = theta_f[chain * PG + G + pnl * 64 + j * 8 + e];
+                    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+                    const float rem1 = v - __bfloat162float(hi);
+                    const __nv_bfloat16 mid = __float2bfloat16_rn(rem1);
+                    const __nv_bfloat16 lo = __float2bfloat16_rn(rem1 - __bfloat162float(mid));
+                    const __nv_bfloat16 pick = term == 0 ? hi : (term == 1 ? mid : lo);
+                    packed[e >> 1] |= (uint32_t)__bfloat16_as_ushort(pick) << ((e & 1) * 16);
                 }
             }
-            *reinterpret_cast<uint4*>(theta_b + pnl * (kN * 128) + n * 128 + ((j ^ (n & 7)) * 16)) =
+            *reinterpret_cast<uint4*>(theta_b + pnl * (kN1 * 128) + n * 128 + ((j ^ (n & 7)) * 16)) =
                 make_uint4(packed[0], packed[1], packed[2], packed[3]);
         }
         fence_proxy_async();
         __syncthreads();
-        const uint32_t tmem_eta = tmem_base;                         // kEG x 16            (<= 64)
-        const uint32_t tmem_g = tmem_base + 64;                      // 2 buffers x NH x 16 (<= 64)
-        const uint32_t tmem_sfa1 = tmem_base + 128;                  // ring x 8 columns
-        const uint32_t tmem_sfa2 = tmem_sfa1 + kSfRing * 8;          // ring x 8 columns
-        const uint32_t tmem_sfb = tmem_sfa2 + kSfRing * 8;           // 4 columns of 2^0
-        const uint32_t tmem_sfb_r = tmem_sfb + 4;                    // DYN: kEG R buffers x 4 columns (col 0 used)
-        static_assert(128 + kSfRing * 16 + 4 + kEG * 4 <= (int)kTmemCols, "TMEM budget");
 
         // Consumers: the j-th chunk of this CTA, or x < 0 when the producer found the work counter exhausted.
         // (an mbarrier per ring slot: the producer arrives after writing the entry — release —, the consumers wait
@@ -296,10 +218,17 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
             if (*pipeline_fault()) return make_int4(-1, 0, 0, 0);   // a stalled pipeline ends every role loop
             return ring[j & (kRingF - 1)];
         };
-        // non-blocking variant for look-ahead: x == -2 when chunk j has not been published yet
-        auto peek_chunk = [&](int j) -> int4 {
-            if (!mbar_try_wait(&bar_ring[j & (kRingF - 1)], (uint32_t)((j / kRingF) & 1))) return make_int4(-2, 0, 0, 0);
-            return ring[j & (kRingF - 1)];
+        // Consumers decide each chunk together: both warpgroups meet at named barriers, so one of them leaving on
+        // a stalled pipeline while the other waits at a barrier would hang.  One thread reads the fault flag and
+        // the ring entry after all 256 have arrived and shares the decision through shared memory.
+        int4* chunk_decided = reinterpret_cast<int4*>(smem + L.off_bars + 128);
+        auto consumer_chunk = [&](int j) -> int4 {
+            const int slot = j & (kRingF - 1);
+            mbar_wait(&bar_ring[slot], (uint32_t)((j / kRingF) & 1));
+            named_sync(1, 256);
+            if (threadIdx.x == 128) *chunk_decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[slot];
+            named_sync(1, 256);
+            return *chunk_decided;
         };
 
         if (warp == 0) {
@@ -336,309 +265,263 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
                 }
                 claim = __shfl_sync(0xffffffffu, ahead, 0);
             }
-        } else if (warp == 1) {
-            {
-                constexpr uint32_t idesc1 = make_idesc_bs(128, kN, 0, 0);
-                // descriptors: constant fields once, the 14-bit (address >> 4) field added per MMA
-                const uint64_t desc_k = make_desc(0, 16, 1024, 2);
-                const uint32_t theta_b_a4 = smem_u32(theta_b) >> 4;
-                const uint32_t x_base_a4 = smem_u32(smem) >> 4;
-                const uint32_t stage_a4 = L.stage_bytes >> 4;
-                Ring stage, buf, sf;   // TMA stages (S), eta buffers (kEG), scale-word slots (kSfRing)
-                for (int j = 0;; ++j) {
-                  const int4 ch = next_chunk(j);
-                  if (ch.x < 0) break;
-                  for (int t = 0; t < ch.z; ++t) {
-                    mbar_wait(&bar_sf_full[sf.idx], sf.phase);
-                    mbar_wait(&bar_eta_empty[buf.idx], buf.phase ^ 1);
-                    mbar_wait(&bar_full[stage.idx], stage.phase);
-                    tc_fence_after();
-                    const uint32_t x_a4 = x_base_a4 + (uint32_t)stage.idx * stage_a4;
-                    const uint32_t d_eta = tmem_eta + buf.idx * kN;
-                    const uint32_t sfa = tmem_sfa1 + sf.idx * 8;
-                    if (elect_one()) {
-                        for (int pnl = 0; pnl < NH; ++pnl) {
+        } else if (warp >= 4) {
+            // ================= consumer warpgroups: rows 64c .. 64c + 63 (eta), features c P/2 .. (gradient)
+            const int c = (warp >> 2) - 1;
+            const int w = warp & 3;
+            const int q = lane & 3;
+            const int ew = warp - 4;                 // consumer warp ordinal: row of the per-warp slots
+            const int tid = threadIdx.x - 128 * (c + 1);
+            const int rg_me = 2 * c + (w >> 1);     // row group of this thread's two eta rows
+            const int NB = P / 128;                  // 64-feature gradient blocks per warpgroup (1 or 2)
+            const uint64_t desc_x = make_desc(0, 16, 1024, 1);      // bf16 X rows / Theta^T: K-major, 128B swizzle
+            const uint64_t desc_kn = make_desc(0, 128, 1024, 0);    // X^T copy and R: K-major, no swizzle
+            const uint32_t theta_b_a = smem_u32(theta_b);
+            const uint32_t x_base_a = smem_u32(smem);
+            const uint32_t r_a = smem_u32(r_buf);
+            unsigned char* xt = xt_buf + c * L.xt_bytes;
+            const uint32_t xt_a = smem_u32(xt);
+            unsigned char* xb = xb_buf + c * L.xb_bytes;
+            const uint32_t xb_a = smem_u32(xb);
+            float gacc[2][kN2 / 2];
 #pragma unroll
-                            for (int ks = 0; ks < 4; ++ks) {   // 4 K-steps of 32 features per 128-feature panel
-                                const uint64_t adesc = desc_k | (uint64_t)(x_a4 + ((pnl * kPanelB + ks * 32) >> 4));
-                                const uint64_t bdesc = desc_k | (uint64_t)(theta_b_a4 + ((pnl * (kN * 128) + ks * 32) >> 4));
-                                umma_fp8_block_scaled(d_eta, adesc, bdesc, idesc1 | ((uint32_t)ks << 29), (pnl | ks) ? 1u : 0u,
-                                                      sfa + pnl * 4, tmem_sfb);
-                            }
-                        }
-                        umma_commit(&bar_eta_full[buf.idx]);
-                    }
-                    __syncwarp();
-                    stage.advance(S);
-                    buf.advance(kEG);
-                    sf.advance(kSfRing);
-                  }
-                }
-            }
-        } else if (warp == 6) {
-            {
-                constexpr uint32_t idesc2 = make_idesc_bs(128, kN, 1, 1);
-                const uint64_t desc_x = make_desc(0, kPanelB, 1024, 2);
-                const uint64_t desc_r = make_desc(0, 128, 128, 0);
-                const uint32_t r_a4 = smem_u32(r_buf) >> 4;
-                const uint32_t x_base_a4 = smem_u32(smem) >> 4;
-                const uint32_t stage_a4 = L.stage_bytes >> 4;
-                Ring stage, buf, sf, gbuf;   // gbuf: TMEM gradient accumulator of the current chunk (2, alternating)
-                for (int j = 0;; ++j) {
-                  const int4 ch = next_chunk(j);
-                  if (ch.x < 0) break;
-                  const int gb = gbuf.idx;
-                  mbar_wait(&bar_g_empty[gb], gbuf.phase ^ 1);   // the epilogue has drained this accumulator
-                  for (int t = 0; t < ch.z; ++t) {
-                    const bool first = t == 0;
-                    const bool last = t == ch.z - 1;
-                    mbar_wait(&bar_r_full[buf.idx], buf.phase);
-                    tc_fence_after();
-                    const uint32_t x_a4 = x_base_a4 + (uint32_t)stage.idx * stage_a4;
-                    const uint32_t rb_a4 = r_a4 + (uint32_t)buf.idx * (L.r_bytes >> 4);
-                    const uint32_t sfa = tmem_sfa2 + sf.idx * 8;
-                    const uint32_t sfbr = DYN ? tmem_sfb_r + buf.idx * 4 : tmem_sfb;
-                    if (elect_one()) {
-                    for (int h = 0; h < NH; ++h) {
+            for (int i = 0; i < 2; ++i)
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) {   // K step = one 32-row group
-                            const uint64_t adesc = desc_x | (uint64_t)(x_a4 + ((h * kPanelB + q * 4 * 1024) >> 4));
-                            const uint64_t bdesc = desc_r | (uint64_t)(rb_a4 + ((q * 4 * 128) >> 4));
-                            // DYN: scale-factor-B byte q of the R buffer's column = exponent of row group q
-                            umma_fp8_block_scaled(tmem_g + (gb * NH + h) * kN, adesc, bdesc,
-                                                  idesc2 | ((uint32_t)q << 29) | (DYN ? ((uint32_t)q << 4) : 0u),
-                                                  (first && q == 0) ? 0u : 1u, sfa + h * 4, sfbr);
-                        }
-                    }
-                    umma_commit(&bar_empty[stage.idx]);
-                    umma_commit(&bar_r_empty[buf.idx]);
-                    if (last) umma_commit(&bar_g_full[gb]);
-                    }
-                    __syncwarp();
-                    stage.advance(S);
-                    buf.advance(kEG);
-                    sf.advance(kSfRing);
-                  }
-                  gbuf.advance(2);
-                }
-            }
-        } else {
-            // ================= epilogue warps: group g = warps 2..5 / 7..10 / 11..14 owns tiles t % kEG == g
-            // The per-tile epilogue is a long serial chain (barrier wake-up, TMEM load, link maths,
-            // smem store + proxy fence, TMEM scale stores).  kEG groups rotate over the tiles so that kEG
-            // chains overlap; group g owns eta/R buffer g, so every barrier still sees 128 arrivals.
-            // Measured (8 x 10M x 256): 1 group 269, 2 groups 279 -> 295 with host-packed scale words,
-            // 3 groups 297 evals/s — beyond two groups the group count is no longer the bound
-            // (prefetching y one iteration ahead did not move it either: 293).
-            const int eg = warp >= 7 ? (warp - 7) / 4 + 1 : 0;
-            const int q4 = warp & 3;
-            const int row = q4 * 32 + lane;
-            const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-            // scale-factor-B: 2^0 everywhere
-#pragma unroll
-            for (int cidx = 0; cidx < 4; ++cidx) tmem_st_x1(tmem_sfb + lane_addr + cidx, 0x7F7F7F7Fu);
-
-            // Scale words of a tile: loaded from global memory early (load_scales, results are not
-            // consumed until store_scales) so that the L2/HBM latency never sits on the per-tile chain.
-            auto load_scales = [&](int seg, int tile_in_seg, uint4 (&pk)[4]) {
-                // 16 words per tile, packed on the host in TMEM order (models/glm.py: pack_tile_scales):
-                //   words 0-7  (MMA #1): word 4g + q  = scales of (row group q, feature blocks 4g .. 4g+3)
-                //   words 8-15 (MMA #2): word 4h + qq = scales of (row groups 0..3, feature block 4h + qq)
-                const long long seg_tiles = (segs_g[seg].n_rows + kTile - 1) / kTile;
-                if (tile_in_seg < seg_tiles) {
-                    const uint4* sp = reinterpret_cast<const uint4*>(segs_g[seg].scales) + (size_t)tile_in_seg * 4;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) pk[i] = __ldg(sp + i);
-                } else {   // an empty tile that pads a chunk: 2^0 everywhere (its rows are all zero)
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) pk[i] = make_uint4(0x7F7F7F7Fu, 0x7F7F7F7Fu, 0x7F7F7F7Fu, 0x7F7F7F7Fu);
-                }
-            };
-            // writes the scale words of the CTA's t_it-th tile into ring slot t_it % kSfRing
-            auto store_scales = [&](int t_it, const uint4 (&pk)[4]) {
-                const uint32_t sfa1[8] = {pk[0].x, pk[0].y, pk[0].z, pk[0].w, pk[1].x, pk[1].y, pk[1].z, pk[1].w};
-                const uint32_t sfa2[8] = {pk[2].x, pk[2].y, pk[2].z, pk[2].w, pk[3].x, pk[3].y, pk[3].z, pk[3].w};
-                const int slot = t_it % kSfRing;
-                tmem_st_x8(tmem_sfa1 + lane_addr + slot * 8, sfa1);
-                tmem_st_x8(tmem_sfa2 + lane_addr + slot * 8, sfa2);
-                tmem_wait_st();
-                tc_fence_before();
-                mbar_arrive(&bar_sf_full[slot]);
-            };
-
-            const int ew = eg * 4 + q4;          // epilogue warp ordinal: row of the per-warp slots
-            const int b = eg;                    // eta / R buffer of this group
-            int it = 0;                          // tiles this CTA has been handed before the current chunk (multiple of kEG)
-            bool stored_ahead = false;           // the scales of this group's first tile of the chunk are already in TMEM
-            Ring gbuf;
+                for (int v = 0; v < kN2 / 2; ++v) gacc[i][v] = 0.f;
+            Ring stage;
+            uint32_t rb = 0;   // R buffer of the current tile (alternates)
             for (int j = 0;; ++j) {
-                const int4 ch = next_chunk(j);
+                const int4 ch = consumer_chunk(j);
                 if (ch.x < 0) break;
                 const float* __restrict__ seg_y = segs_g[ch.x].y;
                 const long long seg_rows = segs_g[ch.x].n_rows;
+                const long long seg_tiles = (seg_rows + kTile - 1) / kTile;
+                const uint8_t* __restrict__ seg_sc = reinterpret_cast<const uint8_t*>(segs_g[ch.x].scales);
                 const int seg_group = segs_g[ch.x].group;
                 const int og = segs_g[ch.x].out_group;   // output block of this chunk's segment
-                // this warp's (hi, lo) slots: LL at +0, intercept gradient g at +(1 + g); fetched a whole chunk early
-                double* slot0 = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KF) * NS1);
-                double2 pre_l[KF], pre_g[KF];
-                if (lane == 0) {
+                float ll_acc[2], gi_acc[2];
+                ll_acc[0] = ll_acc[1] = gi_acc[0] = gi_acc[1] = 0.f;
+                for (int t = 0; t < ch.z; ++t) {
+                    // block scales of this tile (an empty tile that pads a chunk: 2^0, its rows are zero)
+                    const long long tile = (long long)ch.y + t;
+                    const uint8_t* sc = seg_sc + (size_t)tile * 64 + 32;   // byte 4 fb + rg
+                    const bool real_tile = tile < seg_tiles;
+                    float s2[4][2];
 #pragma unroll
-                    for (int k = 0; k < KF; ++k)
-                        if (k < nch) {
-                            pre_l[k] = *reinterpret_cast<const double2*>(slot0 + 2 * (size_t)k * NS1);
-                            pre_g[k] = *reinterpret_cast<const double2*>(slot0 + 2 * (size_t)k * NS1 + 2 * (1 + seg_group));
-                        }
-                }
-                if (!stored_ahead) {
-                    uint4 first[4];
-                    load_scales(ch.x, ch.y + eg, first);
-                    store_scales(it + eg, first);
-                }
-                stored_ahead = false;
-                float ll_acc[KF], gi_cur[KF];
+                    for (int rg = 0; rg < 4; ++rg)
 #pragma unroll
-                for (int k = 0; k < KF; ++k) ll_acc[k] = gi_cur[k] = 0.f;
-                for (int t = eg; t < ch.z; t += kEG) {
-                    const int itl = it + t;
-                    const long long grow = ((long long)ch.y + t) * kTile + row;
-                    const bool valid = grow < seg_rows;
-                    const float y = valid ? __ldg(seg_y + grow) : 0.f;
-                    const uint32_t bph = (uint32_t)((itl / kEG) & 1);
-                    // scale words of this group's NEXT tile (consumed at the end of this iteration): the next tile
-                    // of the chunk, or the group's first tile of the next chunk if that chunk is already known
-                    uint4 next_scales[4];
-                    int next_it = -1;
-                    if (t + kEG < ch.z) {
-                        load_scales(ch.x, ch.y + t + kEG, next_scales);
-                        next_it = itl + kEG;
-                    } else {
-                        const int4 nx = peek_chunk(j + 1);
-                        if (nx.x >= 0) {
-                            load_scales(nx.x, nx.y + eg, next_scales);
-                            next_it = it + ch.z + eg;
-                            stored_ahead = true;
+                        for (int i = 0; i < 2; ++i) {
+                            const int fb = c * (P / 64) + 2 * i + (w >> 1);
+                            s2[rg][i] = (real_tile && i < NB) ? ue8m0(__ldg(sc + 4 * fb + rg)) : 1.f;
                         }
+                    mbar_wait(&bar_full[stage.idx], stage.phase);
+                    const uint32_t x_a = x_base_a + (uint32_t)stage.idx * L.stage_bytes;
+                    const unsigned char* xs = smem + (size_t)stage.idx * L.stage_bytes;
+                    // ---- dequantised bf16 copy of this group's 64 rows (64-feature panels of 64 rows x 128 bytes, 128B
+                    // swizzle): an e4m3 value times its power-of-two block scale is exact in bf16
+                    for (int b = tid; b < 64 * (P / 16); b += 128) {
+                        const int r = b / (P / 16);              // row within the group
+                        const int f = (b % (P / 16)) * 16;       // first of 16 features (one scale block)
+                        const int rr = 64 * c + r, fi = f & 127;
+                        const float bs = real_tile ? ue8m0(__ldg(sc + 4 * (f >> 5) + (rr >> 5))) : 1.f;
+                        const uint4 v = *reinterpret_cast<const uint4*>(xs + (f >> 7) * kPanelB + rr * 128 + (((fi >> 4) ^ (rr & 7)) << 4));
+                        const uint32_t wds[4] = {v.x, v.y, v.z, v.w};
+                        uint32_t o[8];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(wds[i] & 0xFFFFu), __NV_E4M3);
+                            const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(wds[i] >> 16), __NV_E4M3);
+                            const float2 a0 = __half22float2(*reinterpret_cast<const __half2*>(&lo));
+                            const float2 a1 = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                            const __nv_bfloat162 b0 = __floats2bfloat162_rn(a0.x * bs, a0.y * bs), b1 = __floats2bfloat162_rn(a1.x * bs, a1.y * bs);
+                            o[2 * i] = *reinterpret_cast<const uint32_t*>(&b0);
+                            o[2 * i + 1] = *reinterpret_cast<const uint32_t*>(&b1);
+                        }
+                        const int jb = (f & 63) >> 3;            // first of the two 8-feature chunks in the bf16 panel
+                        unsigned char* dst = xb + (f >> 6) * 8192 + r * 128;
+                        *reinterpret_cast<uint4*>(dst + ((jb ^ (r & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+                        *reinterpret_cast<uint4*>(dst + (((jb + 1) ^ (r & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
                     }
-
-                    mbar_wait(&bar_eta_full[b], bph);
-                    tc_fence_after();
-                    float v[16];
-                    tmem_ld_x16(tmem_eta + lane_addr + b * kN, v);
-                    tc_fence_before();
-                    mbar_arrive(&bar_eta_empty[b]);
-                    uint32_t rwords[4] = {0, 0, 0, 0};  // 16 residual bytes of this row: 4 terms per chain
-                    uint8_t* expo_slot = r_expo + (eg * 2 + (int)bph) * 12;
-#pragma unroll
-                    for (int k = 0; k < KF; ++k) {
-                        const float* vk = v + kThetaTerms * k;
-                        const float eta = c_theta[k] * (vk[0] + vk[1] * (1.f / 16) + vk[2] * (1.f / 256) + vk[3] * (1.f / 4096) +
-                                                        vk[4] * (1.f / 65536)) + theta_f[k * PG + seg_group];
-                        float ll = 0.f, r = 0.f;
-                        if (valid && k < nch) link_loglik(DYN ? prm.family : 0, y, eta, ll, r);
-                        ll_acc[k] += ll;
-                        gi_cur[k] += r;
-                        if constexpr (DYN) {
-                            // this 32-row group's scale: 2^e with max|r| / 2^e in [0.5, 1)
-                            float m = fabsf(r);
-#pragma unroll
-                            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                            int e = 0;
-                            if (m > 0.f) frexpf(m, &e);
-                            e = max(-126, min(126, e));
-                            r *= __uint_as_float((uint32_t)(127 - e) << 23);
-                            if (lane == 0) expo_slot[k * 4 + q4] = (uint8_t)(127 + e);
-                        }
-                        uint8_t rt[kResidTerms];
-                        expand16<kResidTerms>(r * 256.f, rt);
-                        rwords[k] = (uint32_t)rt[0] | ((uint32_t)rt[1] << 8) | ((uint32_t)rt[2] << 16) | ((uint32_t)rt[3] << 24);
-                    }
-                    mbar_wait(&bar_r_empty[b], bph ^ 1);
-                    *reinterpret_cast<uint4*>(r_buf + b * L.r_bytes + (row >> 3) * 128 + (row & 7) * 16) =
-                        make_uint4(rwords[0], rwords[1], rwords[2], rwords[3]);
                     fence_proxy_async();
+                    named_sync(2 + c, 128);
+                    // ---- MMA #1 on the dequantised rows: one uninterrupted chain of K steps
+                    float eacc[kN1 / 2];
+#pragma unroll
+                    for (int v = 0; v < kN1 / 2; ++v) eacc[v] = 0.f;
+                    wgmma_fence();
+                    for (int pnl = 0; pnl < P / 64; ++pnl) {
+#pragma unroll
+                        for (int ks = 0; ks < 4; ++ks)
+                            wgmma_bf16<kN1, 0, 0>(eacc, desc_x | (uint64_t)((xb_a + pnl * 8192 + ks * 32) >> 4),
+                                                  desc_x | (uint64_t)((theta_b_a + pnl * (kN1 * 128) + ks * 32) >> 4), (pnl | ks) ? 1u : 0u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(eacc);
+                    // ---- transposed copy of this group's feature half: element (feature fl, row r) at
+                    // (fl / 8) * 1024 + (r / 16) * 128 + (fl % 8) * 16 + r % 16; 4 x 4 byte blocks through registers
+                    for (int b = tid; b < (P / 8) * (kTile / 4); b += 128) {
+                        const int fl = (b % (P / 8)) * 4;        // first of 4 features (local to the half)
+                        const int r = (b / (P / 8)) * 4;         // first of 4 rows
+                        const int f = c * (P / 2) + fl;
+                        const int fi = f & 127;
+                        uint32_t a[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int rr = r + i;
+                            a[i] = *reinterpret_cast<const uint32_t*>(xs + (f >> 7) * kPanelB + rr * 128 +
+                                                                      ((((fi >> 4) ^ (rr & 7))) << 4) + (fi & 15));
+                        }
+                        const uint32_t t0 = __byte_perm(a[0], a[1], 0x5140), t1 = __byte_perm(a[2], a[3], 0x5140);
+                        const uint32_t t2 = __byte_perm(a[0], a[1], 0x7362), t3 = __byte_perm(a[2], a[3], 0x7362);
+                        const uint32_t o[4] = {__byte_perm(t0, t1, 0x5410), __byte_perm(t0, t1, 0x7632),
+                                               __byte_perm(t2, t3, 0x5410), __byte_perm(t2, t3, 0x7632)};
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int fr = fl + i;
+                            *reinterpret_cast<uint32_t*>(xt + (fr >> 3) * 1024 + (r >> 4) * 128 + (fr & 7) * 16 + (r & 15)) = o[i];
+                        }
+                    }
+                    // ---- link, likelihood, residual -> 4 e4m3 terms per chain in R (element (row, n) at
+                    // (n / 8) * 1024 + (row / 16) * 128 + (n % 8) * 16 + row % 16)
+                    float rr_[2][2];
+                    float yv[2];
+                    bool valid[2];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = 64 * c + 16 * w + (lane >> 2) + 8 * h;
+                        const long long grow = tile * kTile + row;
+                        valid[h] = grow < seg_rows;
+                        yv[h] = valid[h] ? __ldg(seg_y + grow) : 0.f;
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int k = 2 * q + e;
+                            const int kk = k < KF ? k : 0;
+                            const float eta = (eacc[2 * h + e] + eacc[4 + 2 * h + e]) + eacc[8 + 2 * h + e] + theta_f[kk * PG + seg_group];
+                            float ll = 0.f, r = 0.f;
+                            if (valid[h] && k < nch) link_loglik(DYN ? prm.family : 0, yv[h], eta, ll, r);
+                            ll_acc[e] += ll;
+                            gi_acc[e] += r;
+                            rr_[h][e] = r;
+                        }
+                    }
+                    float rsc[2] = {1.f, 1.f};   // DYN: 2^e of this row group, max|r| / 2^e in [0.5, 1)
                     if constexpr (DYN) {
-                        // all four row-group exponents of this tile -> one word per chain; B row n = 4 * chain + term
-                        // reads it from lane n of every subpartition
-                        if (eg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-                        else if (eg == 1) asm volatile("bar.sync 2, 128;" ::: "memory");
-                        else asm volatile("bar.sync 3, 128;" ::: "memory");
-                        const int chn = min(lane >> 2, KF - 1);
-                        const uint32_t w = *reinterpret_cast<const uint32_t*>(expo_slot + chn * 4);
-                        tmem_st_x1(tmem_sfb_r + lane_addr + b * 4, w);
-                        tmem_wait_st();
-                        tc_fence_before();
-                    }
-                    mbar_arrive(&bar_r_full[b]);
-
-                    // scales for this group's next tile: its ring slot was last used by the tile kSfRing before it,
-                    // whose MMAs are complete (we just passed r_empty of the previous own tile and eta_full of this one)
-                    if (next_it >= 0) store_scales(next_it, next_scales);
-                }
-                // ---- end of the chunk for this group: per-thread fp32 sums -> fixed butterfly over the warp
-                // (double) -> lane 0 adds the warp's value to its own (hi, lo) slot; all chunk-determined.  The slot
-                // values were fetched at the start of the chunk (`pre`), so no L2 round trip sits here.
-                double lsum[KF], gsum[KF];
 #pragma unroll
-                for (int k = 0; k < KF; ++k) {
-                    lsum[k] = (double)ll_acc[k];
-                    gsum[k] = (double)gi_cur[k];
+                        for (int e = 0; e < 2; ++e) {
+                            float m = fmaxf(fabsf(rr_[0][e]), fabsf(rr_[1][e]));
 #pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
-                        lsum[k] += __shfl_xor_sync(0xffffffffu, lsum[k], o);
-                        gsum[k] += __shfl_xor_sync(0xffffffffu, gsum[k], o);
-                    }
-                }
-                if (lane == 0) {
-#pragma unroll
-                    for (int k = 0; k < KF; ++k)
-                        if (k < nch) {
-                            double* slot = slot0 + 2 * (size_t)k * NS1;
-                            fed::dd_add(pre_l[k].x, pre_l[k].y, lsum[k], 0.0);
-                            fed::dd_add(pre_g[k].x, pre_g[k].y, gsum[k], 0.0);
-                            *reinterpret_cast<double2*>(slot) = pre_l[k];
-                            *reinterpret_cast<double2*>(slot + 2 * (1 + seg_group)) = pre_g[k];
+                            for (int o = 4; o < 32; o <<= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                            if (lane < 4) r_wmax[ew * 8 + 2 * q + e] = m;
                         }
-                }
-                // gradient: chunks hold a multiple of kEG tiles, so the last group always owns a chunk's last tile
-                if (eg == kEG - 1) {
-                    const int gb = gbuf.idx;
-                    mbar_wait(&bar_g_full[gb], gbuf.phase);
-                    tc_fence_after();
-                    for (int h = 0; h < NH; ++h) {
-                        float gv[16];
-                        tmem_ld_x16(tmem_g + lane_addr + (gb * NH + h) * kN, gv);
-                        if (h == NH - 1) {
-                            tc_fence_before();
-                            mbar_arrive(&bar_g_empty[gb]);
+                        named_sync(2 + c, 128);
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float m = fmaxf(r_wmax[(ew & ~1) * 8 + 2 * q + e], r_wmax[(ew | 1) * 8 + 2 * q + e]);
+                            int ex = 0;
+                            if (m > 0.f) frexpf(m, &ex);
+                            ex = max(-126, min(126, ex));
+                            rsc[e] = __uint_as_float((uint32_t)(127 + ex) << 23);
+                            if ((w & 1) == 0 && lane < 4) r_scale[(rb * 4 + rg_me) * 8 + 2 * q + e] = rsc[e];
+                        }
+                    }
+                    unsigned char* rbuf = r_buf + rb * L.r_bytes;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = 64 * c + 16 * w + (lane >> 2) + 8 * h;
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            uint8_t rt[kResidTerms];
+                            expand16<kResidTerms>(rr_[h][e] / rsc[e] * 256.f, rt);
+#pragma unroll
+                            for (int tt = 0; tt < kResidTerms; ++tt)
+                                rbuf[tt * 1024 + (row >> 4) * 128 + (2 * q + e) * 16 + (row & 15)] = rt[tt];
+                        }
+                    }
+                    fence_proxy_async();
+                    named_sync(1, 32 * kConsumerWarpsF);   // R (and the residual scales) of all 128 rows written
+                    // ---- MMA #2, one 32-row group per K step, scaled in registers
+#pragma unroll
+                    for (int rg = 0; rg < 4; ++rg) {
+                        float tmp[2][kN2 / 2];
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+#pragma unroll
+                            for (int v = 0; v < kN2 / 2; ++v) tmp[i][v] = 0.f;
+                        wgmma_fence();
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+                            if (i < NB)
+                                wgmma_e4m3<kN2>(tmp[i], desc_kn | (uint64_t)((xt_a + i * 8 * 1024 + rg * 256) >> 4),
+                                                desc_kn | (uint64_t)((r_a + rb * L.r_bytes + rg * 256) >> 4), 0u);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        float srg[2] = {1.f, 1.f};
+                        if constexpr (DYN) {
+                            srg[0] = r_scale[(rb * 4 + rg) * 8 + 2 * q];
+                            srg[1] = r_scale[(rb * 4 + rg) * 8 + 2 * q + 1];
                         }
 #pragma unroll
-                        for (int k = 0; k < KF; ++k)
-                            if (k < nch) {
-                                double* slot = out + 2 * (((size_t)og * nch + k) * NV1 + 1 + G + h * 128 + row);
-                                double2 cur = *reinterpret_cast<double2*>(slot);
-                                fed::dd_add(cur.x, cur.y,
-                                            (double)kResidNorm * ((double)gv[4 * k] + (double)gv[4 * k + 1] * (1.0 / 16) +
-                                                                  (double)gv[4 * k + 2] * (1.0 / 256) + (double)gv[4 * k + 3] * (1.0 / 4096)),
-                                            0.0);
-                                *reinterpret_cast<double2*>(slot) = cur;
+                        for (int i = 0; i < 2; ++i) {
+                            fence_regs(tmp[i]);
+                            if (i < NB)
+#pragma unroll
+                                for (int v = 0; v < kN2 / 2; ++v) gacc[i][v] = fmaf(s2[rg][i] * srg[v & 1], tmp[i][v], gacc[i][v]);
+                        }
+                    }
+                    mbar_arrive(&bar_empty[stage.idx]);   // this thread is done with the X stage
+                    stage.advance(S);
+                    rb ^= 1u;
+                }
+                // ---- end of the chunk: per-thread fp32 sums -> fixed butterfly over the 8 lanes that share the
+                // chains (double) -> lanes 0..3 add the warp's value to its own (hi, lo) slot; all chunk-determined
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    double lsum = (double)ll_acc[e], gsum = (double)gi_acc[e];
+#pragma unroll
+                    for (int o = 4; o < 32; o <<= 1) {
+                        lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
+                        gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
+                    }
+                    const int k = 2 * q + e;
+                    if (lane < 4 && k < nch) {
+                        double* slot = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KF + k) * NS1);
+                        dd_accumulate(slot, lsum);
+                        dd_accumulate(slot + 2 * (1 + seg_group), gsum);
+                    }
+                }
+                // gradient: feature f = c P/2 + 64 i + 16 w + lane / 4 + 8 h, chain k = 2q + e, terms in columns 8 t + k
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (i < NB) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int f = c * (P / 2) + 64 * i + 16 * w + (lane >> 2) + 8 * h;
+                                const int k = 2 * q + e;
+                                if (k < nch)
+                                    dd_accumulate(out + 2 * (((size_t)og * nch + k) * NV1 + 1 + G + f),
+                                                  (double)kResidNorm * ((double)gacc[i][2 * h + e] + (double)gacc[i][4 + 2 * h + e] * (1.0 / 16) +
+                                                                        (double)gacc[i][8 + 2 * h + e] * (1.0 / 256) +
+                                                                        (double)gacc[i][12 + 2 * h + e] * (1.0 / 4096)));
                             }
                     }
-                }
-                gbuf.advance(2);
-                it += ch.z;
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int v = 0; v < kN2 / 2; ++v) gacc[i][v] = 0.f;
             }
         }
 
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
         fed::pdl_trigger();   // the next evaluation's CTA may take this SM as soon as we exit
         // layout per chain: [LL, gi[G], g[P]] as (hi, lo) pairs; g[] was accumulated in place, LL and gi[] are the
         // per-warp slots summed in warp order
         for (int i = threadIdx.x; i < NOUT * nch * NS1; i += blockDim.x) {
             const int jv = i % NS1, k = (i / NS1) % nch, o = i / (NS1 * nch);
             double hi = 0.0, lo = 0.0;
-            for (int w = 0; w < kLLRowsF; ++w) {
+            for (int w = 0; w < kConsumerWarpsF; ++w) {
                 const double* slot = ll_slots + 2 * ((((size_t)w * NOUT + o) * KF + k) * NS1 + jv);
                 fed::dd_add(hi, lo, slot[0], slot[1]);
             }
@@ -650,7 +533,6 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
         for (int t = 0; t < preloaded; ++t) mbar_wait(&bar_full[t], 0u);
     }
     __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
     const bool fin = fed::epilogue_t<true>(comm, pro, (active && *pipeline_fault()) ? B200FED_ERR_PIPELINE : 0ull, row_doubles,
                                            comm.group_partials);
     if (fin && threadIdx.x == 0) *work_counter = 0u;   // every CTA has stopped claiming: ready for the next launch
@@ -677,9 +559,9 @@ EncodeTiledFn8 get_encode8() {
 
 extern "C" int b200_glm_fp8_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count,
                                     void** tmaps_dev, void** chunks_dev, int* n_chunks) {
-    if (prm->n_features != 128 && prm->n_features != 256) return -21;   // NFB <= 8 scale columns per tile
+    if (prm->n_features != 128 && prm->n_features != 256) return -21;   // <= 8 scale blocks per tile row
     for (int s = 0; s < n_segments; ++s)
-        if (segs_host[s].n_rows + fp8::kTile * fp8::kEG >= (1ll << 31)) return -22;   // row coordinates are 32-bit
+        if (segs_host[s].n_rows + fp8::kTile * fp8::kChunkMultiple >= (1ll << 31)) return -22;   // row coordinates are 32-bit
     if (prm->n_chains < 1 || prm->n_chains > 3 || prm->family < 0 || prm->family > 2) return -23;
     if (prm->ld % 16 != 0) return -24;
     EncodeTiledFn8 encode = get_encode8();
@@ -701,7 +583,7 @@ extern "C" int b200_glm_fp8_prepare(const GlmSegment* segs_host, int n_segments,
     if (e == cudaSuccess) e = cudaMemcpy(*tmaps_dev, host, sizeof(CUtensorMap) * n_segments, cudaMemcpyHostToDevice);
     delete[] host;
     if (e != cudaSuccess) return (int)e;
-    const std::vector<GlmChunk> chunks = build_chunks(segs_host, n_segments, sm_count > 0 ? sm_count : 148, fp8::kTile, fp8::kEG,
+    const std::vector<GlmChunk> chunks = build_chunks(segs_host, n_segments, sm_count > 0 ? sm_count : 132, fp8::kTile, fp8::kChunkMultiple,
                                                         fp8::kMaxChunkF, fp8::kMinChunkF);
     if (*chunks_dev) cudaFree(*chunks_dev);
     e = cudaMalloc(chunks_dev, sizeof(GlmChunk) * (chunks.size() + 1));

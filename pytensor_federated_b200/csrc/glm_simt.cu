@@ -10,9 +10,9 @@
 // A stock two-pass implementation (X @ beta, then X.T @ r) moves the matrix twice.
 //
 // This kernel evaluates one parameter vector per launch and is the numerics reference /
-// general-shape path; glm_tc.cu is the tcgen05 + TMA version that batches MCMC chains.
+// general-shape path; glm_tc.cu is the wgmma + TMA version that batches MCMC chains.
 // There is no GLM in the reference repository; the workload comes from
-// /root/repo/BASELINE.json ("federated logistic GLM, 10M rows x 256 features per shard").
+// BASELINE.json ("federated logistic GLM, 10M rows x 256 features per shard").
 #include <cuda_bf16.h>
 #include "fed_comm.cuh"
 #include "models.h"

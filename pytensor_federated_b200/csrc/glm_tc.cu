@@ -1,24 +1,25 @@
-// Federated GLM log-likelihood + gradient on the 5th-gen tensor cores (tcgen05 + TMEM + TMA).
+// Federated GLM log-likelihood + gradient on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // Per 128-row tile of the bf16 design matrix X (read from HBM exactly ONCE per evaluation):
 //
 //   TMA        X[128 x P] -> smem, 128B-swizzled 64-feature panels (cp.async.bulk.tensor)
-//   MMA #1     eta[128 x N1] = X_tile (A, K-major) . Theta^T (B, K-major)      -> TMEM
+//   MMA #1     eta[128 x N1] = X_tile (A, K-major) . Theta^T (B, K-major)      -> registers
 //              Theta holds, per MCMC chain, a 3-way bf16 split (hi, mid, lo) of the fp32
 //              coefficients, so eta keeps ~fp32 accuracy although the operands are bf16.
-//   epilogue   tcgen05.ld eta; link + log-likelihood; residual r = dll/deta;
+//   epilogue   link + log-likelihood; residual r = dll/deta;
 //              r is split into (hi, lo) bf16 and stored to smem as the B operand of MMA #2
 //   MMA #2     G[P x N2] += X_tile^T (A, **MN-major view of the very same smem tile**) . R
-//              accumulated in TMEM across tiles, flushed to fp64 registers every kFlush tiles
+//              accumulated in registers over the tiles of a chunk, then added to fp64 pairs
 //
 // so the gradient GEMM costs no second pass over X.  Chains are batched along N (the MMA is
 // otherwise idle: the kernel is HBM-bound), which is what makes tensor cores pay here.
-// Roles: warp 0 = TMA producer, warp 1 = MMA #1 issuer, warps 2-5 = epilogue, warp 6 = MMA #2
-// issuer (separate issuers so the gradient MMA of tile t never queues behind the TMA of tile t+1).
+// Roles: warp 0 = TMA producer; consumer warpgroups 1 and 2 (warps 4-11) share every tile: warpgroup c
+// computes eta / the residuals of rows 64c .. 64c + 63 and the gradient of features c P/2 .. (c + 1) P/2 - 1,
+// so every gradient value has one owner thread.  One 256-thread barrier per tile publishes R; the two R
+// buffers alternate, so a buffer is rewritten only after both warpgroups have passed the next tile's barrier.
 // The federation prologue/epilogue (theta broadcast, NVLink reduce) is fed_comm.cuh.
 //
 // Workload: BASELINE.json "federated logistic GLM, 10M rows x 256 features per shard, bf16".
-// Nothing comparable exists in the reference (its model is /root/reference/demo_node.py:31-43).
 #include <vector>
 
 #include <cuda.h>
@@ -32,22 +33,21 @@
 
 namespace tc {
 
-constexpr int kTileM = 128;          // rows per tile (UMMA M for MMA #1, UMMA K-extent for MMA #2)
+constexpr int kTileM = 128;          // rows per tile
 constexpr int kPanel = 64;           // features per 128-byte swizzle span
 constexpr int kPanelBytes = kTileM * 128;  // 16 KB
-// warps: 0 TMA, 1 MMA#1 issuer, 2-5 epilogue group 0, 6 MMA#2 issuer, 7.. further epilogue groups
-constexpr int kMaxChunk = 32;        // tiles per chunk at most (= tiles accumulated in TMEM in fp32 before a flush)
+constexpr int kThreads = 384;        // warpgroup 0: TMA producer (warp 0 only), warpgroups 1, 2: consumers
+constexpr int kConsumerWarps = 8;
+constexpr int kMaxChunk = 32;        // tiles per chunk at most (= tiles accumulated in fp32 registers before a flush)
 constexpr int kMinChunk = 4;
 constexpr int kRing = 16;            // published chunks the consumers may lag behind (needs only ~3)
-constexpr int kLLRows = 16;          // epilogue warps at most (per-warp log-likelihood slots)
+constexpr int kLLRows = 16;          // per-warp log-likelihood slot rows (>= kConsumerWarps)
 
 struct SmemLayout {
     uint32_t stages, stage_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_theta_f, off_icpt, off_ring,
-        off_bars, off_tmem, total, preload;
+        off_bars, total, preload;
 };
-// r_bufs: residual (R) buffers between the epilogue and MMA #2 — 2 normally; 1 for 16 chains, where the 8 KB
-// buy the third TMA stage (the epilogue of 16 chains is long enough to hide the short MMA #2 it then waits for)
-__host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_theta, int n_groups, int chains, int r_bufs) {
+__host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_theta, int n_groups, int chains) {
     SmemLayout L;
     const uint32_t panels = P / kPanel;
     L.stage_bytes = panels * kPanelBytes;
@@ -55,14 +55,14 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
     L.r_bytes = kTileM * n2 * 2;
     // theta (fp32) is staged inside the TMA stage ring and is dead once the bf16 B operand and the intercept
     // table are built, so it costs no shared memory of its own.
-    const uint32_t fixed = L.theta_b_bytes + r_bufs * L.r_bytes + ((chains * n_groups * 4 + 15) & ~15) + kRing * 24 + 192 +
-                           64 + 1024 /*alignment slack*/;
+    const uint32_t fixed = L.theta_b_bytes + 2 * L.r_bytes + ((chains * n_groups * 4 + 15) & ~15) + kRing * 24 + 192 +
+                           1024 /*alignment slack*/;
     uint32_t stages = (227u * 1024u - fixed) / L.stage_bytes;
     if (stages > 4) stages = 4;
     L.stages = stages;
     uint32_t o = stages * L.stage_bytes;
     L.off_theta_b = o; o += L.theta_b_bytes;
-    L.off_r = o; o += r_bufs * L.r_bytes;
+    L.off_r = o; o += 2 * L.r_bytes;
     // theta (fp32) sits in the LAST stage when it fits into one: the TMA warp fills the first stages - 1 stages
     // with this CTA's first tiles BEFORE theta has arrived (`preload`), the last stage is free once the B
     // operand is built.  (larger theta: stage 0 onwards, needs n_theta * 4 <= stages * stage_bytes, no preload)
@@ -72,27 +72,17 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
     L.off_icpt = o; o += (chains * n_groups * 4 + 15) & ~15;
     L.off_ring = o; o += kRing * 24;   // published chunks + one mbarrier per ring slot
     L.off_bars = o; o += 192;
-    L.off_tmem = o; o += 64;
     L.total = o + 1024;
     return L;
 }
 
-// KC = chains per launch.  N1 = pad16(3 KC) eta columns, N2 = pad16(2 KC) residual columns.
+// KC = chains per launch.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
-    static constexpr int N1 = ((3 * KC + 15) / 16) * 16;
-    static constexpr int N2 = ((2 * KC + 15) / 16) * 16;
-    // Epilogue warp groups (128 threads each).  The per-tile epilogue is a serial chain, so it is
-    // parallelised two ways: EGC groups split the chains of a tile (KC >= 4), and EGT = 2 groups
-    // ping-pong on alternate tiles so that two tiles' chains overlap.  Group g: chains of
-    // cg = g % EGC, tiles of parity tp = g / EGC.
-    static constexpr int EGC = KC >= 4 ? 2 : 1;
-    static constexpr int EGT = 2;
-    static constexpr int EG = EGC * EGT;
-    static constexpr int KH = KC / EGC;                 // chains per group
-    static constexpr int kArrive = 128 * EGC;           // arrivals per eta/R/G barrier phase
-    static constexpr int kThreads = 224 + (EG - 1) * 128;
-    static constexpr int RB = KC >= 16 ? 1 : 2;         // R buffers (see smem_layout)
+    static constexpr int C8 = KC <= 8 ? 8 : 16;           // chain columns per theta term
+    static constexpr int N1 = 3 * C8;                     // eta: term t of chain k in column t * C8 + k
+    static constexpr int N2 = ((2 * KC + 7) / 8) * 8;     // residual: (hi, lo) of chain k in columns 2k, 2k + 1
 };
 
 // doubles per CTA row of the partial array: (hi, lo) pairs of the n_vals outputs, then the per-warp slots of
@@ -102,33 +92,20 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
     return 2 * ((size_t)n_vals + (size_t)kLLRows * n_out * kc * (1 + n_groups));
 }
 
-// (hi, lo) += x on a pair that only this thread touches during the launch
-__device__ __forceinline__ void dd_accumulate(double* slot, double x) {
-    double2 cur = *reinterpret_cast<double2*>(slot);
-    fed::dd_add(cur.x, cur.y, x, 0.0);
-    *reinterpret_cast<double2*>(slot) = cur;
-}
-
 // Work is handed out in CHUNKS of consecutive tiles of one segment (host-built table: 32 tiles while much
 // work is left, shrinking to 4 towards the end; always an even number, a segment with an odd tile count
 // gets one empty tile).  The TMA warp claims chunks from a global counter and publishes them to the other
 // roles through a small shared-memory ring, so CTAs on faster SMs simply take more chunks: no CTA waits on
-// a statically assigned straggler.  Everything a chunk contributes (fp32 TMEM accumulation over its tiles,
+// a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
 template <int KC>
-__global__ void __launch_bounds__(Cfg<KC>::kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
+    constexpr int C8 = Cfg<KC>::C8;
     constexpr int N1 = Cfg<KC>::N1;
     constexpr int N2 = Cfg<KC>::N2;
-    constexpr int EG = Cfg<KC>::EG;
-    constexpr int KH = Cfg<KC>::KH;
-    constexpr int EGC = Cfg<KC>::EGC;
-    constexpr int kArrive = Cfg<KC>::kArrive;
-    constexpr int RB = Cfg<KC>::RB;
-    static_assert(Cfg<KC>::EGT == 2, "tile parity <-> eta / R buffer");
-    static_assert(EG * 4 <= kLLRows, "per-warp LL slots");
     extern __shared__ unsigned char smem_dyn[];
     // 1 KB alignment (128B-swizzled TMA tiles) by offsetting INSIDE the shared array: the pointer keeps its
     // shared address space, so the compiler emits LDS / STS instead of generic LD / ST for everything below
@@ -138,9 +115,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     const int PP = (P + 127) & ~127;  // features the tile is padded to: TMA zero-fills the columns past P, their
                                       // Theta rows are zero and their gradient rows are never stored
     const int G = prm.n_groups;
-    const int NH = PP / 128;          // 128-feature halves (UMMA M of MMA #2)
     const int panels = PP / kPanel;
-    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, G, KC, RB);
+    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, G, KC);
     const int S = (int)L.stages;
     const int nch = prm.n_chains < KC ? prm.n_chains : KC;  // chains actually present in theta
     const int NV1 = 1 + G + P;        // outputs per chain: [LL, gi[G], g[P]]
@@ -152,41 +128,22 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     int4* ring = reinterpret_cast<int4*>(smem + L.off_ring);          // (segment or -1, first row, tiles, -)
     uint64_t* bar_ring = reinterpret_cast<uint64_t*>(smem + L.off_ring + kRing * 16);   // slot j % kRing: chunk j published
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L.off_tmem);
-    uint64_t* bar_full = bars;            // [4]
-    uint64_t* bar_empty = bars + 4;       // [4]
-    uint64_t* bar_eta_full = bars + 8;    // [2]
-    uint64_t* bar_eta_empty = bars + 10;  // [2]
-    uint64_t* bar_r_full = bars + 12;     // [2]
-    uint64_t* bar_r_empty = bars + 14;    // [2]
-    uint64_t* bar_g_full = bars + 16;     // [2]
-    uint64_t* bar_g_empty = bars + 18;    // [2]
+    uint64_t* bar_full = bars;            // [4] X stage landed
+    uint64_t* bar_empty = bars + 4;       // [4] X stage consumed by both consumer warpgroups (bars + 128 B: chunk decision)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr uint32_t kTmemCols = (2 * N1 + 2 * 4 * N2) <= 128 ? 128 : ((2 * N1 + 2 * 4 * N2) <= 256 ? 256 : 512);
 
     // ---------------- theta-independent setup: runs BEFORE the dependency wait inside fed::prologue, i.e. it
     // overlaps with the tail of the previous evaluation when launched with programmatic stream serialization
-    for (int i = threadIdx.x; i < (int)(RB * L.r_bytes / 16); i += blockDim.x)
-        reinterpret_cast<uint4*>(r_buf)[i] = make_uint4(0, 0, 0, 0);
     if (threadIdx.x == 0) {
         *pipeline_fault() = 0;
         for (int i = 0; i < kRing; ++i) mbar_init(&bar_ring[i], 1);
-        for (int i = 0; i < 4; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&bar_eta_full[i], 1);
-            mbar_init(&bar_eta_empty[i], kArrive);
-            mbar_init(&bar_r_full[i], kArrive);
-            mbar_init(&bar_r_empty[i], 1);
-            mbar_init(&bar_g_full[i], 1);
-            mbar_init(&bar_g_empty[i], kArrive);
-        }
+        for (int i = 0; i < 4; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 32 * kConsumerWarps); }
         fence_barrier_init();
     }
     if (warp == 0 && lane == 0)
         for (int i = 0; i < prm.n_segments; ++i) tma_prefetch_desc(&tmaps[i]);
-    if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
     // Early loads: X does not depend on theta.  The TMA warp waits for the previous evaluation to retire (its
     // last CTA re-arms the work counter), claims this CTA's first chunk and fills all stages but the one theta
     // is staged in, so the tensor core has `preload` tiles waiting when theta arrives (peers see theta several
@@ -213,12 +170,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             __syncwarp();
         }
     }
-    tc_fence_before();
 
     fed::Prologue pro = fed::prologue(comm, theta_f);   // contains __syncthreads()
     const bool active = !pro.stop && !pro.timed_out;
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int NOUT = prm.n_out;       // output blocks (1 = everything summed; else one per node)
     const int NS1 = 1 + G;            // warp-level values per (block, chain): LL and the G intercept gradients
     const size_t row_doubles = partial_row_doubles(comm.n_vals, KC, NOUT, G);
@@ -230,12 +184,12 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (size_t i = threadIdx.x; i < row_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
             icpt[i] = (i / G) < nch ? theta_f[(i / G) * (G + P) + (i % G)] : 0.f;
-        // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = 3*chain + term
+        // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = term * C8 + chain
         for (int idx = threadIdx.x; idx < panels * N1 * 8; idx += blockDim.x) {
             const int j = idx & 7;              // 16-byte chunk (8 features) within the 128-byte row
             const int n = (idx >> 3) % N1;
             const int pnl = idx / (8 * N1);
-            const int chain = n / 3, term = n % 3;
+            const int chain = n % C8, term = n / C8;
             uint32_t packed[4] = {0, 0, 0, 0};
             if (chain < nch) {
 #pragma unroll
@@ -257,8 +211,6 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         fence_proxy_async();
         __syncthreads();
         if (threadIdx.x == 0) fed::stamp(comm, 2);
-        const uint32_t tmem_eta = tmem_base;                 // 2 buffers x N1 columns
-        const uint32_t tmem_g = tmem_base + 2 * N1;          // 2 buffers x NH x N2 columns
 
         // Consumers: the j-th chunk of this CTA, or x < 0 when the producer found the work counter exhausted.
         // (an mbarrier per ring slot: the producer arrives after writing the entry — release —, the consumers wait
@@ -267,6 +219,18 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             mbar_wait(&bar_ring[j & (kRing - 1)], (uint32_t)((j / kRing) & 1));
             if (*pipeline_fault()) return make_int4(-1, 0, 0, 0);   // a stalled pipeline ends every role loop
             return ring[j & (kRing - 1)];
+        };
+        // Consumers decide each chunk together: both warpgroups meet at named barriers, so one of them leaving on
+        // a stalled pipeline while the other waits at a barrier would hang.  One thread reads the fault flag and
+        // the ring entry after all 256 have arrived and shares the decision through shared memory.
+        int4* chunk_decided = reinterpret_cast<int4*>(smem + L.off_bars + 128);
+        auto consumer_chunk = [&](int j) -> int4 {
+            const int slot = j & (kRing - 1);
+            mbar_wait(&bar_ring[slot], (uint32_t)((j / kRing) & 1));
+            named_sync(1, 256);
+            if (threadIdx.x == 128) *chunk_decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[slot];
+            named_sync(1, 256);
+            return *chunk_decided;
         };
 
         if (warp == 0) {
@@ -307,264 +271,148 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 claim = __shfl_sync(0xffffffffu, ahead, 0);
             }
             if (lane == 0) fed::stamp(comm, 4);
-        } else if (warp == 1) {
-            // ================= MMA #1 issuer: eta = X . Theta^T ================================
-            constexpr uint32_t idesc1 = make_idesc(128, N1, 0, 0);
+        } else if (warp >= 4) {
+            // ================= consumer warpgroups ===============================================
+            const int c = (warp >> 2) - 1;          // rows 64c .. 64c + 63 of every tile, gradient features c PP/2 ..
+            const int w = warp & 3;                 // warp within the group: accumulator rows 16w .. 16w + 15
+            const int q = lane & 3;                 // column pair of the accumulator fragment
+            const int ew = warp - 4;                // consumer warp ordinal: LL slot row
+            const int NB = PP / 128;                // 64-feature gradient blocks per warpgroup (1..3)
+            constexpr int NJ = C8 / 8;              // this thread's chains: k = 8 jc + 2 q + e, jc < NJ, e < 2
             // descriptors: constant fields once, the 14-bit (address >> 4) field added per MMA
-            const uint64_t desc_k = make_desc(0, 16, 1024, 2);
-            const uint32_t theta_b_a4 = smem_u32(theta_b) >> 4;
-            const uint32_t x_base_a4 = smem_u32(smem) >> 4;
-            const uint32_t stage_a4 = L.stage_bytes >> 4;
-            Ring stage, buf;   // TMA stages (S), eta buffers (2)
-            for (int j = 0;; ++j) {
-                const int4 ch = next_chunk(j);
-                if (ch.x < 0) break;
-                for (int t = 0; t < ch.z; ++t) {
-                    mbar_wait(&bar_eta_empty[buf.idx], buf.phase ^ 1);
-                    mbar_wait(&bar_full[stage.idx], stage.phase);
-                    tc_fence_after();
-                    const uint32_t x_a4 = x_base_a4 + (uint32_t)stage.idx * stage_a4;
-                    const uint32_t d_eta = tmem_eta + buf.idx * N1;
-                    if (elect_one()) {
-                        for (int pnl = 0; pnl < panels; ++pnl) {
+            const uint64_t desc_k = make_desc(0, 16, 1024, 1);            // X / Theta^T: K-major, 128B swizzle
+            const uint64_t desc_xt = make_desc(0, kPanelBytes, 1024, 1);  // X^T: MN-major view of the X panels
+            const uint64_t desc_r = make_desc(0, 128, 2048, 0);           // R: K-major (rows contiguous), no swizzle
+            const uint32_t theta_b_a = smem_u32(theta_b);
+            const uint32_t x_base_a = smem_u32(smem);
+            const uint32_t r_a = smem_u32(r_buf);
+            float gacc[3][N2 / 2];
 #pragma unroll
-                            for (int ks = 0; ks < kPanel / 16; ++ks) {
-                                const uint64_t adesc = desc_k | (uint64_t)(x_a4 + ((pnl * kPanelBytes + ks * 32) >> 4));
-                                const uint64_t bdesc = desc_k | (uint64_t)(theta_b_a4 + ((pnl * (N1 * 128) + ks * 32) >> 4));
-                                umma_bf16(d_eta, adesc, bdesc, idesc1, (pnl | ks) ? 1u : 0u);
-                            }
-                        }
-                        umma_commit(&bar_eta_full[buf.idx]);
-                    }
-                    __syncwarp();
-                    stage.advance(S);
-                    buf.advance(2);
-                }
-            }
-        } else if (warp == 6) {
-            // ================= MMA #2 issuer: G += X^T . R ======================================
-            constexpr uint32_t idesc2 = make_idesc(128, N2, 1, 1);
-            constexpr uint32_t r_lbo = (N2 / 8) * 128;  // stride between 8-row K groups of R
-            // A = X^T: MN-major (features contiguous), 128B swizzle.
-            // LBO = stride between 64-feature panels, SBO = stride between 8-row groups.
-            const uint64_t desc_x = make_desc(0, kPanelBytes, 1024, 2);
-            // B = R: MN-major (chain columns contiguous), no swizzle.
-            // LBO = stride between 8-row K groups, SBO = stride between 8-column groups.
-            const uint64_t desc_r = make_desc(0, r_lbo, 128, 0);
-            const uint32_t r_a4 = smem_u32(r_buf) >> 4;
-            const uint32_t x_base_a4 = smem_u32(smem) >> 4;
-            const uint32_t stage_a4 = L.stage_bytes >> 4;
-            Ring stage, buf, gbuf;   // gbuf: TMEM gradient accumulator of the current chunk (2, alternating)
-            for (int j = 0;; ++j) {
-                const int4 ch = next_chunk(j);
-                if (ch.x < 0) break;
-                const int gb = gbuf.idx;
-                mbar_wait(&bar_g_empty[gb], gbuf.phase ^ 1);   // the epilogue has drained this accumulator
-                for (int t = 0; t < ch.z; ++t) {
-                    const bool last = t == ch.z - 1;
-                    mbar_wait(&bar_r_full[buf.idx], buf.phase);
-                    tc_fence_after();
-                    const uint32_t x_a4 = x_base_a4 + (uint32_t)stage.idx * stage_a4;
-                    const uint32_t rb_a4 = r_a4 + (uint32_t)buf.idx * (L.r_bytes >> 4);
-                    if (elect_one()) {
-                        for (int h = 0; h < NH; ++h) {
+            for (int i = 0; i < 3; ++i)
 #pragma unroll
-                            for (int ks = 0; ks < kTileM / 16; ++ks) {
-                                const uint64_t adesc = desc_x | (uint64_t)(x_a4 + (((2 * h) * kPanelBytes + ks * 2 * 1024) >> 4));
-                                const uint64_t bdesc = desc_r | (uint64_t)(rb_a4 + ((ks * 2 * r_lbo) >> 4));
-                                umma_bf16(tmem_g + (gb * NH + h) * N2, adesc, bdesc, idesc2, (t == 0 && ks == 0) ? 0u : 1u);
-                            }
-                        }
-                        umma_commit(&bar_empty[stage.idx]);   // X stage may be refilled
-                        // R may be rewritten.  Two buffers: one barrier per buffer.  One buffer: the tiles of
-                        // the two epilogue groups alternate in it, and each group waits for the OTHER group's
-                        // tile to be consumed — one barrier per tile parity, so that a group can never be two
-                        // phases ahead of the barrier it waits on (parity waits alias after two phases).
-                        umma_commit(&bar_r_empty[RB == 2 ? buf.idx : (t & 1)]);
-                        if (last) umma_commit(&bar_g_full[gb]);
-                    }
-                    __syncwarp();
-                    stage.advance(S);
-                    buf.advance(RB);
-                }
-                gbuf.advance(2);
-            }
-        } else {
-            // ================= epilogue warps: group 0 = warps 2-5, group g >= 1 = warps 7+4(g-1) .. =====
-            const int eg = warp <= 5 ? 0 : (warp - 7) / 4 + 1;
-            const int ew = eg * 4 + (warp <= 5 ? warp - 2 : (warp - 7) % 4);   // epilogue warp ordinal: LL slot row
-            const int cg = eg % EGC;                // which chains
-            const int tp = eg / EGC;                // which tile parity (chunks are even => also this group's eta/R buffer)
-            const int q = warp & 3;                 // TMEM lane quarter this warp may access
-            const int row = q * 32 + lane;          // row of the tile == TMEM lane
-            const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-            const int k0 = cg * KH;                 // first chain of this group
-            const uint32_t r_lbo = (N2 / 8) * 128;
-            // columns fetched per request (power-of-two shapes; the surplus columns are allocated TMEM, ignored)
-            constexpr int kEtaCols = KH == 1 ? 4 : (KH == 2 ? 8 : (KH == 4 ? 16 : 24));
-            constexpr int kGCols = KH <= 2 ? 4 : (KH == 4 ? 8 : 16);
-            constexpr bool kPrefetchSlots = KH <= 2;   // few enough registers to fetch the warp's slots a whole chunk early
-            const int b = tp;                       // eta / R buffer of this group's tiles
-            uint32_t bph = 0;                       // its phase: flips after every tile of this group
-            Ring gbuf;
+                for (int v = 0; v < N2 / 2; ++v) gacc[i][v] = 0.f;
+            Ring stage;
+            uint32_t rb = 0;                        // R buffer of the current tile (alternates)
             for (int j = 0;; ++j) {
-                const int4 ch = next_chunk(j);
+                const int4 ch = consumer_chunk(j);
                 if (ch.x < 0) break;
                 const float* __restrict__ seg_y = segs_g[ch.x].y;   // segment table: global, read once per chunk
                 const long long seg_rows = segs_g[ch.x].n_rows;
                 const int seg_group = segs_g[ch.x].group;
                 const int og = segs_g[ch.x].out_group;               // output block of this chunk's segment
-                // this warp's (hi, lo) slots of the chunk's output block: LL at +0, intercept gradient g at +(1 + g)
-                double* slot0 = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KC + k0) * NS1);
-                double2 pre_l[kPrefetchSlots ? KH : 1], pre_g[kPrefetchSlots ? KH : 1];
-                if constexpr (kPrefetchSlots) {
-                    if (lane == 0) {
+                float ll_acc[2 * NJ], gi_acc[2 * NJ];
 #pragma unroll
-                        for (int k = 0; k < KH; ++k)
-                            if ((k0 + k) < nch) {
-                                pre_l[k] = *reinterpret_cast<const double2*>(slot0 + 2 * (size_t)k * NS1);
-                                pre_g[k] = *reinterpret_cast<const double2*>(slot0 + 2 * (size_t)k * NS1 + 2 * (1 + seg_group));
-                            }
-                    }
-                }
-                float ll_acc[KH], gi_cur[KH];
+                for (int s = 0; s < 2 * NJ; ++s) ll_acc[s] = gi_acc[s] = 0.f;
+                for (int t = 0; t < ch.z; ++t) {
+                    mbar_wait(&bar_full[stage.idx], stage.phase);
+                    const uint32_t x_a = x_base_a + (uint32_t)stage.idx * L.stage_bytes;
+                    // ---- MMA #1: eta of this group's 64 rows
+                    float eacc[N1 / 2];
 #pragma unroll
-                for (int k = 0; k < KH; ++k) ll_acc[k] = gi_cur[k] = 0.f;
-                for (int t = tp; t < ch.z; t += 2) {
-                    const long long grow = (long long)ch.y + (long long)t * kTileM + row;
-                    const bool valid = grow < seg_rows;
-                    const float y = valid ? __ldg(seg_y + grow) : 0.f;
-
-                    mbar_wait(&bar_eta_full[b], bph);
-                    tc_fence_after();
-                    float ev[kEtaCols];
-                    tmem_ld_cols<kEtaCols>(tmem_eta + lane_addr + b * N1 + 3 * k0, ev);   // one TMEM round trip
-                    tc_fence_before();
-                    mbar_arrive(&bar_eta_empty[b]);
-
-                    // link, likelihood, residual -> (hi, lo) bf16 columns of R
-                    uint32_t rpk[KH];
+                    for (int v = 0; v < N1 / 2; ++v) eacc[v] = 0.f;
+                    wgmma_fence();
+                    for (int pnl = 0; pnl < panels; ++pnl) {
 #pragma unroll
-                    for (int k = 0; k < KH; ++k) {
-                        const float eta = (ev[3 * k] + ev[3 * k + 1]) + ev[3 * k + 2];
-                        float ll = 0.f, r = 0.f;
-                        if (valid && (k0 + k) < nch)
-                            link_loglik(prm.family, y, eta + icpt[(k0 + k) * G + seg_group], ll, r);
-                        ll_acc[k] += ll;
-                        gi_cur[k] += r;
-                        const __nv_bfloat16 hi = __float2bfloat16_rn(r);
-                        const __nv_bfloat16 lo = __float2bfloat16_rn(r - __bfloat162float(hi));
-                        rpk[k] = (uint32_t)__bfloat16_as_ushort(hi) | ((uint32_t)__bfloat16_as_ushort(lo) << 16);
-                    }
-                    // R buffer of this tile: with two buffers the group's own; with one, every tile of the CTA uses it
-                    const int rb = RB == 2 ? b : 0;
-                    if constexpr (RB == 2) {
-                        mbar_wait(&bar_r_empty[b], bph ^ 1);
-                    } else {
-                        // wait until MMA #2 has consumed the previous tile (the other group's): for group 0 that is
-                        // the (m)-th commit on the odd barrier before its m-th tile, for group 1 the (m+1)-th on the even
-                        mbar_wait(&bar_r_empty[tp ^ 1], tp == 0 ? (bph ^ 1) : bph);
-                    }
-                    {
-                        // chain k owns columns (2k, 2k+1): 4 bytes at (k / 4) * 128 + (k % 4) * 4 of the row
-                        unsigned char* rrow = r_buf + rb * L.r_bytes + (row >> 3) * r_lbo + (row & 7) * 16;
-                        if constexpr (KH == 8) {
-                            *reinterpret_cast<uint4*>(rrow + (k0 / 4) * 128) = make_uint4(rpk[0], rpk[1], rpk[2], rpk[3]);
-                            *reinterpret_cast<uint4*>(rrow + (k0 / 4 + 1) * 128) = make_uint4(rpk[4], rpk[5], rpk[6], rpk[7]);
-                        } else if constexpr (KH == 4) {
-                            *reinterpret_cast<uint4*>(rrow + (k0 / 4) * 128) = make_uint4(rpk[0], rpk[1], rpk[2], rpk[3]);
-                        } else if constexpr (KH == 2) {
-                            *reinterpret_cast<uint2*>(rrow + (k0 / 4) * 128 + (k0 % 4) * 4) = make_uint2(rpk[0], rpk[1]);
-                        } else {
-                            *reinterpret_cast<uint32_t*>(rrow + (k0 / 4) * 128 + (k0 % 4) * 4) = rpk[0];
+                        for (int ks = 0; ks < kPanel / 16; ++ks) {
+                            const uint64_t adesc = desc_k | (uint64_t)((x_a + pnl * kPanelBytes + c * 64 * 128 + ks * 32) >> 4);
+                            const uint64_t bdesc = desc_k | (uint64_t)((theta_b_a + pnl * (N1 * 128) + ks * 32) >> 4);
+                            wgmma_bf16<N1, 0, 0>(eacc, adesc, bdesc, (pnl | ks) ? 1u : 0u);
                         }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(eacc);
+                    // ---- link, likelihood, residual -> (hi, lo) bf16 columns of R (element (row, n) at
+                    // (n / 8) * 2048 + (row / 8) * 128 + (n % 8) * 16 + (row % 8) * 2)
+                    unsigned char* rbuf = r_buf + rb * L.r_bytes;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = 64 * c + 16 * w + (lane >> 2) + 8 * h;   // row of the tile
+                        const long long grow = (long long)ch.y + (long long)t * kTileM + row;
+                        const bool valid = grow < seg_rows;
+                        const float y = valid ? __ldg(seg_y + grow) : 0.f;
+#pragma unroll
+                        for (int jc = 0; jc < NJ; ++jc)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int k = 8 * jc + 2 * q + e;
+                                const float eta = (eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
+                                                  eacc[4 * (2 * NJ + jc) + 2 * h + e];
+                                float ll = 0.f, r = 0.f;
+                                if (valid && k < nch) link_loglik(prm.family, y, eta + icpt[k * G + seg_group], ll, r);
+                                ll_acc[2 * jc + e] += ll;
+                                gi_acc[2 * jc + e] += r;
+                                if (k < N2 / 2) {
+                                    const __nv_bfloat16 hi = __float2bfloat16_rn(r);
+                                    const __nv_bfloat16 lo = __float2bfloat16_rn(r - __bfloat162float(hi));
+                                    unsigned char* p0 = rbuf + ((2 * k) / 8) * 2048 + (row / 8) * 128 + (row % 8) * 2;
+                                    *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k) % 8) * 16) = hi;
+                                    *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k + 1) % 8) * 16) = lo;
+                                }
+                            }
                     }
                     fence_proxy_async();
-                    mbar_arrive(&bar_r_full[rb]);
-                    bph ^= 1u;
+                    named_sync(1, 32 * kConsumerWarps);   // R of all 128 rows written
+                    // ---- MMA #2: G[this group's features] += X^T . R over the 128 rows of the tile
+                    wgmma_fence();
+#pragma unroll
+                    for (int i = 0; i < 3; ++i)
+                        if (i < NB) {
+                            const uint32_t xa = x_a + (c * NB + i) * kPanelBytes;
+#pragma unroll
+                            for (int ks = 0; ks < kTileM / 16; ++ks) {
+                                const uint64_t adesc = desc_xt | (uint64_t)((xa + ks * 2048) >> 4);
+                                const uint64_t bdesc = desc_r | (uint64_t)((r_a + rb * L.r_bytes + ks * 256) >> 4);
+                                wgmma_bf16<N2, 1, 0>(gacc[i], adesc, bdesc, (t | ks) ? 1u : 0u);
+                            }
+                        }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int i = 0; i < 3; ++i) fence_regs(gacc[i]);
+                    mbar_arrive(&bar_empty[stage.idx]);   // this thread is done with the X stage
+                    stage.advance(S);
+                    rb ^= 1u;
                 }
-                // ---- end of the chunk for this group: fold its sums into the CTA's running pairs ----------
-                // per-thread fp32 sums over the chunk's tiles -> fixed butterfly over the warp (double) ->
-                // lane 0 adds the warp's value to its own slot: every step depends on the chunk only.
-                // The slots live in L2: all their loads are issued together (KH <= 2: already at the start of the
-                // chunk, see `pre`), so the chunk boundary costs one round trip at most, not 2 KH.
-                constexpr int kBatch = KH <= 4 ? KH : 4;   // chains whose slots are in flight together (register budget)
+                // ---- end of the chunk: fold its sums into the CTA's running pairs --------------------
+                // per-thread fp32 sums over the chunk's tiles -> fixed butterfly over the 8 lanes that share the
+                // chains (double) -> lanes 0..3 add the warp's value to its own slot: every step depends on the
+                // chunk only.
 #pragma unroll
-                for (int kb = 0; kb < KH; kb += kBatch) {
-                    double lsum[kBatch], gsum[kBatch];
+                for (int s = 0; s < 2 * NJ; ++s) {
+                    double lsum = (double)ll_acc[s], gsum = (double)gi_acc[s];
 #pragma unroll
-                    for (int k = 0; k < kBatch; ++k) {
-                        lsum[k] = (double)ll_acc[kb + k];
-                        gsum[k] = (double)gi_cur[kb + k];
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            lsum[k] += __shfl_xor_sync(0xffffffffu, lsum[k], o);
-                            gsum[k] += __shfl_xor_sync(0xffffffffu, gsum[k], o);
-                        }
+                    for (int o = 4; o < 32; o <<= 1) {
+                        lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
+                        gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
                     }
-                    if (lane == 0) {
-                        double2 cl[kBatch], cg[kBatch];
-#pragma unroll
-                        for (int k = 0; k < kBatch; ++k) {
-                            if constexpr (kPrefetchSlots) {
-                                cl[k] = pre_l[kb + k];
-                                cg[k] = pre_g[kb + k];
-                            } else if ((k0 + kb + k) < nch) {
-                                const double* slot = slot0 + 2 * (size_t)(kb + k) * NS1;
-                                cl[k] = *reinterpret_cast<const double2*>(slot);
-                                cg[k] = *reinterpret_cast<const double2*>(slot + 2 * (1 + seg_group));
-                            }
-                        }
-#pragma unroll
-                        for (int k = 0; k < kBatch; ++k)
-                            if ((k0 + kb + k) < nch) {
-                                double* slot = slot0 + 2 * (size_t)(kb + k) * NS1;
-                                fed::dd_add(cl[k].x, cl[k].y, lsum[k], 0.0);
-                                fed::dd_add(cg[k].x, cg[k].y, gsum[k], 0.0);
-                                *reinterpret_cast<double2*>(slot) = cl[k];
-                                *reinterpret_cast<double2*>(slot + 2 * (1 + seg_group)) = cg[k];
-                            }
+                    const int k = 8 * (s >> 1) + 2 * q + (s & 1);
+                    if (lane < 4 && k < nch) {
+                        double* slot = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KC + k) * NS1);
+                        dd_accumulate(slot, lsum);
+                        dd_accumulate(slot + 2 * (1 + seg_group), gsum);
                     }
                 }
-                // gradient: the group that handled the chunk's last tile (odd index) drains the TMEM accumulator
-                if (tp == 1) {
-                    const int gb = gbuf.idx;
-                    mbar_wait(&bar_g_full[gb], gbuf.phase);
-                    tc_fence_after();
-                    // one 128-feature half at a time keeps 16 values live instead of 64; the running pairs live in
-                    // this CTA's row of the partial array (L2): one thread owns each of them
+                // gradient: feature f = 64 (c NB + i) + 16 w + lane / 4 + 8 h, chain k = 4 jn + q, (hi, lo) adjacent
 #pragma unroll
-                    for (int h = 0; h < 4; ++h)
-                        if (h < NH) {
-                            float gv[kGCols];
-                            tmem_ld_cols<kGCols>(tmem_g + lane_addr + (gb * NH + h) * N2 + 2 * k0, gv);
-                            if (h == NH - 1) {
-                                tc_fence_before();
-                                mbar_arrive(&bar_g_empty[gb]);   // MMA #2 may start the chunk after next in this buffer
+                for (int i = 0; i < 3; ++i)
+                    if (i < NB) {
+#pragma unroll
+                        for (int jn = 0; jn < N2 / 8; ++jn)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int f = 64 * (c * NB + i) + 16 * w + (lane >> 2) + 8 * h;
+                                const int k = 4 * jn + q;
+                                if (k < nch && f < P)
+                                    dd_accumulate(out + 2 * (((size_t)og * nch + k) * NV1 + 1 + G + f),
+                                                  (double)gacc[i][4 * jn + 2 * h] + (double)gacc[i][4 * jn + 2 * h + 1]);
                             }
-                            const bool real = h * 128 + row < P;   // rows of the padding carry zeros: nothing to add
-                            double2 cur[KH];
-#pragma unroll
-                            for (int k = 0; k < KH; ++k)
-                                cur[k] = ((k0 + k) < nch && real)
-                                             ? *reinterpret_cast<const double2*>(out + 2 * (((size_t)og * nch + k0 + k) * NV1 + 1 + G + h * 128 + row))
-                                             : make_double2(0.0, 0.0);
-#pragma unroll
-                            for (int k = 0; k < KH; ++k) {
-                                fed::dd_add(cur[k].x, cur[k].y, (double)gv[2 * k] + (double)gv[2 * k + 1], 0.0);
-                                if ((k0 + k) < nch && real)
-                                    *reinterpret_cast<double2*>(out + 2 * (((size_t)og * nch + k0 + k) * NV1 + 1 + G + h * 128 + row)) = cur[k];
-                            }
-                        }
-                }
-                gbuf.advance(2);
+                    }
             }
         }
 
         // ---------------- CTA partial: fold the per-warp LL slots and the intercept gradients ----------
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
         fed::pdl_trigger();   // the next evaluation's CTA may take this SM as soon as we exit
         if (threadIdx.x == 0) fed::stamp(comm, 5);
         // layout per (output block, chain): [LL, gi[G], g[P]] as (hi, lo) pairs; g[] was accumulated in place,
@@ -572,7 +420,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (int i = threadIdx.x; i < NOUT * nch * NS1; i += blockDim.x) {
             const int j = i % NS1, k = (i / NS1) % nch, o = i / (NS1 * nch);
             double hi = 0.0, lo = 0.0;
-            for (int w = 0; w < EG * 4; ++w) {
+            for (int w = 0; w < kConsumerWarps; ++w) {
                 const double* slot = ll_slots + 2 * ((((size_t)w * NOUT + o) * KC + k) * NS1 + j);
                 fed::dd_add(hi, lo, slot[0], slot[1]);
             }
@@ -585,7 +433,6 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (int t = 0; t < preloaded; ++t) mbar_wait(&bar_full[t], 0u);
     }
     __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
     const unsigned long long status = *pipeline_fault() ? B200FED_ERR_PIPELINE : 0ull;
     const bool fin = fed::epilogue_t<true>(comm, pro, status, row_doubles, comm.group_partials);
     if (fin && threadIdx.x == 0) *work_counter = 0u;   // every CTA has stopped claiming: ready for the next launch
@@ -640,7 +487,7 @@ extern "C" int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, 
     if (e == cudaSuccess) e = cudaMemcpy(*tmaps_dev, host, sizeof(CUtensorMap) * n_segments, cudaMemcpyHostToDevice);
     delete[] host;
     if (e != cudaSuccess) return (int)e;
-    const std::vector<GlmChunk> chunks = build_chunks(segs_host, n_segments, sm_count > 0 ? sm_count : 148, tc::kTileM, 2,
+    const std::vector<GlmChunk> chunks = build_chunks(segs_host, n_segments, sm_count > 0 ? sm_count : 132, tc::kTileM, 2,
                                                         tc::kMaxChunk, tc::kMinChunk);
     if (*chunks_dev) cudaFree(*chunks_dev);
     e = cudaMalloc(chunks_dev, sizeof(GlmChunk) * (chunks.size() + 1));
@@ -678,12 +525,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
 #define LAUNCH_TC(KC)                                                                                              \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
-                                                 prm->n_groups, KC, tc::Cfg<KC>::RB);                              \
+                                                 prm->n_groups, KC);                                               \
         if (L.stages < 2) return -2;                                                                               \
         cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
-        cfg.blockDim = dim3(tc::Cfg<KC>::kThreads);                                                                \
+        cfg.blockDim = dim3(tc::kThreads);                                                                         \
         cfg.dynamicSmemBytes = L.total;                                                                            \
         cfg.stream = stream;                                                                                       \
         cudaLaunchAttribute attr[1];                                                                               \

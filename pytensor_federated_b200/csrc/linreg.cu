@@ -1,12 +1,12 @@
 // Federated Gaussian linear regression: per-shard  LL, dLL/d(intercept), dLL/d(slope).
 //
-// Maths of the reference's only shipped model (/root/reference/demo_node.py:31-43):
+// Maths of the reference's only shipped model (demo_node.py:31-43):
 //   pred = a + b*x ;  LL = sum log N(y | pred, sigma)
 //   dLL/da = sum (y-pred)/sigma^2 ;  dLL/db = sum (y-pred)*x/sigma^2
 // The reference evaluates this in a PyTensor-compiled CPU function behind gRPC; here it
 // is one fused broadcast->compute->reduce kernel (see fed_comm.cuh).  Each shard has its
 // own (intercept, slope) pair in theta so that hierarchical models
-// (/root/reference/demo_model.py:28-36: per-group intercepts, shared slope) evaluate all
+// (demo_model.py:28-36: per-group intercepts, shared slope) evaluate all
 // of their remote calls in ONE launch.  Everything is fp64: the reference returns float64
 // and its users compare against NumPy at ~1e-12.
 #include "fed_comm.cuh"

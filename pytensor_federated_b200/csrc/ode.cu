@@ -1,7 +1,7 @@
 // Federated ODE parameter estimation: [timepoints, theta] -> trajectories -> LL and dLL/dtheta.
 //
-// Workload named in /root/repo/BASELINE.json ("federated ODE parameter estimation ... 4 shards
-// on 4 GPUs"); the reference only describes it in prose (/root/reference/README.md:39-52: the
+// Workload named in BASELINE.json ("federated ODE parameter estimation ... 4 shards
+// on 4 GPUs"); the reference only describes it in prose (README.md:39-52: the
 // federated function is an ODE solve whose data never leaves the node).  Model: Lotka-Volterra
 //     u' = alpha u - beta u v ,  v' = delta u v - gamma v ,  theta = (alpha, beta, gamma, delta)
 // with forward sensitivities S = d(u,v)/dtheta integrated alongside (10 coupled ODEs), classic

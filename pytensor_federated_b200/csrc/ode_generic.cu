@@ -1,7 +1,7 @@
 // Federated ODE parameter estimation for a USER-SUPPLIED right-hand side.
 //
 // The reference's premise is that the federated function is arbitrary — its README describes "an ODE solve
-// whose data never leaves the node" (/root/reference/README.md:39-52).  csrc/ode.cu hard-codes one system
+// whose data never leaves the node" (README.md:39-52).  csrc/ode.cu hard-codes one system
 // (Lotka-Volterra with hand-written sensitivities); this file is the general case: the user writes ONLY the
 // right-hand side, once, as a snippet of CUDA C over a scalar type `T`
 //

@@ -15,7 +15,7 @@
 //        for the root's epoch flag, so a peer's host never sits on the critical path.
 //
 // The reference's counterpart of this file is its asyncio/gRPC client+server pair
-// (/root/reference/pytensor_federated/service.py:75-158, :326-423).
+// (pytensor_federated/service.py:75-158, :326-423).
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -89,7 +89,7 @@ CommLayout comm_layout(int world, int n_theta, int n_vals) {
 
 struct Engine {
     int device = 0, rank = 0, world = 1, n_theta = 0, n_vals = 0;
-    int grid = 1, sm_count = 148;
+    int grid = 1, sm_count = 132;
     cudaStream_t stream = nullptr;
     bool owns_comm = false;
     unsigned char* comm_local = nullptr;

@@ -1,5 +1,5 @@
-// tcgen05 / TMEM / TMA / mbarrier PTX wrappers and UMMA descriptor builders shared by the
-// tensor-core GLM kernels (glm_tc.cu: bf16, glm_fp8.cu: block-scaled fp8).  sm_100a only.
+// wgmma / TMA / mbarrier PTX wrappers and shared-memory descriptors shared by the tensor-core GLM
+// kernels (glm_tc.cu: bf16, glm_fp8.cu: block-scaled fp8).  sm_90a only.
 #pragma once
 #include <cstdlib>
 
@@ -71,9 +71,8 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// generic-proxy stores to shared memory -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
     asm volatile(
@@ -86,88 +85,95 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_out, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_out)), "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x4(uint32_t taddr, float (&v)[4]) {
-    uint32_t a, b, c, d;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(a), "=r"(b), "=r"(c), "=r"(d)
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    v[0] = __uint_as_float(a); v[1] = __uint_as_float(b); v[2] = __uint_as_float(c); v[3] = __uint_as_float(d);
-}
-// N consecutive fp32 columns of this warp's 32 TMEM lanes in ONE round trip: every tcgen05.ld of the request is
-// issued before the single tcgen05.wait::ld (issue + wait live in one asm statement, so the compiler cannot
-// touch the destination registers in between).  N in {4, 8, 16, 24, 32}.
+// Named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// ------------------------------------------------------------------ wgmma (sm_90a)
+// Warpgroup MMA: 128 threads (4 consecutive warps, the first a multiple of 4) issue together; the fp32
+// accumulator of an m64nN tile lives in registers, N / 2 per thread: d[4j + 2h + e] = (row 16 w + lane / 4 + 8 h,
+// column 8 j + 2 (lane % 4) + e) for warp w of the group.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, float (&v)[N]) {
-    static_assert(N == 4 || N == 8 || N == 16 || N == 24 || N == 32, "supported widths");
-    uint32_t r[N];
-    if constexpr (N == 4) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n\ttcgen05.wait::ld.sync.aligned;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
-    } else if constexpr (N == 8) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n\ttcgen05.wait::ld.sync.aligned;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr) : "memory");
-    } else if constexpr (N == 16) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\ttcgen05.wait::ld.sync.aligned;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(taddr) : "memory");
-    } else if constexpr (N == 24) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%24];\n\t"
-                     "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%16, %17, %18, %19, %20, %21, %22, %23}, [%25];\n\ttcgen05.wait::ld.sync.aligned;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]) : "r"(taddr), "r"(taddr + 16) : "memory");
-    } else {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\ttcgen05.wait::ld.sync.aligned;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]) : "r"(taddr) : "memory");
-    }
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accumulator reads / writes across wgmma issue and wait.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
 #pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, float (&v)[16]) { tmem_ld_cols<16>(taddr, v); }
+// bf16 x bf16 -> fp32, K = 16.  TA / TB: 0 = K-major, 1 = MN-major operand in shared memory.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    static_assert(N == 8 || N == 16 || N == 24 || N == 32 || N == 48, "instantiated widths");
+    if constexpr (N == 8) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+    } else if constexpr (N == 16) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+    } else if constexpr (N == 24) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, %12, %13, p, 1, 1, %15, %16;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+    } else if constexpr (N == 32) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+    } else if constexpr (N == 48) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+}
+
+// e4m3 x e4m3 -> fp32, K = 32 (both operands K-major: sm_90 has no transposed 8-bit operands).
+template <int N>
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    static_assert(N == 32 || N == 40, "instantiated widths");
+    if constexpr (N == 32) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d));
+    } else if constexpr (N == 40) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n40k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %20, %21, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+            : "l"(adesc), "l"(bdesc), "r"(scale_d));
+    }
+}
 
 // ------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor (sm_100): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout type [61,64) (0 = none/interleave, 2 = 128B swizzle).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+// Shared-memory matrix descriptor (sm_90): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
+// layout [62,64) (0 = no swizzle, 1 = 128B swizzle).  K-major: SBO = stride between 8-row groups along M / N,
+// LBO = stride between the two core matrices along K (no swizzle only).  MN-major 128B swizzle: LBO = stride
+// between 64-element spans along M / N, SBO = stride between 8-row groups along K.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle128) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout & 7) << 61;
+    d |= (uint64_t)(swizzle128 ? 1 : 0) << 62;
     return d;
 }
-// Instruction descriptor for kind::f16 with bf16 operands and fp32 accumulation.
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4)      // D format: f32
-           | (1u << 7)    // A format: bf16
-           | (1u << 10)   // B format: bf16
-           | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
-}
 
-// Programmatic dependent launch for back-to-back evaluations (B200FED_NO_PDL=1 disables it for A/B runs).
+// Programmatic dependent launch for back-to-back evaluations (B200FED_NO_PDL=1 disables it).
 inline bool use_pdl() {
     static const bool on = [] {
         const char* v = getenv("B200FED_NO_PDL");
@@ -188,6 +194,13 @@ struct Ring {
         }
     }
 };
+
+// (hi, lo) += x on a pair that only this thread touches during the launch
+__device__ __forceinline__ void dd_accumulate(double* slot, double x) {
+    double2 cur = *reinterpret_cast<double2*>(slot);
+    fed::dd_add(cur.x, cur.y, x, 0.0);
+    *reinterpret_cast<double2*>(slot) = cur;
+}
 
 __device__ __forceinline__ void link_loglik(int family, float y, float eta, float& ll, float& r) {
     if (family == 0) {

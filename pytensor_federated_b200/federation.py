@@ -2,7 +2,7 @@
 
 In the reference a *node* is a server process with a private dataset; a model that pools N nodes
 creates N clients/Ops and lets the graph add the log-potentials
-(``/root/reference/demo_model.py:17-36``, README "distributed" diagram).  Here the N nodes are the
+(``demo_model.py:17-36``, README "distributed" diagram).  Here the N nodes are the
 N data shards resident on the GPUs of one NVSwitch domain, and :class:`NodeFederation` gives each
 of them the reference's call signatures:
 
@@ -215,7 +215,7 @@ def register_replicas(engines: Sequence[FederatedEngine], host: str = "gpu", fir
     ``ArraysToArraysServiceClient(hosts_and_ports=...)`` / ``LogpGradServiceClient(hosts_and_ports=...)``.
 
     The client then behaves as it does towards replicated gRPC servers in the reference
-    (``/root/reference/pytensor_federated/service.py:239-275``, ``:407-416``): it connects to the replica with
+    (``pytensor_federated/service.py:239-275``, ``:407-416``): it connects to the replica with
     the fewest clients (chains of a sampler spread over the GPUs), and when a replica is lost — its engine shut
     down or timed out — the call is retried on a surviving one.  A *sharded* federation cannot do that (a lost
     shard is lost data); replicas trade HBM for availability and for chain-level parallelism."""

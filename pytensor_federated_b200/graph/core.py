@@ -1,9 +1,9 @@
 """A small symbolic graph IR with the slice of PyTensor's API that the federated Ops need.
 
-Why this exists: the reference's L4 layer (``/root/reference/pytensor_federated/op_async.py``,
+Why this exists: the reference's L4 layer (``pytensor_federated/op_async.py``,
 ``wrapper_ops.py``) is written against PyTensor (``Op``, ``Apply``, ``FunctionGraph``,
 ``optdb``, ``pytensor.grad``, ``DisconnectedType`` — list in SURVEY.md §2.5).  PyTensor is not
-available in the B200 image, so the same Op sources run on this IR when PyTensor is missing
+available in the offline image, so the same Op sources run on this IR when PyTensor is missing
 (see :mod:`pytensor_federated_b200._graph_backend`), which makes ``make_node`` / ``perform`` /
 ``grad`` / graph fusion executable and testable here, and gives the in-repo samplers
 (:mod:`pytensor_federated_b200.sampling`) a differentiable model language.

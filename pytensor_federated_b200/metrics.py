@@ -1,6 +1,6 @@
 """Optional Prometheus metrics of a serving node.
 
-The reference's only metric endpoint is the ``GetLoad`` RPC (``/root/reference/pytensor_federated/
+The reference's only metric endpoint is the ``GetLoad`` RPC (``pytensor_federated/
 service.py:88-96``).  A production node additionally wants scrapeable counters and latency histograms;
 ``ServiceMetrics`` wraps ``prometheus_client`` (when installed) behind a no-op fallback, so the service
 code never has to test for it:

@@ -1,4 +1,4 @@
-"""Model families with fused sm_100a kernels (and eager PyTorch oracles)."""
+"""Model families with fused sm_90a kernels (and eager PyTorch oracles)."""
 from .base import ShardModel
 from .custom import CustomFamily
 from .glm import Fp8GlmShards, GlmShards, dequantize_block_fp8, quantize_block_fp8, synth_logistic_shard, synth_logistic_shard_fp8

@@ -1,13 +1,13 @@
 """Contract between a model family and the federation engine.
 
-A *shard model* is the B200-native counterpart of the black-box ``compute_func`` that a
-reference node serves (``/root/reference/pytensor_federated/service.py:78-86``): it owns the
+A *shard model* is the GPU-native counterpart of the black-box ``compute_func`` that a
+reference node serves (``pytensor_federated/service.py:78-86``): it owns the
 node's private data (resident in HBM) and knows
 
 * how the client's input arrays are packed into the theta mailbox (32-bit words),
 * how the reduced ``[LL, dLL/dtheta ...]`` vector of doubles is unpacked into the flat
   ``(logp, *gradients)`` tuple of the ``wrap_logp_grad_func`` convention
-  (``/root/reference/pytensor_federated/common.py:26-49``),
+  (``pytensor_federated/common.py:26-49``),
 * how to attach itself to a native engine (which kernel, which launch shape), and
 * an eager PyTorch implementation of the same maths (numerics oracle for the kernels and the
   compute step of the NCCL/gloo baseline path).

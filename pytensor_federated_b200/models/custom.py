@@ -1,14 +1,14 @@
 """User-defined likelihoods on the fused path.
 
 The reference's premise is that a node serves an *arbitrary* function
-(``/root/reference/README.md:26-35``).  Arbitrary Python still goes through
+(``README.md:26-35``).  Arbitrary Python still goes through
 ``ArraysToArraysService`` / ``register_local_node``; but any GLM-shaped model
 ``eta = intercept[group] + X beta`` with a custom per-observation log-likelihood can run inside the
 fused broadcast -> compute -> reduce kernel: the likelihood is a snippet of CUDA C that assigns
 
     ll  — log-likelihood of one observation,   r  — d ll / d eta
 
-from ``y`` and ``eta`` (floats).  It is compiled for sm_100a into its own shared object (nvcc, cached
+from ``y`` and ``eta`` (floats).  It is compiled for sm_90a into its own shared object (nvcc, cached
 by content hash under ``csrc/build/custom``) and plugged into the general-shape kernel
 (``csrc/glm_generic.cu``).  Example — Student-t regression with 4 degrees of freedom::
 

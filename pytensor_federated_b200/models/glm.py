@@ -1,6 +1,6 @@
 """Generalised linear model shards with a low-precision, HBM-resident design matrix.
 
-Workloads from ``/root/repo/BASELINE.json`` (not present in the reference, whose only model is
+Workloads from ``BASELINE.json`` (not present in the reference, whose only model is
 the 10-point linear regression): *federated logistic GLM, 10M rows x 256 features per shard,
 bf16 design matrix* and *hierarchical GLM, 8 partial-pooling groups, fp8 block-scaled design
 matrix*.  ``theta = [intercept[G], beta[P]]`` (float32) per chain; a segment (shard) uses
@@ -38,7 +38,7 @@ class GlmShards(ShardModel):
     n_chains
         Parameter vectors evaluated per call (K).  ``K > 1`` needs the tensor-core kernel.
     kernel
-        ``"simt"`` (one chain, any P % 8 == 0 up to 512), ``"tc"`` (tcgen05 + TMA: bf16, any P % 8 == 0 up to
+        ``"simt"`` (one chain, any P % 8 == 0 up to 512), ``"tc"`` (wgmma + TMA: bf16, any P % 8 == 0 up to
         384 — the tile is padded to whole 128-feature blocks by TMA's zero fill —, up to 16 chains) or ``"auto"``.
     node_ids, n_nodes
         Keep the result PER NODE instead of summed: segment ``s`` is (part of) node ``node_ids[s]`` of
@@ -46,7 +46,7 @@ class GlmShards(ShardModel):
         (every kernel: the tensor-core kernels route a chunk's sums to its node's block, the CUDA-core kernels flush
         at node boundaries into fixed-point accumulators).  ``evaluate`` still returns the sum; :meth:`per_node` and
         :class:`~pytensor_federated_b200.federation.NodeFederation` expose the blocks — the reference's
-        one-Op-per-node pattern (``/root/reference/demo_model.py:28-36``) answered by one launch.
+        one-Op-per-node pattern (``demo_model.py:28-36``) answered by one launch.
     """
 
     def __init__(
@@ -147,7 +147,7 @@ class GlmShards(ShardModel):
 
     # -- native ----------------------------------------------------------------------------
     def use_tensor_cores(self):
-        """Kernel selector passed to the runtime: 0 = SIMT, 1 = tcgen05 (bf16), 2 = block-scaled fp8,
+        """Kernel selector passed to the runtime: 0 = SIMT, 1 = tensor cores (bf16), 2 = block-scaled fp8,
         3 / 4 = general-shape fallback (bf16 / fp32 design matrix)."""
         import torch
 
@@ -167,7 +167,7 @@ class GlmShards(ShardModel):
             if generic is None:
                 raise ValueError("the general-shape kernel needs a bf16 or fp32 design matrix")
             return generic
-        # auto: the tcgen05 kernel wherever its shape constraints hold (it is faster even for one chain:
+        # auto: the tensor-core kernel wherever its shape constraints hold (it is faster even for one chain:
         # TMA streaming + the X tile reused from smem for both GEMMs), then SIMT, then the general kernel
         bf16 = X0.dtype == torch.bfloat16
         tc_ok = (bf16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384 and self.n_chains <= 16
@@ -196,7 +196,7 @@ class GlmShards(ShardModel):
         rows = (C.c_longlong * n)(*[X.shape[0] for X in self.Xs])
         grp = (C.c_int * n)(*self.groups)
         code = int(self.use_tensor_cores())
-        #: which fused kernel serves this model ("tc" / "fp8" = tcgen05 tensor cores, else CUDA cores)
+        #: which fused kernel serves this model ("tc" / "fp8" = wgmma tensor cores, else CUDA cores)
         self.selected_kernel = {0: "simt", 1: "tc", 2: "fp8", 3: "generic-bf16", 4: "generic-fp32"}[code]
         if self.kernel == "auto" and code not in (1, 2) and not hasattr(self.family, "code_id"):
             import logging
@@ -345,10 +345,11 @@ def dequantize_block_fp8(Xq, scales, block: int = 32):
 
 
 def pack_tile_scales(scales, n_features: int):
-    """Re-orders the UE8M0 block scales ``[4 * tiles, P / 32]`` into the 16 words per 128-row tile that
-    ``csrc/glm_fp8.cu`` copies into the TMEM scale-factor columns: words 0-7 for ``eta = X . Theta^T``
-    (word ``4g + q`` = row group ``q``, feature blocks ``4g..4g+3``), words 8-15 for ``G += X^T . R``
-    (word ``4h + qq`` = row groups 0..3 of feature block ``4h + qq``).  Returns ``uint8 [tiles, 64]``."""
+    """Re-orders the UE8M0 block scales ``[4 * tiles, P / 32]`` into 16 words per 128-row tile: words 0-7
+    feature-block-major per row group (word ``4g + q`` = row group ``q``, feature blocks ``4g..4g+3``),
+    words 8-15 row-group-major per feature block (word ``4h + qq`` = row groups 0..3 of feature block
+    ``4h + qq``).  ``csrc/glm_fp8.cu`` reads words 8-15: byte ``32 + 4 fb + q`` is the scale of (row group
+    ``q``, feature block ``fb``) of the tile, one 32-byte line per tile.  Returns ``uint8 [tiles, 64]``."""
     import torch
 
     nfb = n_features // 32
@@ -367,9 +368,9 @@ class Fp8GlmShards(GlmShards):
 
     The hierarchical-GLM configuration of BASELINE.json: one partial-pooling group (intercept) per
     shard/GPU, e4m3 design matrix with 32 x 32 UE8M0 block scales, evaluated by ``csrc/glm_fp8.cu``
-    (``tcgen05.mma.kind::mxf8f6f4.block_scale``).  Up to 3 chains per launch.  The residuals of the
-    Poisson and Gaussian families are unbounded, so the kernel block-scales them too (one UE8M0
-    exponent per 32-row group, written to the MMA's scale-factor-B columns).
+    (e4m3 wgmma, block scales applied in fp32 registers per 32-deep K step).  Up to 3 chains per launch.
+    The residuals of the Poisson and Gaussian families are unbounded, so the kernel scales them too (one
+    power of two per 32-row group and chain).
     """
 
     def __init__(self, Xqs, scales, ys, *, groups=None, n_groups: int = 1, n_chains: int = 1,

@@ -1,10 +1,10 @@
 """Gaussian linear regression shards — the reference's demo model, GPU-resident.
 
-Maths: ``/root/reference/demo_node.py:31-43`` (``LinearModelBlackbox``); data synthesis for the
-demo: ``/root/reference/demo_node.py:59-61``.  One :class:`LinregShards` object holds the shards
+Maths: ``demo_node.py:31-43`` (``LinearModelBlackbox``); data synthesis for the
+demo: ``demo_node.py:59-61``.  One :class:`LinregShards` object holds the shards
 that live on ONE GPU; ``theta`` is ``[(intercept_s, slope_s) for s in all shards of the
 federation]`` so that a hierarchical model with per-group intercepts
-(``/root/reference/demo_model.py:28-36``) is evaluated in one fused launch, and the result
+(``demo_model.py:28-36``) is evaluated in one fused launch, and the result
 keeps per-shard ``[LL, dLL/da, dLL/db]`` so the client graph can weight/sum them itself.
 """
 from __future__ import annotations

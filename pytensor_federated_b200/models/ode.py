@@ -1,8 +1,8 @@
 """ODE parameter-estimation shards (RK4 with forward sensitivities).
 
-Workload from ``/root/repo/BASELINE.json`` ("federated ODE parameter estimation
+Workload from ``BASELINE.json`` ("federated ODE parameter estimation
 ([timepoints, theta] -> trajectory -> LL), 4 shards on 4 GPUs"); the reference describes the
-use-case only in prose (``/root/reference/README.md:39-52``).  Every series has its own known
+use-case only in prose (``README.md:39-52``).  Every series has its own known
 initial state; Gaussian observation noise on every state.
 
 The default system is Lotka–Volterra, ``theta = (alpha, beta, gamma, delta)``, with hand-written
@@ -74,7 +74,7 @@ class OdeSystem:
         return h.hexdigest()[:16]
 
     def compile(self) -> C.CDLL:
-        """Builds (or loads from the cache) the shared object of this system for sm_100a."""
+        """Builds (or loads from the cache) the shared object of this system for sm_90a."""
         if self._lib is not None:
             return self._lib
         from .. import build as native_build
@@ -111,7 +111,7 @@ class OdeShards(ShardModel):
     them (RK4 with forward sensitivities) and returns the Gaussian log-likelihood and its gradient w.r.t.
     ``theta``.  ``system=None`` is Lotka–Volterra (``csrc/ode.cu``, ``theta = (alpha, beta, gamma,
     delta)``); any :class:`OdeSystem` runs through ``csrc/ode_generic.cu``.  The reference only describes this
-    workload in prose (``/root/reference/README.md:39-52``)."""
+    workload in prose (``README.md:39-52``)."""
 
     def __init__(self, ts: Sequence, y0s: Sequence, y_obs: Sequence, sigmas: Sequence[float], substeps: int = 8,
                  system: Optional[OdeSystem] = None, node_ids: Optional[Sequence[int]] = None,

@@ -1,9 +1,9 @@
 """``npproto.ndarray`` message (wire-compatible with the reference).
 
-Schema: ``/root/reference/protobufs/npproto/ndarray.proto:7-12`` —
+Schema: ``protobufs/npproto/ndarray.proto:7-12`` —
 ``bytes data=1; string dtype=2; repeated int64 shape=3; repeated int64 strides=4``.
 The reference's class is betterproto-generated
-(``/root/reference/pytensor_federated/npproto/__init__.py:12-22``); this one is
+(``pytensor_federated/npproto/__init__.py:12-22``); this one is
 hand-written on top of :mod:`pytensor_federated_b200._pb` and keeps the two
 methods the reference's users touch: ``bytes(msg)`` and ``Msg().parse(data)``.
 """

@@ -1,6 +1,6 @@
 """Converters between ``numpy.ndarray``/``torch.Tensor`` and :class:`Ndarray`.
 
-Reference: ``/root/reference/pytensor_federated/npproto/utils.py:9-24``.
+Reference: ``pytensor_federated/npproto/utils.py:9-24``.
 
 Differences on purpose (SURVEY.md §2.1):
 

@@ -1,6 +1,6 @@
 """Asynchronous Ops and the graph rewrite that runs independent ones concurrently.
 
-Capabilities of ``/root/reference/pytensor_federated/op_async.py``:
+Capabilities of ``pytensor_federated/op_async.py``:
 
 * ``AsyncOp`` — an Op whose computation is a coroutine (``perform_async``); the synchronous
   ``perform`` drives it on a re-entrant event loop (``:16-34``).
@@ -221,7 +221,7 @@ def find_parallelizable_applies(fg: FunctionGraph, op_cls: type) -> List[Apply]:
     rank with at least two members is returned, in topological order.  Calling this repeatedly
     while fusing (see :func:`parallelize_all_async_applies`) therefore works through a dependency
     chain level by level, like the reference's greedy scan
-    (``/root/reference/pytensor_federated/op_async.py:135-167``), but it also pairs up independent
+    (``pytensor_federated/op_async.py:135-167``), but it also pairs up independent
     nodes that a dependent node separates in the topological order.
     """
     by_rank: dict = {}

@@ -1,4 +1,4 @@
-"""Native operators: ctypes access to the sm_100a kernels and the host runtime."""
+"""Native operators: ctypes access to the sm_90a kernels and the host runtime."""
 from . import native
 
 __all__ = ["native"]

@@ -1,4 +1,4 @@
-"""ctypes binding of ``libb200fed.so`` (the sm_100a kernels + host runtime).
+"""ctypes binding of ``libb200fed.so`` (the sm_90a kernels + host runtime).
 
 The library is built in-tree by :mod:`pytensor_federated_b200.build`.  On a machine with a
 GPU a missing/unloadable library is a hard error — there is no silent PyTorch fallback for

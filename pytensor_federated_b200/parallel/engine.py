@@ -3,7 +3,7 @@
 Two interchangeable data planes behind one interface:
 
 ``backend="fused"`` (the product)
-    One hand-written sm_100a kernel per GPU does broadcast -> compute -> reduce with in-kernel
+    One hand-written sm_90a kernel per GPU does broadcast -> compute -> reduce with in-kernel
     NVLink stores/multicast (``csrc/fed_comm.cuh``).  The root's host thread only memcpy's theta
     into pinned memory, launches, and spins on a pinned completion flag; peer hosts pre-enqueue
     kernels that wait on the device.  No NCCL call, no serialisation, no RPC on the path.
@@ -14,7 +14,7 @@ Two interchangeable data planes behind one interface:
     it doubles as the oracle in multi-process tests and runs on CPU with gloo.
 
 The reference's equivalent of one ``evaluate`` call is N concurrent gRPC round trips plus a
-client-side sum (``/root/reference/pytensor_federated/op_async.py:114-130``,
+client-side sum (``pytensor_federated/op_async.py:114-130``,
 ``service.py:150-158``).
 """
 from __future__ import annotations

@@ -1,8 +1,8 @@
 """Runtime-built protobuf descriptors of the wire schema.
 
 The reference generates Python classes from ``protobufs/*.proto`` with ``protoc``
-(``/root/reference/protobufs/generate.py:15-27``).  ``protoc`` is not part of the
-B200 image, so the same schema is assembled as a ``FileDescriptorProto`` here.
+(``protobufs/generate.py:15-27``).  ``protoc`` is not part of the
+offline image, so the same schema is assembled as a ``FileDescriptorProto`` here.
 It serves two purposes: (1) an independent oracle for the hand-written codec in
 :mod:`pytensor_federated_b200._pb` (see ``tests/test_npproto.py``) and (2)
 stock ``google.protobuf`` message classes for users who want them, e.g. to talk

@@ -1,9 +1,9 @@
 """Service messages, async client stub and server base of ``ArraysToArraysService``.
 
-Schema: ``/root/reference/protobufs/service.proto:6-41``.  The reference's module
+Schema: ``protobufs/service.proto:6-41``.  The reference's module
 of the same role is betterproto/grpclib-generated
-(``/root/reference/pytensor_federated/rpc.py:31-187``).  This one is hand-written
-against ``grpc.aio`` (the gRPC stack that ships in the B200 image) and is used
+(``pytensor_federated/rpc.py:31-187``).  This one is hand-written
+against ``grpc.aio`` (the gRPC stack that ships in the offline image) and is used
 for the *compatibility* data path only (off-box clients, arbitrary Python
 compute functions).  On-box GPU nodes are reached through the fused NVLink path
 in :mod:`pytensor_federated_b200.parallel` and never touch this module.
@@ -240,7 +240,7 @@ def _serialize(message) -> bytes:
 class ArraysToArraysServiceStub:
     """Async client stub over a ``grpc.aio`` channel.
 
-    Counterpart of ``/root/reference/pytensor_federated/rpc.py:74-126``.
+    Counterpart of ``pytensor_federated/rpc.py:74-126``.
     """
 
     def __init__(self, channel) -> None:
@@ -286,7 +286,7 @@ class ArraysToArraysServiceBase:
     """Server base: subclasses implement the three coroutines; ``__mapping__`` and
     :meth:`generic_handler` expose them to a ``grpc.aio`` server.
 
-    Counterpart of ``/root/reference/pytensor_federated/rpc.py:129-187``.
+    Counterpart of ``pytensor_federated/rpc.py:129-187``.
     """
 
     async def evaluate(self, input_arrays: InputArrays) -> OutputArrays:
@@ -354,7 +354,7 @@ class ArraysToArraysServiceBase:
 class Server:
     """Tiny façade over ``grpc.aio.server`` with the grpclib-style lifecycle the
     reference's launchers use (``Server([service]); await start(host, port);
-    await wait_closed()`` — ``/root/reference/demo_node.py:76-79``)."""
+    await wait_closed()`` — ``demo_node.py:76-79``)."""
 
     def __init__(self, services: Sequence[ArraysToArraysServiceBase], *, tls=None) -> None:
         """``tls``: a :class:`~pytensor_federated_b200.config.TlsConfig` with ``cert`` + ``key`` (+ ``ca`` when

@@ -1,7 +1,7 @@
 """Gradient-based inference drivers for federated log-potentials.
 
-The reference delegates sampling to PyMC (``/root/reference/demo_model.py:38-44``:
-``pm.find_MAP()`` + ``pm.sample()``/NUTS).  PyMC is not available in the B200 image, so this
+The reference delegates sampling to PyMC (``demo_model.py:38-44``:
+``pm.find_MAP()`` + ``pm.sample()``/NUTS).  PyMC is not available in the offline image, so this
 package ships the drivers that exercise the hot path — MAP by L-BFGS, HMC and NUTS with
 dual-averaging step-size adaptation, and random-walk Metropolis for gradient-free potentials (``LogpOp``) — on top of any ``logp_dlogp(theta) -> (float, ndarray)``
 callable, plus a minimal model builder over the graph IR.  With PyMC installed the Ops plug into

@@ -4,7 +4,7 @@ This is the sampler that matches the tensor-core GLM kernels: ``GlmShards(..., n
 K parameter vectors in one fused launch for (almost) the price of one, because the design matrix is
 streamed from HBM once and the chains ride along the MMA's N dimension.  The reference gets chain
 parallelism from one process per chain, each with its own gRPC connection
-(``/root/reference/pytensor_federated/test_wrapper_ops.py:305-317``); here K chains share one launch.
+(``pytensor_federated/test_wrapper_ops.py:305-317``); here K chains share one launch.
 
 ``logp_dlogp_batch(theta[K, D]) -> (logp[K], grad[K, D])``.
 """

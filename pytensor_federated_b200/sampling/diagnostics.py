@@ -1,6 +1,6 @@
 """Convergence diagnostics for multi-chain draws: split-R-hat, effective sample size, a summary table.
 
-The reference's demo prints PyMC/ArviZ's summary after ``pm.sample`` (``/root/reference/demo_model.py:44``);
+The reference's demo prints PyMC/ArviZ's summary after ``pm.sample`` (``demo_model.py:44``);
 these are the same estimators (Vehtari et al. 2021: rank-free split-R-hat, Geyer initial-positive-sequence
 ESS with FFT autocovariances) for the in-repo samplers, including the lock-step batched HMC whose draws
 already come as ``[draws, chains, dim]``.

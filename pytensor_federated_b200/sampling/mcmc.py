@@ -335,7 +335,7 @@ def metropolis_sample(
     """Random-walk Metropolis for gradient-free potentials (``LogpOp`` / ``LogpServiceClient``).
 
     The reference samples its gradient-free black box with ``pm.Metropolis()``
-    (``/root/reference/pytensor_federated/test_wrapper_ops.py:68-118``); this is the in-repo counterpart:
+    (``pytensor_federated/test_wrapper_ops.py:68-118``); this is the in-repo counterpart:
     all coordinates are proposed jointly from ``N(0, (scale * s)^2)`` with a per-coordinate ``s``; during
     ``tune`` the global scale is adapted every ``tune_interval`` steps from the acceptance rate of the
     interval (the schedule PyMC uses: shrink below 20 % / 5 % / 0.1 %, grow above 50 % / 75 % / 95 %) and

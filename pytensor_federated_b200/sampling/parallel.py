@@ -2,7 +2,7 @@
 
 With PyMC the reference runs one chain per process (``pm.sample(cores=4)``); every process gets its own
 connection (``thread_pid_id`` keyed connection cache) and ``hosts_and_ports`` places it on the replica
-with the fewest open streams (``/root/reference/pytensor_federated/service.py:239-275``,
+with the fewest open streams (``pytensor_federated/service.py:239-275``,
 ``test_wrapper_ops.py:305-317``).  :func:`sample_parallel` is that driver for the in-repo samplers: the
 model is *built inside each worker* by a picklable factory, so clients connect (and balance) there.
 """

@@ -1,6 +1,6 @@
 """``ArraysToArraysService`` / ``ArraysToArraysServiceClient`` — transport layer.
 
-Capabilities mirrored from ``/root/reference/pytensor_federated/service.py``:
+Capabilities mirrored from ``pytensor_federated/service.py``:
 
 * server wrapper around a ``ComputeFunc`` with ``Evaluate`` / ``EvaluateStream`` /
   ``GetLoad`` (``:75-115``), load metric = 1-min loadavg per core and RAM % (``:88-96``)
@@ -58,7 +58,7 @@ HostPort = Tuple[str, int]
 
 CONNECT_SLEEP_RANGE: Tuple[float, float] = (0.2, 2.0)
 """Random delay before load probing that de-synchronises parallel MCMC chains
-(``/root/reference/pytensor_federated/service.py:250``).  Override with the
+(``pytensor_federated/service.py:250``).  Override with the
 ``B200FED_CONNECT_SLEEP="lo,hi"`` environment variable (e.g. ``"0,0"`` in tests)."""
 
 

@@ -1,6 +1,6 @@
 """Type and signature definitions (no runtime behaviour).
 
-Reference: ``/root/reference/pytensor_federated/signatures.py:8-33``.
+Reference: ``pytensor_federated/signatures.py:8-33``.
 """
 from typing import Callable, Sequence, Tuple
 

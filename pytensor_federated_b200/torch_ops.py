@@ -4,7 +4,7 @@ The reference integrates with PyTensor only.  Users whose sampler or optimiser l
 (Pyro, custom HMC, ``torch.optim``) get the same contract here: a federated ``LogpGradFunc``
 becomes a differentiable scalar whose backward pass re-uses the gradients returned by the same
 remote evaluation — one federated call per forward+backward, like ``LogpGradOp.grad``
-(``/root/reference/pytensor_federated/wrapper_ops.py:119-132``).
+(``pytensor_federated/wrapper_ops.py:119-132``).
 """
 from __future__ import annotations
 

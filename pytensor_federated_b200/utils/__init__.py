@@ -1,6 +1,6 @@
 """Generic helpers with only external dependencies.
 
-Reference: ``/root/reference/pytensor_federated/utils.py:13-61``.
+Reference: ``pytensor_federated/utils.py:13-61``.
 """
 from .aio import argmin_none_or_func, get_useful_event_loop
 

@@ -1,6 +1,6 @@
 """Event-loop and selection helpers.
 
-Reference behaviour: ``/root/reference/pytensor_federated/utils.py:13-34`` (argmin
+Reference behaviour: ``pytensor_federated/utils.py:13-34`` (argmin
 that ignores ``None``) and ``:37-61`` (a loop one can always ``run_until_complete``
 on, re-entrantly patched with ``nest_asyncio`` when already running).
 """

@@ -1,6 +1,6 @@
 """Ops that put federated functions into a differentiable graph.
 
-Capabilities of ``/root/reference/pytensor_federated/wrapper_ops.py``: ``ArraysToArraysOp``
+Capabilities of ``pytensor_federated/wrapper_ops.py``: ``ArraysToArraysOp``
 (``:14-33``), ``LogpOp`` (``:44-69``), ``LogpGradOp`` with its ``grad`` (``:84-132``) and their
 ``Async*`` twins (``:36-41``, ``:72-81``, ``:135-146``).  ``make_node`` arities, output types and
 the ``grad`` contract are the reference's, so a PyMC model that used its ``LogpGradOp`` compiles
@@ -117,8 +117,8 @@ class FederatedLogpGradOp(FusableAsyncOp, LogpGradOp):
     shard index.  Evaluated alone it asks the engine for that node's ``(logp, grads)``.  When the
     ``fuse_asyncs`` rewrite has put several such applies (same federation) into one
     :class:`ParallelAsyncOp`, they are all answered by a single fused broadcast->compute->reduce
-    launch across the GPUs — the B200-native replacement of N concurrent gRPC round trips
-    (``/root/reference/pytensor_federated/op_async.py:114-130``).
+    launch across the GPUs — the GPU-native replacement of N concurrent gRPC round trips
+    (``pytensor_federated/op_async.py:114-130``).
     """
 
     def __init__(self, federation, node: int) -> None:

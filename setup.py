@@ -1,6 +1,6 @@
-"""Packaging: the native library is compiled for sm_100a at build time when nvcc is present.
+"""Packaging: the native library is compiled for sm_90a at build time when nvcc is present.
 
-Counterpart of ``/root/reference/setup.py`` (which has no native step).
+Counterpart of ``setup.py`` (which has no native step).
 """
 import os
 import sys

@@ -48,7 +48,7 @@ def straight_line_blackbox(intercept, slope):
     """Gradient-free black box: log-likelihood of y = 2 x + 0.5 (+ noise, sd 0.1) at 15 points.
 
     The fixture of the reference's gradient-free end-to-end test
-    (``/root/reference/pytensor_federated/test_wrapper_ops.py:55-65``): same data-generating recipe, so the
+    (``pytensor_federated/test_wrapper_ops.py:55-65``): same data-generating recipe, so the
     golden value of that test, ``logp(0.4, 1.2) = -1511.41423640139``, must come out here too."""
     import scipy.stats
 

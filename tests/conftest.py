@@ -12,5 +12,5 @@ os.environ.setdefault("B200FED_CONNECT_SLEEP", "0,0")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `-m gpu`)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 GPUs")

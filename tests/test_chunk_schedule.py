@@ -9,7 +9,7 @@ from pytensor_federated_b200.ops import native
 TILE = 128
 
 
-def chunk_table(n_rows, sm_count=148, multiple=2, max_chunk=32, min_chunk=4):
+def chunk_table(n_rows, sm_count=132, multiple=2, max_chunk=32, min_chunk=4):
     lib = native.load()
     rows = (C.c_longlong * len(n_rows))(*n_rows)
     cap = 1 << 20
@@ -39,16 +39,16 @@ def test_chunks_shrink_towards_the_end_of_the_work():
     sizes = table[:, 2]
     assert sizes[0] == 32 and sizes[len(sizes) // 2] == 32
     assert sizes[-1] <= 6
-    # the tail that keeps 148 SMs busy after the last big chunk is handed out is made of small chunks
+    # the tail that keeps 132 SMs busy after the last big chunk is handed out is made of small chunks
     tail = sizes[-300:]
     assert tail.max() <= 8 and (np.diff(sizes[-2000:].astype(int)) <= 2).all()
     # far more chunks than SMs, but not so many that claiming them matters (one atomic per chunk)
-    assert 148 * 20 < len(sizes) < 148 * 300
+    assert 132 * 20 < len(sizes) < 132 * 300
 
 
 def test_small_problems_still_spread_over_the_sms():
     table = chunk_table([100_000])            # 782 tiles
-    assert len(table) >= 148
+    assert len(table) >= 132
     tiny = chunk_table([9000])                # 71 tiles
     assert (tiny[:, 2] == 2).all() and len(tiny) == 36
 

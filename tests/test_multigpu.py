@@ -1,4 +1,4 @@
-"""Fused broadcast -> compute -> reduce across GPUs (needs >= 2 B200s; run with gpurun --gpus N).
+"""Fused broadcast -> compute -> reduce across GPUs (needs >= 2 GPUs).
 
 Every scenario runs at world = 2, 4 and 8; a world larger than the number of visible GPUs is skipped."""
 import os

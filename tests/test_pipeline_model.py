@@ -1,15 +1,14 @@
-"""Executable model of the warp-specialised pipeline of csrc/glm_fp8.cu (and, without the scale ring, of
-csrc/glm_tc.cu): TMA producer, MMA #1 issuer, kEG epilogue groups, MMA #2 issuer, mbarriers with phase
-parity.  A randomised scheduler interleaves the roles; the model checks what the barrier protocol has
-to guarantee for every interleaving:
+"""Executable model of a warp-specialised mbarrier pipeline with separate roles: TMA producer, MMA #1 issuer,
+kEG epilogue groups, MMA #2 issuer, a scale-word ring, mbarriers with phase parity.  This was the protocol of
+the tensor-core GLM kernels when they targeted tcgen05 (accumulators in tensor memory); the sm_90a kernels
+use a different one, modelled in tests/test_consumer_protocol_model.py.  What stays relevant here is the
+generic ring arithmetic the producer still uses (it % S, (it / S) & 1 and the arrive / parity-wait pairing of
+an S-deep stage ring), exercised with many roles and barriers over thousands of schedules:
 
 * no dead-lock for any tile count (including fewer tiles than stages / groups, partial flush periods);
 * a smem stage, an eta / R buffer or a scale-ring slot is never overwritten before its consumer is done;
 * every tile's eta is consumed by the group that owns the tile, with that tile's scale words;
 * every tile is accumulated into G exactly once and every flush period is read out exactly once.
-
-The index / parity formulas are the kernel's (it % S, (it / S) & 1, it % kEG, ...), so a change to the
-kernel's protocol has to be mirrored here — and is then exercised over thousands of schedules on the CPU.
 """
 import random
 

@@ -2,7 +2,7 @@
 
 PyTensor cannot be installed in this image, so the branch that makes the Ops genuine PyTensor Ops would
 otherwise never execute.  The stand-in lays the in-repo IR out under PyTensor's public module paths (the ones
-``/root/reference/pytensor_federated/op_async.py:4-11`` and ``wrapper_ops.py:4-8`` import); a fresh interpreter
+``pytensor_federated/op_async.py:4-11`` and ``wrapper_ops.py:4-8`` import); a fresh interpreter
 with the stand-in on its path must select ``BACKEND == "pytensor"``, register ``fuse_asyncs`` in *that* optdb,
 and build / differentiate / compile the wrapper Ops through those imports.  It proves the import surface and
 the module-level registration, not PyTensor's own semantics."""

@@ -18,6 +18,7 @@
 // recombined in fp32/fp64, so the low precision of the operand does not leak into the gradient.
 // Poisson / Gaussian residuals are unbounded: there (template DYN) every 32-row group of R gets its own
 // power-of-two scale s_r (from the group's largest |r|), so the expansion is relative to the block maximum.
+// Observation weights make even logistic residuals unbounded, so weighted models take the DYN scaling too.
 //
 // Roles and pipeline as in glm_tc.cu.  Workload: BASELINE.json "hierarchical GLM, 8 partial-pooling groups
 // (one per GPU), fp8 block-scaled design matrix" (groups = intercepts).
@@ -102,8 +103,9 @@ __host__ __device__ inline SmemLayoutF smem_layout(int P, int n_theta, int n_gro
     return L;
 }
 
-// KF = chains per launch: 1 or 3; DYN = per-row-group residual scales (families with unbounded residuals)
-template <int KF, bool DYN>
+// KF = chains per launch: 1 or 3; DYN = per-row-group residual scales (families with unbounded residuals, or
+// weights); ROWS = some segment has per-row offsets or weights (see csrc/glm_tc.cu)
+template <int KF, bool DYN, bool ROWS>
 __global__ void __launch_bounds__(kThreadsF, 1)
 fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                    const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -294,6 +296,8 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
                 const int4 ch = consumer_chunk(j);
                 if (ch.x < 0) break;
                 const float* __restrict__ seg_y = segs_g[ch.x].y;
+                const float* __restrict__ seg_o = ROWS ? segs_g[ch.x].offset : nullptr;   // null: absent (chunk-uniform)
+                const float* __restrict__ seg_w = ROWS ? segs_g[ch.x].weight : nullptr;
                 const long long seg_rows = segs_g[ch.x].n_rows;
                 const long long seg_tiles = (seg_rows + kTile - 1) / kTile;
                 const uint8_t* __restrict__ seg_sc = reinterpret_cast<const uint8_t*>(segs_g[ch.x].scales);
@@ -393,13 +397,25 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
                         const long long grow = tile * kTile + row;
                         valid[h] = grow < seg_rows;
                         yv[h] = valid[h] ? __ldg(seg_y + grow) : 0.f;
+                        float o = 0.f, wt = 1.f;   // offset and weight of the row
+                        if constexpr (ROWS) {
+                            if (valid[h] && seg_o) o = __ldg(seg_o + grow);
+                            if (valid[h] && seg_w) wt = __ldg(seg_w + grow);
+                        }
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int k = 2 * q + e;
                             const int kk = k < KF ? k : 0;
-                            const float eta = (eacc[2 * h + e] + eacc[4 + 2 * h + e]) + eacc[8 + 2 * h + e] + theta_f[kk * PG + seg_group];
+                            float eta = (eacc[2 * h + e] + eacc[4 + 2 * h + e]) + eacc[8 + 2 * h + e] + theta_f[kk * PG + seg_group];
+                            if constexpr (ROWS) eta = __fadd_rn(eta, o);   // offset after the intercept
                             float ll = 0.f, r = 0.f;
-                            if (valid[h] && k < nch) link_loglik(DYN ? prm.family : 0, yv[h], eta, ll, r);
+                            if (valid[h] && k < nch) {
+                                link_loglik(DYN ? prm.family : 0, yv[h], eta, ll, r);
+                                if constexpr (ROWS) {   // weight after the likelihood; a zero weight selects 0
+                                    ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                    r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                }
+                            }
                             ll_acc[e] += ll;
                             gi_acc[e] += r;
                             rr_[h][e] = r;
@@ -602,9 +618,10 @@ extern "C" int b200_launch_glm_fp8(const FedComm* comm, const GlmSegment* segs_d
     const fp8::SmemLayoutF L = fp8::smem_layout(prm->n_features, comm->n_theta, prm->n_groups);
     if (L.stages < 2) return -2;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define B200FED_FP8_LAUNCH(KF, DYN)                                                                                       \
+#define B200FED_FP8_LAUNCH(KF, DYN, ROWS)                                                                                 \
     do {                                                                                                                 \
-        cudaFuncSetAttribute(fp8::fed_glm_fp8_kernel<KF, DYN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(fp8::fed_glm_fp8_kernel<KF, DYN, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
+                             (int)L.total);                                                                              \
         cudaLaunchConfig_t cfg{};                                                                                        \
         cfg.gridDim = dim3(grid);                                                                                        \
         cfg.blockDim = dim3(fp8::kThreadsF);                                                                             \
@@ -615,14 +632,24 @@ extern "C" int b200_launch_glm_fp8(const FedComm* comm, const GlmSegment* segs_d
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                          \
         cfg.attrs = attr;                                                                                                \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                            \
-        cudaLaunchKernelEx(&cfg, fp8::fed_glm_fp8_kernel<KF, DYN>, *comm, segs_dev, *prm, maps,                          \
+        cudaLaunchKernelEx(&cfg, fp8::fed_glm_fp8_kernel<KF, DYN, ROWS>, *comm, segs_dev, *prm, maps,                    \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                       \
     } while (0)
-    const bool dyn = prm->family != 0;  // unbounded residuals: per-row-group scales for the R operand
+    // unbounded residuals (Poisson, Gaussian, or any weighted model): per-row-group scales for the R operand
+    const bool dyn = prm->family != 0 || (prm->row_data & kGlmRowWeights);
+    const bool rows = prm->row_data != 0;
     if (prm->n_chains == 1) {
-        if (dyn) B200FED_FP8_LAUNCH(1, true); else B200FED_FP8_LAUNCH(1, false);
+        if (rows) {
+            if (dyn) B200FED_FP8_LAUNCH(1, true, true); else B200FED_FP8_LAUNCH(1, false, true);
+        } else {
+            if (dyn) B200FED_FP8_LAUNCH(1, true, false); else B200FED_FP8_LAUNCH(1, false, false);
+        }
     } else {
-        if (dyn) B200FED_FP8_LAUNCH(3, true); else B200FED_FP8_LAUNCH(3, false);
+        if (rows) {
+            if (dyn) B200FED_FP8_LAUNCH(3, true, true); else B200FED_FP8_LAUNCH(3, false, true);
+        } else {
+            if (dyn) B200FED_FP8_LAUNCH(3, true, false); else B200FED_FP8_LAUNCH(3, false, false);
+        }
     }
 #undef B200FED_FP8_LAUNCH
     return (int)cudaGetLastError();

@@ -130,7 +130,17 @@ fed_glm_generic_kernel(FedComm comm, const GlmSegment* __restrict__ segs, GlmPar
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) p += __shfl_xor_sync(0xffffffffu, p, o);
                 float ll, r;
-                link_loglik_g(prm.family, __ldg(seg.y + row), p + icpt, ll, r);
+                // per-row offset / weight (null: absent, uniform per segment) around the likelihood, custom ones
+                // included; rounded on their own, so w = 1, o = 0 gives the bits of the plain model, and a zero weight
+                // selects 0 over a non-finite y or offset
+                float eta = p + icpt;
+                if (seg.offset) eta = __fadd_rn(eta, __ldg(seg.offset + row));
+                link_loglik_g(prm.family, __ldg(seg.y + row), eta, ll, r);
+                if (seg.weight) {
+                    const float wt = __ldg(seg.weight + row);
+                    ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                    r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                }
 #pragma unroll
                 for (int j = 0; j < J; ++j) g[j] = fmaf(r, x[j], g[j]);
                 if (lane == 0) {

@@ -1,6 +1,6 @@
 // Federated GLM log-likelihood + gradient, single pass over a bf16 design matrix (SIMT path).
 //
-//   eta = intercept[group] + X beta ;  LL = sum ll(y, eta) ;  r = dll/deta
+//   eta = intercept[group] + X beta (+ offset) ;  LL = sum w ll(y, eta) ;  r = w dll/deta
 //   dLL/dintercept[g] = sum_{rows of g} r ;  dLL/dbeta = X^T r
 //
 // X is read from HBM exactly once per evaluation: a warp loads 8 rows (one 16-byte
@@ -192,7 +192,15 @@ fed_glm_simt_kernel(FedComm comm, const GlmSegment* __restrict__ segs, GlmParams
             float ll = 0.f, r = 0.f;
             if (myrow < seg.n_rows) {
                 const float y = __ldg(seg.y + myrow);
+                // per-row offset / weight (null: absent, uniform per segment); rounded on their own, so w = 1, o = 0
+                // gives the bits of the plain model, and a zero weight selects 0 over a non-finite y or offset
+                if (seg.offset) eta = __fadd_rn(eta, __ldg(seg.offset + myrow));
                 link_loglik(prm.family, y, eta, ll, r);
+                if (seg.weight) {
+                    const float wt = __ldg(seg.weight + myrow);
+                    ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                    r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                }
             }
             ll_acc += ll;
             gi += r;

@@ -76,7 +76,8 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
     return L;
 }
 
-// KC = chains per launch.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// KC = chains per launch; ROWS = some segment has per-row offsets or weights (GlmSegment::offset / weight), so
+// models without them run an instantiation with no trace of the extra loads.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -99,7 +100,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC>
+template <int KC, bool ROWS>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -297,6 +298,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 const int4 ch = consumer_chunk(j);
                 if (ch.x < 0) break;
                 const float* __restrict__ seg_y = segs_g[ch.x].y;   // segment table: global, read once per chunk
+                const float* __restrict__ seg_o = ROWS ? segs_g[ch.x].offset : nullptr;   // null: absent (chunk-uniform)
+                const float* __restrict__ seg_w = ROWS ? segs_g[ch.x].weight : nullptr;
                 const long long seg_rows = segs_g[ch.x].n_rows;
                 const int seg_group = segs_g[ch.x].group;
                 const int og = segs_g[ch.x].out_group;               // output block of this chunk's segment
@@ -304,6 +307,19 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                 for (int s = 0; s < 2 * NJ; ++s) ll_acc[s] = gi_acc[s] = 0.f;
                 for (int t = 0; t < ch.z; ++t) {
+                    // row data: y, offset and weight of this thread's two rows, loaded before the tile is waited for
+                    // and MMA #1 runs, so three dependent global reads do not sit between the two GEMMs
+                    float y_r[2], o_r[2], w_r[2];
+                    if constexpr (ROWS) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const long long grow = (long long)ch.y + (long long)t * kTileM + 64 * c + 16 * w + (lane >> 2) + 8 * h;
+                            const bool valid = grow < seg_rows;
+                            y_r[h] = valid ? __ldg(seg_y + grow) : 0.f;
+                            o_r[h] = valid && seg_o ? __ldg(seg_o + grow) : 0.f;
+                            w_r[h] = valid && seg_w ? __ldg(seg_w + grow) : 1.f;
+                        }
+                    }
                     mbar_wait(&bar_full[stage.idx], stage.phase);
                     const uint32_t x_a = x_base_a + (uint32_t)stage.idx * L.stage_bytes;
                     // ---- MMA #1: eta of this group's 64 rows
@@ -330,7 +346,14 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                         const int row = 64 * c + 16 * w + (lane >> 2) + 8 * h;   // row of the tile
                         const long long grow = (long long)ch.y + (long long)t * kTileM + row;
                         const bool valid = grow < seg_rows;
-                        const float y = valid ? __ldg(seg_y + grow) : 0.f;
+                        float y, o = 0.f, wt = 1.f;   // response, offset and weight of the row
+                        if constexpr (ROWS) {
+                            y = y_r[h];
+                            o = o_r[h];
+                            wt = w_r[h];
+                        } else {
+                            y = valid ? __ldg(seg_y + grow) : 0.f;
+                        }
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc)
 #pragma unroll
@@ -339,7 +362,18 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 const float eta = (eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
                                 float ll = 0.f, r = 0.f;
-                                if (valid && k < nch) link_loglik(prm.family, y, eta + icpt[k * G + seg_group], ll, r);
+                                if (valid && k < nch) {
+                                    if constexpr (ROWS) {
+                                        // offset after the intercept, weight after the likelihood, both rounded on their
+                                        // own (no FMA contraction): w = 1, o = 0 gives the bits of the plain model; a
+                                        // zero weight selects 0, so a masked row's non-finite y or o never reaches a sum
+                                        link_loglik(prm.family, y, __fadd_rn(eta + icpt[k * G + seg_group], o), ll, r);
+                                        ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                        r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                    } else {
+                                        link_loglik(prm.family, y, eta + icpt[k * G + seg_group], ll, r);
+                                    }
+                                }
                                 ll_acc[2 * jc + e] += ll;
                                 gi_acc[2 * jc + e] += r;
                                 if (k < N2 / 2) {
@@ -522,12 +556,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC)                                                                                              \
+#define LAUNCH_TC(KC, ROWS)                                                                                        \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
                                                  prm->n_groups, KC);                                               \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -538,13 +572,14 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC>, *comm, segs_dev, *prm, maps,                           \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS>, *comm, segs_dev, *prm, maps,                     \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
-    if (kc == 1) LAUNCH_TC(1);
-    else if (kc == 4) LAUNCH_TC(4);
-    else if (kc == 8) LAUNCH_TC(8);
-    else LAUNCH_TC(16);
+    const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
+    if (kc == 1) { if (rows) LAUNCH_TC(1, true); else LAUNCH_TC(1, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true); else LAUNCH_TC(4, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true); else LAUNCH_TC(8, false); }
+    else { if (rows) LAUNCH_TC(16, true); else LAUNCH_TC(16, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

@@ -16,6 +16,8 @@ struct GlmSegment {
     const void* X;        // [n_rows, ld] row-major; bf16 (or fp8 e4m3 for the block-scaled kernel)
     const float* y;       // [n_rows] response (0/1 for logistic)
     const void* scales;   // fp8 only: per-(row, 32-feature block) ue8m0 scales, else null
+    const float* offset;  // [n_rows] known part of eta added after the intercept, or null (no offset)
+    const float* weight;  // [n_rows] observation weights (>= 0; 0 masks the row), or null (weight 1)
     long long n_rows;
     long long first_tile; // prefix sum over segments of ceil(n_rows / tile_rows)
     int group;            // which intercept this segment uses
@@ -32,7 +34,11 @@ struct GlmParams {
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)
+    int row_data;         // kGlmRowOffsets | kGlmRowWeights when any segment has them: selects the kernel instantiation
 };
+
+constexpr int kGlmRowOffsets = 1;
+constexpr int kGlmRowWeights = 2;
 
 // Unit of work of the dynamically scheduled tensor-core GLM kernel: n_tiles consecutive 128-row tiles of one
 // segment starting at tile first_tile (n_tiles is even; the last one may lie past the segment's rows).

@@ -549,17 +549,23 @@ int b200_engine_set_linreg(void* h, int n_shards, const void** x, const void** y
 
 int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y, const void** scales,
                         const long long* n_rows, const int* groups, int n_features, int ld, int n_groups,
-                        int n_chains, int family, int use_tensor_cores, const int* out_groups, int n_out) {
+                        int n_chains, int family, int use_tensor_cores, const int* out_groups, int n_out,
+                        const float** offsets, const float** weights) {
     Engine* e = static_cast<Engine*>(h);
     CK(cudaSetDevice(e->device));
     const int tile_rows = (use_tensor_cores == 1 || use_tensor_cores == 2) ? 128 : 8;
     e->glm_segs.resize(n_segments);
     long long tiles = 0;
+    int row_data = 0;
     for (int s = 0; s < n_segments; ++s) {
         GlmSegment g{};
         g.X = X[s];
         g.y = y[s];
         g.scales = scales ? scales[s] : nullptr;
+        g.offset = offsets ? offsets[s] : nullptr;   // per-row data: a null array or entry means none
+        g.weight = weights ? weights[s] : nullptr;
+        if (g.offset) row_data |= kGlmRowOffsets;
+        if (g.weight) row_data |= kGlmRowWeights;
         g.n_rows = n_rows[s];
         g.first_tile = tiles;
         g.group = groups[s];
@@ -571,7 +577,8 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         e->glm_segs[s] = g;
         tiles += (n_rows[s] + tile_rows - 1) / tile_rows;
     }
-    e->glm = GlmParams{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1, early_loads_enabled() ? 1 : 0};
+    e->glm = GlmParams{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
+                       early_loads_enabled() ? 1 : 0, row_data};
     if ((long long)e->glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
         g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
         return -33;

@@ -47,6 +47,22 @@ class GlmShards(ShardModel):
         at node boundaries into fixed-point accumulators).  ``evaluate`` still returns the sum; :meth:`per_node` and
         :class:`~pytensor_federated_b200.federation.NodeFederation` expose the blocks — the reference's
         one-Op-per-node pattern (``demo_model.py:28-36``) answered by one launch.
+    offsets, weights
+        Per-row data, ``None`` or one entry per segment: ``None`` (no offset / weight 1 for that segment) or a 1-D
+        tensor of the segment's ``n_rows`` (converted once to contiguous float32; a tensor must already live on the
+        device of X).  Every kernel evaluates
+
+            eta_i = intercept[group] + x_i' beta + o_i,     LL = sum_i w_i ll(y_i, eta_i),
+            dLL/dbeta = sum_i w_i r_i x_i,   dLL/dintercept[g] = sum_{i in g} w_i r_i,   r_i = dll/deta at eta_i,
+
+        the family constants weighted with the rest: Gaussian rows give ``w (-d^2 / 2 - log(2 pi) / 2)``, Poisson
+        rows still omit ``-lgamma(y + 1)``.  Offsets carry exposures (``log t`` for Poisson rates) and known
+        per-row terms; weights carry binomial trial counts (``y = k / n``, ``w = n``), frequency and survey
+        weights.  A row of weight 0 contributes exactly nothing, even if its ``y`` or offset is not finite (its X
+        row must be finite), which masks rows (held-out folds, bad rows) without copying X.  Weights must be
+        finite and >= 0, offsets finite wherever the weight is not 0.  ``w = 1, o = 0`` reproduces the plain
+        model bit for bit on the ``tc``, ``simt`` and general-shape kernels.  The kernels read the tensors given
+        here on every evaluation, as they read X and y.
     """
 
     def __init__(
@@ -62,6 +78,8 @@ class GlmShards(ShardModel):
         scales: Optional[Sequence] = None,
         node_ids: Optional[Sequence[int]] = None,
         n_nodes: Optional[int] = None,
+        offsets: Optional[Sequence] = None,
+        weights: Optional[Sequence] = None,
     ) -> None:
         import torch
 
@@ -69,6 +87,17 @@ class GlmShards(ShardModel):
             raise ValueError("Xs and ys must have the same length")
         self.Xs = list(Xs)
         self.ys = [y.to(torch.float32).contiguous() for y in ys]
+        self.weights = self._row_data(weights, "weights")
+        self.offsets = self._row_data(offsets, "offsets")
+        for si, (o, w) in enumerate(zip(self.offsets, self.weights)):
+            if w is not None and not bool(torch.all(torch.isfinite(w) & (w >= 0))):
+                raise ValueError(f"weights of segment {si} must be finite and >= 0")
+            if o is not None:
+                bad = ~torch.isfinite(o)
+                if w is not None:
+                    bad &= w != 0   # a masked row may carry anything
+                if bool(torch.any(bad)):
+                    raise ValueError(f"offsets of segment {si} must be finite on every row of non-zero weight")
         self.scales = list(scales) if scales is not None else None
         self.groups = list(groups) if groups is not None else [0] * len(Xs)
         self.n_groups = int(n_groups)
@@ -92,6 +121,35 @@ class GlmShards(ShardModel):
         if self.node_ids is not None and (len(self.node_ids) != len(self.Xs) or not all(0 <= i < self.n_nodes for i in self.node_ids)):
             raise ValueError("node_ids needs one node index in [0, n_nodes) per segment")
         self.n_vals = self.n_nodes * self.n_chains * (1 + self.n_params)
+
+    def _row_data(self, entries, name: str) -> list:
+        """One contiguous float32 tensor (or None) per segment, on the device of the segment's X."""
+        import torch
+
+        if entries is None:
+            return [None] * len(self.Xs)
+        entries = list(entries)
+        if len(entries) != len(self.Xs):
+            raise ValueError(f"{name} needs one entry (None or a tensor) per segment: got {len(entries)} for {len(self.Xs)}")
+        out = []
+        for si, (v, X) in enumerate(zip(entries, self.Xs)):
+            if v is None:
+                out.append(None)
+                continue
+            if isinstance(v, torch.Tensor):
+                if v.device != X.device:
+                    raise ValueError(f"{name} of segment {si} are on device {v.device}, its X on {X.device}")
+            else:
+                v = torch.as_tensor(np.asarray(v), device=X.device)
+            if v.dim() != 1 or v.shape[0] != X.shape[0]:
+                raise ValueError(f"{name} of segment {si} must be 1-D with {X.shape[0]} rows, got shape {tuple(v.shape)}")
+            out.append(v.to(torch.float32).contiguous())
+        return out
+
+    @property
+    def has_row_data(self) -> bool:
+        """Whether some segment has offsets or weights."""
+        return any(v is not None for v in self.offsets + self.weights)
 
     @property
     def n_rows(self) -> int:
@@ -206,10 +264,14 @@ class GlmShards(ShardModel):
                 "P <= 384, 16-byte aligned rows): using the %s CUDA-core kernel — single pass, but slower",
                 self.n_features, self.Xs[0].dtype, self.ld, self.selected_kernel)
         out_grp = (C.c_int * n)(*self.node_ids) if self.node_ids is not None else None
+        op = native.void_p_array([o.data_ptr() if o is not None else 0 for o in self.offsets]) \
+            if any(o is not None for o in self.offsets) else None
+        wp = native.void_p_array([w.data_ptr() if w is not None else 0 for w in self.weights]) \
+            if any(w is not None for w in self.weights) else None
         native.check(
             lib.b200_engine_set_glm(
                 handle, n, Xp, yp, sp, rows, grp, self.n_features, self.ld, self.n_groups,
-                self.n_chains, _family_code(self.family), code, out_grp, self.n_nodes,
+                self.n_chains, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
             ),
             "set_glm",
         )
@@ -237,6 +299,8 @@ class GlmShards(ShardModel):
                 r1 = min(X.shape[0], r0 + chunk_rows)
                 Xf = self._dequant_rows(si, r0, r1).to(dtype)
                 eta = Xf @ B.T + icg                                # [n, K]
+                if self.offsets[si] is not None:
+                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
                 yy = y[r0:r1].to(dtype).unsqueeze(1)
                 if hasattr(self.family, "code_id"):
                     if self.family.torch_fn is None:
@@ -253,10 +317,23 @@ class GlmShards(ShardModel):
                     d = yy - eta
                     ll = -0.5 * d * d - 0.918938533204672742
                     r = d
+                ll, r = self._weigh(si, r0, r1, ll, r)
                 out[:, 0] += ll.double().sum(0)
                 out[:, 1 + g] += r.double().sum(0)
                 out[:, 1 + self.n_groups :] += (r.T @ Xf).double()
         return full.reshape(-1).cpu().numpy()
+
+    def _weigh(self, seg: int, r0: int, r1: int, ll, r):
+        """``(w ll, w r)`` of rows ``[r0, r1)`` of segment ``seg``; rows of weight 0 give exactly 0 (a select, not
+        a product: their ``ll`` may be NaN)."""
+        import torch
+
+        w = self.weights[seg]
+        if w is None:
+            return ll, r
+        ww = w[r0:r1].to(ll.dtype).unsqueeze(1)
+        keep = ww != 0
+        return torch.where(keep, ww * ll, torch.zeros_like(ll)), torch.where(keep, ww * r, torch.zeros_like(r))
 
     def _dequant_rows(self, seg: int, r0: int, r1: int):
         """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
@@ -278,8 +355,10 @@ class GlmShards(ShardModel):
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float32)).reshape(self.n_chains, -1).to(self.device)
         bt = torch.as_tensor(np.asarray(beta, dtype=np.float32)).reshape(self.n_chains, self.n_features).to(self.device)
         out = torch.zeros(self.n_chains, 1 + self.n_params, dtype=torch.float64, device=self.device)
-        for X, y, g in zip(self.Xs, self.ys, self.groups):
+        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
             eta = (X @ bt.T.to(torch.bfloat16)).float() + ic[:, g]          # [n, K]
+            if self.offsets[si] is not None:
+                eta = eta + self.offsets[si].unsqueeze(1)
             yy = y.unsqueeze(1)
             if self.family == "logistic":
                 ll = yy * eta - torch.nn.functional.softplus(eta)
@@ -292,13 +371,18 @@ class GlmShards(ShardModel):
                 d = yy - eta
                 ll = -0.5 * d * d - 0.918938533204672742
                 r = d
+            ll, r = self._weigh(si, 0, X.shape[0], ll, r)
             out[:, 0] += ll.sum(0).double()
             out[:, 1 + g] += r.sum(0).double()
             out[:, 1 + self.n_groups :] += (r.T.to(torch.bfloat16) @ X).double()
         return out.reshape(-1).cpu().numpy()
 
+    def _row_data_bytes(self) -> int:
+        """Bytes of offsets and weights read per evaluation (4 per row per vector present)."""
+        return int(sum(4 * v.shape[0] for v in self.offsets + self.weights if v is not None))
+
     def bytes_per_eval(self) -> int:
-        return int(sum(X.shape[0] * (self.n_features * X.element_size() + 4) for X in self.Xs))
+        return int(sum(X.shape[0] * (self.n_features * X.element_size() + 4) for X in self.Xs)) + self._row_data_bytes()
 
     def flops_per_eval(self) -> int:
         return int(4 * self.n_rows * self.n_features * self.n_chains)
@@ -370,15 +454,16 @@ class Fp8GlmShards(GlmShards):
     shard/GPU, e4m3 design matrix with 32 x 32 UE8M0 block scales, evaluated by ``csrc/glm_fp8.cu``
     (e4m3 wgmma, block scales applied in fp32 registers per 32-deep K step).  Up to 3 chains per launch.
     The residuals of the Poisson and Gaussian families are unbounded, so the kernel scales them too (one
-    power of two per 32-row group and chain).
+    power of two per 32-row group and chain); so are weighted residuals, of any family.  ``offsets`` and
+    ``weights`` are those of :class:`GlmShards`.
     """
 
     def __init__(self, Xqs, scales, ys, *, groups=None, n_groups: int = 1, n_chains: int = 1,
-                 family: str = "logistic", node_ids=None, n_nodes=None) -> None:
+                 family: str = "logistic", node_ids=None, n_nodes=None, offsets=None, weights=None) -> None:
         if not 1 <= n_chains <= 3:
             raise ValueError("the fp8 kernel batches at most 3 chains per launch")
         super().__init__(Xqs, ys, groups=groups, n_groups=n_groups, family=family, n_chains=n_chains, kernel="fp8",
-                         scales=scales, node_ids=node_ids, n_nodes=n_nodes)
+                         scales=scales, node_ids=node_ids, n_nodes=n_nodes, offsets=offsets, weights=weights)
         self._kernel_scales = [pack_tile_scales(s, self.n_features) for s in self.scales]
 
     @classmethod
@@ -396,7 +481,8 @@ class Fp8GlmShards(GlmShards):
         return dequantize_block_fp8(self.Xs[seg][r0:r1], self.scales[seg][r0 // 32 : (r1 + 31) // 32])
 
     def bytes_per_eval(self) -> int:
-        return int(sum(X.shape[0] * (self.n_features + 4) + s.numel() for X, s in zip(self.Xs, self._kernel_scales)))
+        return int(sum(X.shape[0] * (self.n_features + 4) + s.numel() for X, s in zip(self.Xs, self._kernel_scales))) + \
+            self._row_data_bytes()
 
 
 def synth_logistic_shard(n_rows: int, n_features: int, *, seed: int, device, chunk_rows: int = 1 << 20,

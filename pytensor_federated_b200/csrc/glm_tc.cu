@@ -77,7 +77,9 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
 }
 
 // KC = chains per launch; ROWS = some segment has per-row offsets or weights (GlmSegment::offset / weight), so
-// models without them run an instantiation with no trace of the extra loads.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// models without them run an instantiation with no trace of the extra loads; SOFTMAX = the multinomial family
+// (code 3), whose C classes ride along N as "virtual chains": column v = k C + c is class c of chain k, and the
+// columns of one row are coupled only through the log-sum-exp of the epilogue (tc::softmax_loglik).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -100,7 +102,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS>
+template <int KC, bool ROWS, bool SOFTMAX>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -292,6 +294,20 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             for (int i = 0; i < 3; ++i)
 #pragma unroll
                 for (int v = 0; v < N2 / 2; ++v) gacc[i][v] = 0.f;
+            // SOFTMAX: chain and class of this thread's columns v = 8 jc + 2 q + e (chain -1: past K C)
+            int sm_chain[2 * NJ];
+            float sm_cls[2 * NJ];
+            int sm_chains = 0;
+            if constexpr (SOFTMAX) {
+                const int NC = prm.n_classes;
+                sm_chains = nch / NC;
+#pragma unroll
+                for (int s = 0; s < 2 * NJ; ++s) {
+                    const int v = 8 * (s >> 1) + 2 * q + (s & 1);
+                    sm_chain[s] = v < nch ? v / NC : -1;
+                    sm_cls[s] = (float)(v % NC);
+                }
+            }
             Ring stage;
             uint32_t rb = 0;                        // R buffer of the current tile (alternates)
             for (int j = 0;; ++j) {
@@ -354,6 +370,24 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                         } else {
                             y = valid ? __ldg(seg_y + grow) : 0.f;
                         }
+                        // SOFTMAX: the row's log-sum-exp per chain over the quad; every lane takes part, whether its
+                        // row is valid or not (a row past the segment is dropped below, as in the other families)
+                        float sm_ll[2 * NJ], sm_r[2 * NJ];
+                        if constexpr (SOFTMAX) {
+                            float sm_eta[2 * NJ];
+#pragma unroll
+                            for (int s = 0; s < 2 * NJ; ++s) {
+                                const int jc = s >> 1, e = s & 1;
+                                // the intercept table has KC rows but a lane's columns reach 8 NJ - 1 (7 in the
+                                // KC = 4 bucket): a column past K C (chain -1, never used) reads row 0, so the
+                                // index stays inside the table whatever G is
+                                const int k = sm_chain[s] >= 0 ? 8 * jc + 2 * q + e : 0;
+                                sm_eta[s] = ((eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
+                                             eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k * G + seg_group];
+                                sm_ll[s] = sm_r[s] = 0.f;
+                            }
+                            softmax_loglik<2 * NJ, KC / 2>(sm_eta, sm_chain, sm_cls, sm_chains, y, sm_ll, sm_r);
+                        }
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc)
 #pragma unroll
@@ -363,7 +397,15 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
                                 float ll = 0.f, r = 0.f;
                                 if (valid && k < nch) {
-                                    if constexpr (ROWS) {
+                                    if constexpr (SOFTMAX) {
+                                        // weight as in ROWS (offsets are rejected for this family)
+                                        ll = sm_ll[2 * jc + e];
+                                        r = sm_r[2 * jc + e];
+                                        if constexpr (ROWS) {
+                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                        }
+                                    } else if constexpr (ROWS) {
                                         // offset after the intercept, weight after the likelihood, both rounded on their
                                         // own (no FMA contraction): w = 1, o = 0 gives the bits of the plain model; a
                                         // zero weight selects 0, so a masked row's non-finite y or o never reaches a sum
@@ -556,12 +598,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS)                                                                                        \
+#define LAUNCH_TC(KC, ROWS, SOFTMAX)                                                                               \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
                                                  prm->n_groups, KC);                                               \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -572,14 +614,20 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS>, *comm, segs_dev, *prm, maps,                     \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX>, *comm, segs_dev, *prm, maps,            \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
-    if (kc == 1) { if (rows) LAUNCH_TC(1, true); else LAUNCH_TC(1, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true); else LAUNCH_TC(4, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true); else LAUNCH_TC(8, false); }
-    else { if (rows) LAUNCH_TC(16, true); else LAUNCH_TC(16, false); }
+    if (prm->family == 3) {                 // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
+        if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true); else LAUNCH_TC(4, false, true); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true); else LAUNCH_TC(8, false, true); }
+        else { if (rows) LAUNCH_TC(16, true, true); else LAUNCH_TC(16, false, true); }
+    }
+    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false); else LAUNCH_TC(1, false, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false); else LAUNCH_TC(4, false, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false); else LAUNCH_TC(8, false, false); }
+    else { if (rows) LAUNCH_TC(16, true, false); else LAUNCH_TC(16, false, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

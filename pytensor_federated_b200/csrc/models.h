@@ -30,11 +30,14 @@ struct GlmParams {
     int ld;               // row stride of X in elements
     int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain
     int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P])
-    int family;           // 0 = logistic (Bernoulli), 1 = Poisson (log link), 2 = Gaussian (identity, unit variance)
+    int family;           // 0 = logistic (Bernoulli), 1 = Poisson (log link), 2 = Gaussian (identity, unit variance),
+                          // 3 = multinomial (softmax over n_classes columns; tensor-core bf16 kernel only)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)
     int row_data;         // kGlmRowOffsets | kGlmRowWeights when any segment has them: selects the kernel instantiation
+    int n_classes;        // multinomial: C classes per chain, n_chains = K C "virtual chains" (column k C + c is class
+                          // c of chain k; theta row k C + c = (intercept[:, c], beta[:, c]) of chain k); else 1
 };
 
 constexpr int kGlmRowOffsets = 1;

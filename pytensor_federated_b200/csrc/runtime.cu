@@ -550,9 +550,33 @@ int b200_engine_set_linreg(void* h, int n_shards, const void** x, const void** y
 int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y, const void** scales,
                         const long long* n_rows, const int* groups, int n_features, int ld, int n_groups,
                         int n_chains, int family, int use_tensor_cores, const int* out_groups, int n_out,
-                        const float** offsets, const float** weights) {
+                        const float** offsets, const float** weights, int n_classes) {
     Engine* e = static_cast<Engine*>(h);
     CK(cudaSetDevice(e->device));
+    // family 3 (multinomial) exists in the bf16 tensor-core kernel only; the CUDA-core kernels would take an
+    // unknown family code for the Gaussian one, so it must never reach them
+    if (family == 3) {
+        if (use_tensor_cores != 1) {
+            g_last_error = "the multinomial family runs on the bf16 tensor-core kernel only";
+            return -34;
+        }
+        if (n_classes < 2 || n_classes > 16) {
+            g_last_error = "the multinomial family needs 2 <= n_classes <= 16";
+            return -35;
+        }
+        if (n_chains % n_classes != 0) {
+            g_last_error = "the multinomial family needs n_chains = K x n_classes (one column per chain and class)";
+            return -36;
+        }
+        for (int s = 0; s < n_segments && offsets; ++s)
+            if (offsets[s]) {
+                g_last_error = "the multinomial family takes no offsets (one common to all classes cancels)";
+                return -37;
+            }
+    } else if (n_classes != 1) {
+        g_last_error = "n_classes must be 1 for every family but the multinomial one";
+        return -38;
+    }
     const int tile_rows = (use_tensor_cores == 1 || use_tensor_cores == 2) ? 128 : 8;
     e->glm_segs.resize(n_segments);
     long long tiles = 0;
@@ -578,7 +602,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         tiles += (n_rows[s] + tile_rows - 1) / tile_rows;
     }
     e->glm = GlmParams{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
-                       early_loads_enabled() ? 1 : 0, row_data};
+                       early_loads_enabled() ? 1 : 0, row_data, n_classes};
     if ((long long)e->glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
         g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
         return -33;

@@ -221,5 +221,58 @@ __device__ __forceinline__ void link_loglik(int family, float y, float eta, floa
     }
 }
 
+// Multinomial (softmax) likelihood of one row, family 3.  The row's columns are spread over the four lanes of a
+// quad (the lanes sharing lane >> 2); this lane holds NS of them: eta[s] is column s of this lane, chain[s] the
+// chain it belongs to (-1: no chain, i.e. a column past K*C) and cls[s] its class.  Per chain, the row maximum m
+// and s = sum_c exp(eta_c - m) are reduced over the quad with xor-1 / xor-2 butterflies, which every lane runs
+// for every chain below n_chains (a warp-uniform bound): a lane holding no column of a chain contributes -inf / 0.
+// Both butterfly steps add or compare the same two values on both partners, so all four lanes get the same bits.
+// The chain loops only reduce and hand the result to the lane's columns of that chain; the exponentials, logs and
+// reciprocals are evaluated once per column afterwards (NS each, not NS per chain).
+// Results: ll[s] = [y == c] (eta_c - m - log s), r[s] = [y == c] - exp(eta_c - m) / s; |r| <= 1.
+template <int NS, int MAX_CHAINS>
+__device__ __forceinline__ void softmax_loglik(const float (&eta)[NS], const int (&chain)[NS], const float (&cls)[NS],
+                                               int n_chains, float y, float (&ll)[NS], float (&r)[NS]) {
+    float mx[NS], sm[NS];   // row maximum and sum of exponentials of each column's chain
+#pragma unroll
+    for (int s = 0; s < NS; ++s) mx[s] = 0.f, sm[s] = 1.f;
+#pragma unroll
+    for (int k = 0; k < MAX_CHAINS; ++k) {
+        if (k >= n_chains) break;
+        float m = -INFINITY;
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) m = fmaxf(m, eta[s]);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) mx[s] = m;
+    }
+    float ex[NS];
+#pragma unroll
+    for (int s = 0; s < NS; ++s) ex[s] = __expf(eta[s] - mx[s]);
+#pragma unroll
+    for (int k = 0; k < MAX_CHAINS; ++k) {
+        if (k >= n_chains) break;
+        float sum = 0.f;
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) sum += ex[s];
+        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) sm[s] = sum;
+    }
+#pragma unroll
+    for (int s = 0; s < NS; ++s)
+        if (chain[s] >= 0) {
+            const bool hit = y == cls[s];
+            ll[s] = hit ? (eta[s] - mx[s]) - __logf(sm[s]) : 0.f;
+            r[s] = (hit ? 1.f : 0.f) - ex[s] * __fdividef(1.f, sm[s]);
+        }
+}
+
 
 }  // namespace tc

@@ -95,14 +95,17 @@ class NodeFederation:
 
     def _evaluate_glm(self, requests):
         m = self.engine.model
-        G, K = m.n_groups, m.n_chains
+        # multinomial models: intercept (G, C) and beta (P, C) per chain, flattened row-major
+        C = m.n_classes
+        G, K = m.n_groups * C, m.n_chains
+        beta_shape = (m.n_features, C) if m.multinomial else (m.n_features,)
         chains: Dict[bytes, int] = {}      # distinct parameter vector -> chain
         rows: List[np.ndarray] = []
         chain_of: Dict[int, int] = {}
         shapes: Dict[int, tuple] = {}
         for node, (intercept, beta) in requests.items():
             ic = np.asarray(intercept, dtype=np.float32)
-            vec = np.concatenate([ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features)])
+            vec = np.concatenate([ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features * C)])
             key = vec.tobytes()
             if key not in chains:
                 if len(rows) == K:
@@ -115,12 +118,17 @@ class NodeFederation:
             chain_of[node] = chains[key]
             shapes[node] = ic.shape
         theta = np.stack(rows + [rows[0]] * (K - len(rows)))                       # unused chains repeat the first
-        inputs = [theta[:, :G], theta[:, G:]] if K > 1 else [theta[0, :G], theta[0, G:]]
+        if m.multinomial:
+            ic_shape = (m.n_groups, C)
+            inputs = ([theta[:, :G].reshape((K,) + ic_shape), theta[:, G:].reshape((K,) + beta_shape)] if K > 1
+                      else [theta[0, :G].reshape(ic_shape), theta[0, G:].reshape(beta_shape)])
+        else:
+            inputs = [theta[:, :G], theta[:, G:]] if K > 1 else [theta[0, :G], theta[0, G:]]
         per = m.per_node(self.engine.evaluate_raw(inputs))                         # [n_nodes, K, 1 + G + P]
         out = {}
         for node in requests:
             v = per[node, chain_of[node]]
-            out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].copy()])
+            out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].reshape(beta_shape).copy()])
         return out
 
     def evaluate_node(self, node: int, *inputs) -> Tuple[np.ndarray, List[np.ndarray]]:

@@ -1,7 +1,8 @@
 """Model families with fused sm_90a kernels (and eager PyTorch oracles)."""
 from .base import ShardModel
 from .custom import CustomFamily
-from .glm import Fp8GlmShards, GlmShards, dequantize_block_fp8, quantize_block_fp8, synth_logistic_shard, synth_logistic_shard_fp8
+from .glm import (Fp8GlmShards, GlmShards, dequantize_block_fp8, quantize_block_fp8, synth_logistic_shard,
+                  synth_logistic_shard_fp8, synth_multinomial_shard)
 from .linreg import LinregShards, make_demo_data
 from .ode import LOTKA_VOLTERRA, OdeShards, OdeSystem, synth_lv_shard, synth_ode_shard
 
@@ -16,6 +17,7 @@ __all__ = [
     "dequantize_block_fp8",
     "synth_logistic_shard",
     "synth_logistic_shard_fp8",
+    "synth_multinomial_shard",
     "OdeShards",
     "OdeSystem",
     "LOTKA_VOLTERRA",

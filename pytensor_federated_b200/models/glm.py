@@ -16,7 +16,7 @@ import numpy as np
 
 from .base import ShardModel
 
-FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2}
+FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3}
 
 
 def _family_code(family) -> int:
@@ -63,6 +63,25 @@ class GlmShards(ShardModel):
         finite and >= 0, offsets finite wherever the weight is not 0.  ``w = 1, o = 0`` reproduces the plain
         model bit for bit on the ``tc``, ``simt`` and general-shape kernels.  The kernels read the tensors given
         here on every evaluation, as they read X and y.
+    family, n_classes
+        ``"logistic"``, ``"poisson"``, ``"gaussian"``, a :class:`CustomFamily`, or ``"multinomial"`` with
+        ``n_classes=C``: softmax (categorical) regression over C classes.  ``ys`` then holds class labels
+        ``0 .. C-1`` (stored as float32, so exact up to 2^24); every row of non-zero weight must carry an integer
+        label in ``[0, C)``, a row of weight 0 may carry anything.  The inputs per call are ``intercept[G, C]`` (also
+        ``[C]`` when G = 1) and ``beta[P, C]``, batched ``[K, G, C]`` and ``[K, P, C]``; gradients come back in the
+        shapes of the inputs, and
+
+            eta_ic = intercept[group, c] + x_i' beta[:, c],     LL = sum_i w_i (eta_{i, y_i} - logsumexp_c eta_ic).
+
+        ``2 <= C <= 16`` and ``K * C <= 16``.  Only the bf16 tensor-core kernel evaluates this family (bf16 X,
+        P % 8 == 0, 8 <= P <= 384, 16-byte aligned rows): ``kernel="simt"`` / ``"generic"``, :class:`Fp8GlmShards`
+        and shapes outside these raise a ValueError, and so do ``offsets`` (an offset common to all classes
+        cancels in the softmax).  The kernel runs the C classes of chain k as columns ``k C + c`` of a K C-chain
+        launch, so a C-class model reads X once, like a C-chain logistic one.
+
+        This full parameterisation is not identified without priors: adding one vector to every class column of
+        ``(intercept, beta)`` leaves LL unchanged (its gradients sum to 0 over the classes).  A reference-category
+        model is obtained by fixing one column (say class 0) at 0 and ignoring its gradient.
     """
 
     def __init__(
@@ -80,6 +99,7 @@ class GlmShards(ShardModel):
         n_nodes: Optional[int] = None,
         offsets: Optional[Sequence] = None,
         weights: Optional[Sequence] = None,
+        n_classes: Optional[int] = None,
     ) -> None:
         import torch
 
@@ -121,6 +141,41 @@ class GlmShards(ShardModel):
         if self.node_ids is not None and (len(self.node_ids) != len(self.Xs) or not all(0 <= i < self.n_nodes for i in self.node_ids)):
             raise ValueError("node_ids needs one node index in [0, n_nodes) per segment")
         self.n_vals = self.n_nodes * self.n_chains * (1 + self.n_params)
+        #: classes per chain (multinomial family; 1 for every other family)
+        self.n_classes = 1
+        self.multinomial = isinstance(family, str) and family == "multinomial"
+        if self.multinomial:
+            self._init_multinomial(n_classes)
+        elif n_classes is not None:
+            raise ValueError("n_classes is for family='multinomial' only")
+
+    def _init_multinomial(self, n_classes) -> None:
+        """Checks of the multinomial family, then its sizes: C (G + P) parameters per chain, and the kernel's
+        output of K C virtual chains (one ``[LL, gi[G], g[P]]`` block per chain and class)."""
+        import torch
+
+        if self.kernel not in ("auto", "tc"):
+            raise ValueError(f"kernel={self.kernel!r}: the multinomial family runs on the bf16 tensor-core kernel only "
+                             "(kernel='tc' or 'auto')")
+        if n_classes is None or not 2 <= int(n_classes) <= 16:
+            raise ValueError(f"the multinomial family needs n_classes in [2, 16], got {n_classes}")
+        C = int(n_classes)
+        if self.n_chains * C > 16:
+            raise ValueError(f"n_chains x n_classes must be <= 16 (the tensor-core kernel's columns per launch), got "
+                             f"{self.n_chains} x {C}")
+        if any(o is not None for o in self.offsets):
+            raise ValueError("offsets are not supported by the multinomial family: an offset common to all classes "
+                             "cancels in the softmax")
+        for si, (y, w) in enumerate(zip(self.ys, self.weights)):
+            bad = ~((y == torch.floor(y)) & (y >= 0) & (y < C))   # NaN fails every comparison
+            if w is not None:
+                bad &= w != 0   # a masked row may carry anything
+            if bool(torch.any(bad)):
+                raise ValueError(f"labels of segment {si} must be integers in [0, {C}) on every row of non-zero weight")
+        self.n_classes = C
+        self.n_params = C * (self.n_groups + self.n_features)
+        self.n_theta_words = self.n_chains * self.n_params
+        self.n_vals = self.n_nodes * self.n_chains * C * (1 + self.n_groups + self.n_features)
 
     def _row_data(self, entries, name: str) -> list:
         """One contiguous float32 tensor (or None) per segment, on the device of the segment's X."""
@@ -157,13 +212,16 @@ class GlmShards(ShardModel):
 
     # -- packing ---------------------------------------------------------------------------
     def call_context(self, inputs):
-        """``(batched, intercept shape)`` of one call: a 2-D ``beta`` means one row per chain."""
+        """``(batched, intercept shape)`` of one call: a 2-D ``beta`` means one row per chain (multinomial: a 3-D
+        ``beta[K, P, C]``)."""
         intercept, beta = inputs
-        return (np.ndim(beta) == 2, np.shape(intercept))
+        return (np.ndim(beta) == (3 if self.multinomial else 2), np.shape(intercept))
 
     _pack_views = None
 
     def pack_theta(self, inputs, out: np.ndarray):
+        if self.multinomial:
+            return self._pack_theta_multinomial(inputs, out)
         intercept, beta = inputs
         views = self._pack_views
         if views is None or views[0] is not out:
@@ -180,6 +238,22 @@ class GlmShards(ShardModel):
         views[2][...] = bt.reshape(self.n_chains, self.n_features)
         return ctx
 
+    def _pack_theta_multinomial(self, inputs, out: np.ndarray):
+        """Theta words as ``[K C][G + P]``: row ``k C + c`` is ``(intercept[:, c], beta[:, c])`` of chain k, the
+        kernel's virtual chain of class c."""
+        intercept, beta = inputs
+        K, C, G, P = self.n_chains, self.n_classes, self.n_groups, self.n_features
+        views = self._pack_views
+        if views is None or views[0] is not out:
+            th = out.view(np.float32).reshape(K, C, G + P)
+            views = self._pack_views = (out, th[:, :, :G], th[:, :, G:])
+        ic, bt = np.asarray(intercept), np.asarray(beta)
+        ctx = (bt.ndim == 3, ic.shape)
+        self._batched, self._icpt_shape = ctx
+        views[1][...] = ic.reshape(K, G, C).transpose(0, 2, 1)
+        views[2][...] = bt.reshape(K, P, C).transpose(0, 2, 1)
+        return ctx
+
     _batched = False
     _icpt_shape = ()
 
@@ -191,10 +265,20 @@ class GlmShards(ShardModel):
         return ctx
 
     def per_node(self, vals: np.ndarray) -> np.ndarray:
-        """The reduced vector as ``[n_nodes, n_chains, 1 + G + P]`` (``[LL, d intercepts, d beta]`` per block)."""
+        """The reduced vector as ``[n_nodes, n_chains, 1 + G + P]`` (``[LL, d intercepts, d beta]`` per block).
+        Multinomial: ``[n_nodes, n_chains, 1 + G C + P C]``, ``[LL, d intercept (G, C), d beta (P, C)]`` with the
+        matrices row-major, summed from the kernel's blocks of the chain's C classes."""
+        if self.multinomial:
+            n, K, C, G = self.n_nodes, self.n_chains, self.n_classes, self.n_groups
+            raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C, 1 + G + self.n_features)
+            return np.concatenate([raw[..., 0].sum(axis=2)[..., None],
+                                   raw[..., 1 : 1 + G].transpose(0, 1, 3, 2).reshape(n, K, G * C),
+                                   raw[..., 1 + G :].transpose(0, 1, 3, 2).reshape(n, K, self.n_features * C)], axis=2)
         return np.asarray(vals, dtype=np.float64).reshape(self.n_nodes, self.n_chains, 1 + self.n_params)
 
     def unpack_result(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
+        if self.multinomial:
+            return self._unpack_multinomial(vals, ctx)
         v = self.per_node(vals).sum(axis=0) if self.n_nodes > 1 else np.asarray(vals, dtype=np.float64).reshape(self.n_chains, 1 + self.n_params)
         G = self.n_groups
         batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
@@ -202,6 +286,17 @@ class GlmShards(ShardModel):
             return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
                     v[:, 1 + G :].copy()]
         return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G :].copy()]
+
+    def _unpack_multinomial(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
+        v = self.per_node(vals).sum(axis=0)                         # [K, 1 + G C + P C]
+        K, GC, PC = self.n_chains, self.n_groups * self.n_classes, self.n_features * self.n_classes
+        batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
+        beta_shape = (self.n_features, self.n_classes)
+        if batched:
+            return [v[:, 0].copy(), v[:, 1 : 1 + GC].reshape((K,) + tuple(icpt_shape[1:])).copy(),
+                    v[:, 1 + GC : 1 + GC + PC].reshape((K,) + beta_shape).copy()]
+        return [np.asarray(v[0, 0]), v[0, 1 : 1 + GC].reshape(icpt_shape).copy(),
+                v[0, 1 + GC : 1 + GC + PC].reshape(beta_shape).copy()]
 
     # -- native ----------------------------------------------------------------------------
     def use_tensor_cores(self):
@@ -214,6 +309,13 @@ class GlmShards(ShardModel):
             if X0.dtype not in (torch.bfloat16, torch.float32) or self.n_chains != 1 or self.n_features > 1024:
                 raise ValueError("custom likelihoods need a bf16/fp32 design matrix, one chain and P <= 1024")
             return 3 if X0.dtype == torch.bfloat16 else 4
+        if self.multinomial:   # the bf16 tensor-core kernel or nothing: no other kernel has this family
+            if not (X0.dtype == torch.bfloat16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384
+                    and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0):
+                raise ValueError(f"the multinomial family runs on the bf16 tensor-core kernel only, which needs a bf16 "
+                                 f"design matrix with P % 8 == 0, 8 <= P <= 384 and 16-byte aligned rows (got "
+                                 f"{X0.dtype}, P = {self.n_features}, row stride {self.ld})")
+            return 1
         if self.kernel == "fp8":
             return 2
         if self.kernel == "tc":
@@ -271,7 +373,8 @@ class GlmShards(ShardModel):
         native.check(
             lib.b200_engine_set_glm(
                 handle, n, Xp, yp, sp, rows, grp, self.n_features, self.ld, self.n_groups,
-                self.n_chains, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
+                self.n_chains * self.n_classes, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
+                self.n_classes,
             ),
             "set_glm",
         )
@@ -286,6 +389,8 @@ class GlmShards(ShardModel):
         import torch
 
         dtype = dtype or torch.float32
+        if self.multinomial:
+            return self._multinomial_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(self.n_chains, -1)
@@ -331,9 +436,50 @@ class GlmShards(ShardModel):
         w = self.weights[seg]
         if w is None:
             return ll, r
-        ww = w[r0:r1].to(ll.dtype).unsqueeze(1)
+        ww = w[r0:r1].to(ll.dtype).reshape((-1,) + (1,) * (ll.dim() - 1))   # broadcast over chains (and classes)
         keep = ww != 0
         return torch.where(keep, ww * ll, torch.zeros_like(ll)), torch.where(keep, ww * r, torch.zeros_like(r))
+
+    def _multinomial_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
+        """The multinomial family's partial in the kernel's layout ``[n_nodes][K C][1 + G + P]`` (block ``k C + c``:
+        ``[LL_kc, gi_kc[G], g_kc[P]]`` with ``LL_kc = sum_i w_i [y_i == c] log_softmax(eta_i)_c``,
+        ``r_ikc = [y_i == c] - softmax(eta_i)_c``).  ``bf16_gemms``: the collective baseline, two bf16 GEMMs
+        with ``beta`` as ``[P, K C]`` and fp32 elementwise work; else the oracle in ``dtype``."""
+        import torch
+
+        intercept, beta = inputs
+        self._note_shapes(inputs)
+        K, C, G, P = self.n_chains, self.n_classes, self.n_groups, self.n_features
+        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G, C).to(self.device, dtype)
+        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P, C)
+        B = bt.permute(1, 0, 2).reshape(P, K * C).to(self.device, torch.bfloat16 if bf16_gemms else dtype)   # column k C + c
+        full = torch.zeros(self.n_nodes, K * C, 1 + G + P, dtype=torch.float64, device=self.device)
+        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
+            out = full[self.node_ids[si] if self.node_ids is not None else 0]
+            w = self.weights[si]
+            for r0 in range(0, X.shape[0], chunk_rows):
+                r1 = min(X.shape[0], r0 + chunk_rows)
+                if bf16_gemms:
+                    Xf = X[r0:r1]
+                    eta = (Xf @ B).to(dtype)
+                else:
+                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
+                    eta = Xf @ B
+                n = r1 - r0
+                eta = eta.reshape(n, K, C) + ic[:, g, :]
+                lab = y[r0:r1]
+                if w is not None:   # masked rows may carry NaN or out-of-range labels: any valid class will do
+                    lab = torch.where(w[r0:r1] != 0, lab, torch.zeros_like(lab))
+                hit = torch.nn.functional.one_hot(lab.long(), C).bool().unsqueeze(1)   # [n, 1, C]
+                logp = torch.log_softmax(eta, dim=-1)
+                ll = torch.where(hit, logp, torch.zeros_like(logp))
+                r = hit.to(dtype) - torch.exp(logp)
+                ll, r = self._weigh(si, r0, r1, ll, r)
+                out[:, 0] += ll.double().sum(0).reshape(K * C)
+                out[:, 1 + g] += r.double().sum(0).reshape(K * C)
+                rT = r.reshape(n, K * C).T
+                out[:, 1 + G :] += (rT.to(torch.bfloat16) @ Xf if bf16_gemms else rT @ Xf).double()
+        return full.reshape(-1).cpu().numpy()
 
     def _dequant_rows(self, seg: int, r0: int, r1: int):
         """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
@@ -350,6 +496,8 @@ class GlmShards(ShardModel):
 
         if self.Xs[0].dtype != torch.bfloat16:
             return self.reference_partial(inputs)
+        if self.multinomial:
+            return self._multinomial_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float32)).reshape(self.n_chains, -1).to(self.device)
@@ -385,7 +533,7 @@ class GlmShards(ShardModel):
         return int(sum(X.shape[0] * (self.n_features * X.element_size() + 4) for X in self.Xs)) + self._row_data_bytes()
 
     def flops_per_eval(self) -> int:
-        return int(4 * self.n_rows * self.n_features * self.n_chains)
+        return int(4 * self.n_rows * self.n_features * self.n_chains * self.n_classes)
 
 
 def quantize_block_fp8(X, block: int = 32):
@@ -502,6 +650,27 @@ def synth_logistic_shard(n_rows: int, n_features: int, *, seed: int, device, chu
         X[r0:r1] = xb
         p = torch.sigmoid(xb.float() @ beta_true + 0.3)
         y[r0:r1] = (torch.rand(r1 - r0, generator=gen, device=device) < p).float()
+    return X, y, beta_true
+
+
+def synth_multinomial_shard(n_rows: int, n_features: int, n_classes: int, *, seed: int, device,
+                            chunk_rows: int = 1 << 20, beta_scale: float = 0.05):
+    """Synthetic softmax-regression shard generated on the device in chunks (bf16 ``X ~ N(0,1)``,
+    ``y ~ Categorical(softmax(X beta* + b*))`` as float32 labels ``0 .. C-1``).  Returns ``(X, y, beta* [P, C])``."""
+    import torch
+
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, n_classes, generator=gen, device=device) * beta_scale).float()
+    b_true = (torch.randn(n_classes, generator=gen, device=device) * 0.3).float()
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        p = torch.softmax(xb.float() @ beta_true + b_true, dim=1)
+        y[r0:r1] = torch.multinomial(p, 1, generator=gen).squeeze(1).float()
     return X, y, beta_true
 
 

@@ -516,6 +516,13 @@ def default_inputs_from_words(model: ShardModel, words: np.ndarray):
     if isinstance(model, LinregShards):
         th = words.view(np.float64).reshape(model.n_shards_total, 2)
         return th[:, 0].copy(), th[:, 1].copy()
+    if isinstance(model, GlmShards) and model.multinomial:
+        # words [K C][G + P] (row k C + c: class c of chain k) -> intercept [K, G, C], beta [K, P, C]
+        th = words.view(np.float32).reshape(model.n_chains, model.n_classes, model.n_groups + model.n_features)
+        ic, bt = th[:, :, : model.n_groups].transpose(0, 2, 1), th[:, :, model.n_groups :].transpose(0, 2, 1)
+        if model.n_chains == 1:
+            return ic[0].copy(), bt[0].copy()
+        return ic.copy(), bt.copy()
     if isinstance(model, GlmShards):
         th = words.view(np.float32).reshape(model.n_chains, model.n_params)
         if model.n_chains == 1:

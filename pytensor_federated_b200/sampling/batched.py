@@ -161,11 +161,23 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
     Any number of chains may be passed: the kernel's capacity per launch is ``K`` (at most 16 for the bf16
     tensor-core kernel, 3 for the fp8 kernel); more chains are evaluated in ``ceil(chains / K)`` launches and a
     short last tile is padded by repeating its last chain, so 64 chains on a K = 16 engine cost four passes over the
-    data instead of sixty-four."""
+    data instead of sixty-four.
+
+    A multinomial engine (``family="multinomial"``, C classes) takes ``theta = [intercept (G, C), beta (P, C)]`` per
+    chain, both flattened row-major."""
     cap = int(getattr(engine.model, "n_chains", 1))
+    n_classes = int(getattr(engine.model, "n_classes", 1)) if getattr(engine.model, "multinomial", False) else 1
+    split = n_groups * n_classes   # theta columns that are intercepts
+
+    def shaped(ic: np.ndarray, beta: np.ndarray):
+        """Inputs of ``engine.evaluate``; ``ic`` / ``beta`` have the chains (if any) in their leading axis."""
+        if n_classes == 1:
+            return ic, beta
+        lead = ic.shape[:-1]
+        return ic.reshape(lead + (n_groups, n_classes)), beta.reshape(lead + (-1, n_classes))
 
     def tile(theta: np.ndarray):
-        logp, d_ic, d_beta = engine.evaluate(theta[:, :n_groups], theta[:, n_groups:])
+        logp, d_ic, d_beta = engine.evaluate(*shaped(theta[:, :split], theta[:, split:]))
         return np.asarray(logp).reshape(-1), np.concatenate([np.asarray(d_ic).reshape(cap, -1), np.asarray(d_beta).reshape(cap, -1)], axis=1)
 
     def fn(theta: np.ndarray):
@@ -180,8 +192,8 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
             if k < cap:
                 block = np.concatenate([block, np.repeat(block[-1:], cap - k, axis=0)], axis=0)
             if cap == 1:   # single-chain engines take unbatched inputs
-                logp, d_ic, d_beta = engine.evaluate(block[0, :n_groups], block[0, n_groups:])
-                lp, gr = np.asarray(logp).reshape(1), np.concatenate([np.asarray(d_ic).reshape(-1), np.asarray(d_beta)])[None]
+                logp, d_ic, d_beta = engine.evaluate(*shaped(block[0, :split], block[0, split:]))
+                lp, gr = np.asarray(logp).reshape(1), np.concatenate([np.asarray(d_ic).reshape(-1), np.asarray(d_beta).reshape(-1)])[None]
             else:
                 lp, gr = tile(block)
             logps.append(lp[:k])

@@ -79,7 +79,11 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
 // KC = chains per launch; ROWS = some segment has per-row offsets or weights (GlmSegment::offset / weight), so
 // models without them run an instantiation with no trace of the extra loads; SOFTMAX = the multinomial family
 // (code 3), whose C classes ride along N as "virtual chains": column v = k C + c is class c of chain k, and the
-// columns of one row are coupled only through the log-sum-exp of the epilogue (tc::softmax_loglik).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// columns of one row are coupled only through the log-sum-exp of the epilogue (tc::softmax_loglik); DISP = a family
+// with a learned dispersion parameter (codes 4 and 5, tc::gaussian_scale_loglik / tc::negbin_loglik): theta rows
+// have stride G + P + 1, the intercept table is followed by kDispWords per-chain constants, the epilogue produces a
+// third per-row value q = dll/dlog_dispersion next to ll and r, and each chain's output block is
+// [LL, gi[G], g[P], dlog_dispersion].  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -89,10 +93,10 @@ struct Cfg {
 };
 
 // doubles per CTA row of the partial array: (hi, lo) pairs of the n_vals outputs, then the per-warp slots of
-// the values that a whole warp contributes to — [kLLRows][n_out][KC][1 + G]: log-likelihood and the G
-// intercept gradients of every (output block, chain)
-__host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int n_out, int n_groups) {
-    return 2 * ((size_t)n_vals + (size_t)kLLRows * n_out * kc * (1 + n_groups));
+// the values that a whole warp contributes to — [kLLRows][n_out][KC][1 + G + disp]: log-likelihood, the G
+// intercept gradients and (disp = 1: families with a dispersion parameter) its gradient, of every (output block, chain)
+__host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int n_out, int n_groups, int disp = 0) {
+    return 2 * ((size_t)n_vals + (size_t)kLLRows * n_out * kc * (1 + n_groups + disp));
 }
 
 // Work is handed out in CHUNKS of consecutive tiles of one segment (host-built table: 32 tiles while much
@@ -102,7 +106,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS, bool SOFTMAX>
+template <int KC, bool ROWS, bool SOFTMAX, bool DISP>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -119,15 +123,17 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                       // Theta rows are zero and their gradient rows are never stored
     const int G = prm.n_groups;
     const int panels = PP / kPanel;
-    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, G, KC);
+    // DISP: the intercept table [KC][G] is followed by the per-chain dispersion constants [KC][kDispWords]
+    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, G + (DISP ? kDispWords : 0), KC);
     const int S = (int)L.stages;
     const int nch = prm.n_chains < KC ? prm.n_chains : KC;  // chains actually present in theta
-    const int NV1 = 1 + G + P;        // outputs per chain: [LL, gi[G], g[P]]
+    const int NV1 = 1 + G + P + DISP; // outputs per chain: [LL, gi[G], g[P]] (DISP: and dlog_dispersion)
 
     unsigned char* theta_b = smem + L.off_theta_b;
     unsigned char* r_buf = smem + L.off_r;
     float* theta_f = reinterpret_cast<float*>(smem + L.off_theta_f);  // valid until the setup barrier only
     float* icpt = reinterpret_cast<float*>(smem + L.off_icpt);        // [KC][G] intercepts
+    float* disp = icpt + KC * G;                                        // DISP: [KC][kDispWords] per-chain constants
     int4* ring = reinterpret_cast<int4*>(smem + L.off_ring);          // (segment or -1, first row, tiles, -)
     uint64_t* bar_ring = reinterpret_cast<uint64_t*>(smem + L.off_ring + kRing * 16);   // slot j % kRing: chunk j published
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
@@ -177,16 +183,19 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     fed::Prologue pro = fed::prologue(comm, theta_f);   // contains __syncthreads()
     const bool active = !pro.stop && !pro.timed_out;
     const int NOUT = prm.n_out;       // output blocks (1 = everything summed; else one per node)
-    const int NS1 = 1 + G;            // warp-level values per (block, chain): LL and the G intercept gradients
-    const size_t row_doubles = partial_row_doubles(comm.n_vals, KC, NOUT, G);
+    const int NS1 = 1 + G + DISP;     // warp-level values per (block, chain): LL, the G intercept gradients (and q)
+    const size_t row_doubles = partial_row_doubles(comm.n_vals, KC, NOUT, G, DISP);
     double* out = comm.cta_partials + (size_t)blockIdx.x * row_doubles;   // this CTA's running sums, (hi, lo) pairs
-    double* ll_slots = out + 2 * (size_t)comm.n_vals;                     // [kLLRows][NOUT][KC][1 + G] pairs
+    double* ll_slots = out + 2 * (size_t)comm.n_vals;                     // [kLLRows][NOUT][KC][NS1] pairs
 
     if (active) {
         // ---------------- theta-dependent setup --------------------------------------------------
         for (size_t i = threadIdx.x; i < row_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
-            icpt[i] = (i / G) < nch ? theta_f[(i / G) * (G + P) + (i % G)] : 0.f;
+            icpt[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
+        if constexpr (DISP)
+            for (int k = threadIdx.x; k < KC; k += blockDim.x)
+                dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = term * C8 + chain
         for (int idx = threadIdx.x; idx < panels * N1 * 8; idx += blockDim.x) {
             const int j = idx & 7;              // 16-byte chunk (8 features) within the 128-byte row
@@ -198,7 +207,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                 for (int e = 0; e < 8; ++e) {
                     const int f = pnl * kPanel + j * 8 + e;
-                    const float v = f < P ? theta_f[chain * (G + P) + G + f] : 0.f;
+                    const float v = f < P ? theta_f[chain * (G + P + DISP) + G + f] : 0.f;
                     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
                     const float rem1 = v - __bfloat162float(hi);
                     const __nv_bfloat16 mid = __float2bfloat16_rn(rem1);
@@ -319,9 +328,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 const long long seg_rows = segs_g[ch.x].n_rows;
                 const int seg_group = segs_g[ch.x].group;
                 const int og = segs_g[ch.x].out_group;               // output block of this chunk's segment
-                float ll_acc[2 * NJ], gi_acc[2 * NJ];
+                float ll_acc[2 * NJ], gi_acc[2 * NJ], ds_acc[2 * NJ];   // ds: DISP only (dll/dlog_dispersion)
 #pragma unroll
-                for (int s = 0; s < 2 * NJ; ++s) ll_acc[s] = gi_acc[s] = 0.f;
+                for (int s = 0; s < 2 * NJ; ++s) ll_acc[s] = gi_acc[s] = ds_acc[s] = 0.f;
                 for (int t = 0; t < ch.z; ++t) {
                     // row data: y, offset and weight of this thread's two rows, loaded before the tile is waited for
                     // and MMA #1 runs, so three dependent global reads do not sit between the two GEMMs
@@ -395,9 +404,21 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 const int k = 8 * jc + 2 * q + e;
                                 const float eta = (eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
-                                float ll = 0.f, r = 0.f;
+                                float ll = 0.f, r = 0.f, dq = 0.f;
                                 if (valid && k < nch) {
-                                    if constexpr (SOFTMAX) {
+                                    if constexpr (DISP) {
+                                        // offset and weight as in ROWS, the weight applied to all three values
+                                        float et = eta + icpt[k * G + seg_group];
+                                        if constexpr (ROWS) et = __fadd_rn(et, o);
+                                        const float* dt = disp + k * kDispWords;   // k < nch <= KC: inside the table
+                                        if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
+                                        else negbin_loglik(y, et, dt, ll, r, dq);
+                                        if constexpr (ROWS) {
+                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                            dq = wt == 0.f ? 0.f : __fmul_rn(wt, dq);
+                                        }
+                                    } else if constexpr (SOFTMAX) {
                                         // weight as in ROWS (offsets are rejected for this family)
                                         ll = sm_ll[2 * jc + e];
                                         r = sm_r[2 * jc + e];
@@ -418,6 +439,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 }
                                 ll_acc[2 * jc + e] += ll;
                                 gi_acc[2 * jc + e] += r;
+                                if constexpr (DISP) ds_acc[2 * jc + e] += dq;
                                 if (k < N2 / 2) {
                                     const __nv_bfloat16 hi = __float2bfloat16_rn(r);
                                     const __nv_bfloat16 lo = __float2bfloat16_rn(r - __bfloat162float(hi));
@@ -456,17 +478,19 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 // chunk only.
 #pragma unroll
                 for (int s = 0; s < 2 * NJ; ++s) {
-                    double lsum = (double)ll_acc[s], gsum = (double)gi_acc[s];
+                    double lsum = (double)ll_acc[s], gsum = (double)gi_acc[s], dsum = (double)ds_acc[s];
 #pragma unroll
                     for (int o = 4; o < 32; o <<= 1) {
                         lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
                         gsum += __shfl_xor_sync(0xffffffffu, gsum, o);
+                        if constexpr (DISP) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
                     }
                     const int k = 8 * (s >> 1) + 2 * q + (s & 1);
                     if (lane < 4 && k < nch) {
                         double* slot = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KC + k) * NS1);
                         dd_accumulate(slot, lsum);
                         dd_accumulate(slot + 2 * (1 + seg_group), gsum);
+                        if constexpr (DISP) dd_accumulate(slot + 2 * (1 + G), dsum);
                     }
                 }
                 // gradient: feature f = 64 (c NB + i) + 16 w + lane / 4 + 8 h, chain k = 4 jn + q, (hi, lo) adjacent
@@ -491,8 +515,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         __syncthreads();
         fed::pdl_trigger();   // the next evaluation's CTA may take this SM as soon as we exit
         if (threadIdx.x == 0) fed::stamp(comm, 5);
-        // layout per (output block, chain): [LL, gi[G], g[P]] as (hi, lo) pairs; g[] was accumulated in place,
-        // LL and gi[] are the per-warp slots summed in warp order
+        // layout per (output block, chain): [LL, gi[G], g[P]] as (hi, lo) pairs (DISP: then dlog_dispersion);
+        // g[] was accumulated in place, LL, gi[] (and dlog_dispersion) are the per-warp slots summed in warp order
         for (int i = threadIdx.x; i < NOUT * nch * NS1; i += blockDim.x) {
             const int j = i % NS1, k = (i / NS1) % nch, o = i / (NS1 * nch);
             double hi = 0.0, lo = 0.0;
@@ -500,8 +524,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 const double* slot = ll_slots + 2 * ((((size_t)w * NOUT + o) * KC + k) * NS1 + j);
                 fed::dd_add(hi, lo, slot[0], slot[1]);
             }
-            out[2 * (((size_t)o * nch + k) * NV1 + j)] = hi;
-            out[2 * (((size_t)o * nch + k) * NV1 + j) + 1] = lo;
+            const int jo = (DISP && j == 1 + G) ? 1 + G + P : j;   // slot 1 + G: the last value of the block
+            out[2 * (((size_t)o * nch + k) * NV1 + jo)] = hi;
+            out[2 * (((size_t)o * nch + k) * NV1 + jo) + 1] = lo;
         }
         if (threadIdx.x == 0) fed::stamp(comm, 6);
     } else if (warp == 0) {
@@ -588,8 +613,9 @@ extern "C" int b200_glm_tc_chunk_table(const long long* n_rows, int n_segments, 
 }
 
 // doubles in the partial array of the tensor-core kernel: one row of (hi, lo) pairs + per-warp LL slots per CTA
-extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups) {
-    return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups);
+// (dispersion = 1: families 4 and 5, whose slots also hold dlog_dispersion)
+extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int dispersion) {
+    return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups, dispersion ? 1 : 0);
 }
 
 extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps,
@@ -598,12 +624,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS, SOFTMAX)                                                                               \
+#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP)                                                                         \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
-                                                 prm->n_groups, KC);                                               \
+                                                 prm->n_groups + (DISP ? tc::kDispWords : 0), KC);                 \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -614,20 +640,27 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX>, *comm, segs_dev, *prm, maps,            \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP>, *comm, segs_dev, *prm, maps,            \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
     if (prm->family == 3) {                 // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
         if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true); else LAUNCH_TC(4, false, true); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true); else LAUNCH_TC(8, false, true); }
-        else { if (rows) LAUNCH_TC(16, true, true); else LAUNCH_TC(16, false, true); }
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false); else LAUNCH_TC(4, false, true, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false); else LAUNCH_TC(8, false, true, false); }
+        else { if (rows) LAUNCH_TC(16, true, true, false); else LAUNCH_TC(16, false, true, false); }
     }
-    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false); else LAUNCH_TC(1, false, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false); else LAUNCH_TC(4, false, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false); else LAUNCH_TC(8, false, false); }
-    else { if (rows) LAUNCH_TC(16, true, false); else LAUNCH_TC(16, false, false); }
+    else if (prm->family == 4 || prm->family == 5) {   // learned dispersion: theta rows [G + P + 1]
+        if (prm->n_classes != 1) return -3;
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true); else LAUNCH_TC(1, false, false, true); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true); else LAUNCH_TC(4, false, false, true); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true); else LAUNCH_TC(8, false, false, true); }
+        else { if (rows) LAUNCH_TC(16, true, false, true); else LAUNCH_TC(16, false, false, true); }
+    }
+    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false); else LAUNCH_TC(1, false, false, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false); else LAUNCH_TC(4, false, false, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false); else LAUNCH_TC(8, false, false, false); }
+    else { if (rows) LAUNCH_TC(16, true, false, false); else LAUNCH_TC(16, false, false, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

@@ -44,7 +44,7 @@ int b200_launch_glm_tc(const FedComm*, const GlmSegment*, const GlmParams*, cons
                        int n_chunks, unsigned int* work_counter, int grid, cudaStream_t);
 int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count, void** tmaps_dev,
                         void** chunks_dev, int* n_chunks);
-size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups);
+size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int dispersion);
 int b200_launch_ode(const FedComm*, const OdeShard*, int, int, cudaStream_t);
 int b200_launch_glm_fp8(const FedComm*, const GlmSegment*, const GlmParams*, const void* tmaps, const void* chunks,
                         int n_chunks, unsigned int* work_counter, int grid, cudaStream_t stream);
@@ -577,6 +577,19 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         g_last_error = "n_classes must be 1 for every family but the multinomial one";
         return -38;
     }
+    // families 4 and 5 (Gaussian with unknown scale, negative binomial) carry a log-dispersion parameter after
+    // beta; like family 3 they exist in the bf16 tensor-core kernel only
+    const bool dispersion = family == 4 || family == 5;
+    if (dispersion && use_tensor_cores != 1) {
+        g_last_error = family == 4 ? "the gaussian_scale family runs on the bf16 tensor-core kernel only"
+                                   : "the negative_binomial family runs on the bf16 tensor-core kernel only";
+        return -39;
+    }
+    // checked before any engine state changes, so a refused call leaves the engine's model as it was
+    if (dispersion && (long long)(n_out > 0 ? n_out : 1) * n_chains * (2 + n_groups + n_features) != e->n_vals) {
+        g_last_error = "n_vals does not match n_out x n_chains x (2 + n_groups + n_features)";
+        return -33;
+    }
     const int tile_rows = (use_tensor_cores == 1 || use_tensor_cores == 2) ? 128 : 8;
     e->glm_segs.resize(n_segments);
     long long tiles = 0;
@@ -603,7 +616,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
     }
     e->glm = GlmParams{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
                        early_loads_enabled() ? 1 : 0, row_data, n_classes};
-    if ((long long)e->glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
+    if (!dispersion && (long long)e->glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
         g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
         return -33;
     }
@@ -636,7 +649,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
             g_last_error = "tensor-core GLM path rejected this shape (rc=" + std::to_string(rc) + ")";
             return rc;
         }
-        e->tc_row_doubles = b200_glm_tc_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups);
+        e->tc_row_doubles = b200_glm_tc_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups, dispersion ? 1 : 0);
         if (e->tc_partials) cudaFree(e->tc_partials);
         const size_t tc_doubles = (size_t)e->sm_count * e->tc_row_doubles + ((size_t)e->sm_count / 16 + 2) * e->n_vals * 2;
         CK(cudaMalloc((void**)&e->tc_partials, tc_doubles * 8));

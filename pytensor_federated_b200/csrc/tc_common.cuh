@@ -274,5 +274,124 @@ __device__ __forceinline__ void softmax_loglik(const float (&eta)[NS], const int
         }
 }
 
+// Families with a learned dispersion parameter: theta per chain is [intercept[G], beta[P], log_dispersion], and
+// the per-chain constants below, derived from log_dispersion at setup (in double), sit in a table of kDispWords
+// floats per chain behind the intercepts.
+//   family 4, Gaussian with unknown scale, s = log sigma:   ll = -(d / sigma)^2 / 2 - s - log(2 pi) / 2,  d = y - eta
+//   family 5, negative binomial (NB2), a = log alpha, mu = exp(eta), var = mu + mu^2 / alpha:
+//             ll = lgamma(y + alpha) - lgamma(alpha) + alpha log(alpha / (alpha + mu)) + y log(mu / (alpha + mu))
+//             (-lgamma(y + 1) omitted, as in the Poisson family, to which it tends as alpha -> inf)
+constexpr int kDispWords = 9;
+// table words: Gaussian
+constexpr int kDwSinv = 0;     // 1 / sigma = exp(-s)
+constexpr int kDwS = 1;        // s
+// table words: negative binomial.  lgamma / digamma differences in y are evaluated at alpha' = alpha + m >= 8
+// (m = 0 for alpha >= 8) by the Stirling series, and shifted back by the recurrences
+//   lgamma(y + alpha) - lgamma(alpha) = [..](alpha') - log prod_{j<m} (y + alpha + j) + log prod_{j<m} (alpha + j),
+//   psi(y + alpha) - psi(alpha)       = [..](alpha') - sum_{j<m} 1 / (y + alpha + j) + sum_{j<m} 1 / (alpha + j);
+// the sums over alpha alone are per-chain constants.
+constexpr int kDwAlpha = 0;    // alpha
+constexpr int kDwA = 1;        // a = log alpha
+constexpr int kDwM = 2;        // m (0 .. 8)
+constexpr int kDwAp = 3;       // alpha'
+constexpr int kDwIap = 4;      // 1 / alpha'
+constexpr int kDwAph = 5;      // alpha' - 1/2
+constexpr int kDwLa = 6;       // log alpha' - log alpha
+constexpr int kDwCl = 7;       // log prod_{j<m} (alpha + j) - S(alpha'),  S(z) = 1/(12 z) - 1/(360 z^3) + 1/(1260 z^5)
+constexpr int kDwCd = 8;       // sum_{j<m} 1 / (alpha + j) - T(alpha'), T(z) = -1/(2 z) - 1/(12 z^2) + 1/(120 z^4) - 1/(252 z^6)
+
+// The table entries of one chain (family 4 or 5) from its log_dispersion ld.
+__device__ inline void dispersion_constants(int family, float ld, float* t) {
+    const double l = (double)ld;
+    if (family == 4) {
+        t[kDwSinv] = (float)exp(-l);   // exactly 1 at s = 0: family 4 then gives family 2's bits
+        t[kDwS] = ld;
+        return;
+    }
+    const double alpha = exp(l);
+    const int m = alpha < 8.0 ? (int)ceil(8.0 - alpha) : 0;
+    const double ap = alpha + m;
+    double lp = 0.0, sr = 0.0;
+    for (int j = 0; j < m; ++j) {
+        lp += log(alpha + j);
+        sr += 1.0 / (alpha + j);
+    }
+    const double i1 = 1.0 / ap, i2 = i1 * i1;
+    const double S = i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260)));
+    const double T = -0.5 * i1 - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252)));
+    t[kDwAlpha] = (float)alpha;
+    t[kDwA] = ld;
+    t[kDwM] = (float)m;
+    t[kDwAp] = (float)ap;
+    t[kDwIap] = (float)i1;
+    t[kDwAph] = (float)(ap - 0.5);
+    t[kDwLa] = (float)(log(ap) - l);
+    t[kDwCl] = (float)(lp - S);
+    t[kDwCd] = (float)(sr - T);
+}
+
+// Family 4 of one row: ll, r = dll/deta and q = dll/ds.  The scaled residual dn = d / sigma goes through family 2's
+// expression before s is subtracted, and every sigma operation is exact at sigma = 1, so s = 0 gives family 2's
+// ll and r bit for bit.
+__device__ __forceinline__ void gaussian_scale_loglik(float y, float eta, const float* t, float& ll, float& r, float& q) {
+    const float sinv = t[kDwSinv];
+    const float dn = (y - eta) * sinv;
+    ll = (-0.5f * dn * dn - 0.918938533204672742f) - t[kDwS];
+    r = dn * sinv;
+    q = dn * dn - 1.f;
+}
+
+// Family 5 of one row: ll, r = dll/deta = y - (alpha + y) sigmoid(x) and
+// q = dll/da = alpha [psi(y + alpha) - psi(alpha) - softplus(x)] - r, with x = eta - a.
+//   ll = D + y eta - (alpha + y) softplus(x),  D = lgamma(y + alpha) - lgamma(alpha) - y a,
+// which takes y log alpha out of both lgamma terms analytically.  At alpha' (see kDwCl):
+//   D = (y + alpha' - 1/2) log1p(y / alpha') - y + S(y + alpha') + y (log alpha' - a) - log prod_{j<m} (y + alpha + j)
+//       + [log prod_{j<m} (alpha + j) - S(alpha')]
+//   psi(y + alpha) - psi(alpha) = log1p(y / alpha') + T(y + alpha') - sum_{j<m} 1 / (y + alpha + j) + [per chain]
+// so for alpha >> y nothing of size alpha or y log alpha is ever subtracted: D ~ y (y - 1) / (2 alpha) comes out
+// of one FMA with log1p, not of a difference of two lgamma values of size alpha log alpha.  The shift runs a fixed
+// 8-step predicated loop (m is per chain), as two products of at most 4 factors (no overflow for y <= 2^24): one
+// log and one division each, whatever y is.  softplus and the exponential use log1pf / expf, which are
+// relatively accurate at very negative x, where alpha softplus(x) ~ mu.
+__device__ __forceinline__ void negbin_loglik(float y, float eta, const float* t, float& ll, float& r, float& q) {
+    const float alpha = t[kDwAlpha], ap = t[kDwAp];
+    const float x = eta - t[kDwA];
+    const float e = expf(-fabsf(x));
+    const float sp = fmaxf(x, 0.f) + log1pf(e);
+    const float inv = __fdividef(1.f, 1.f + e);
+    const float sig = x >= 0.f ? inv : e * inv;
+    // recurrence from alpha up to alpha' (m factors y + alpha + j, two products of 4)
+    float lp = 0.f, sr = 0.f;
+    const int m = (int)t[kDwM];
+    if (m > 0) {
+        const float ya = y + alpha;
+#pragma unroll
+        for (int g = 0; g < 2; ++g) {
+            float pr = 1.f, nu = 0.f;   // prod f and (sum 1 / f) prod f over this group's factors
+#pragma unroll
+            for (int j = 4 * g; j < 4 * g + 4; ++j)
+                if (j < m) {
+                    const float f = ya + (float)j;
+                    nu = nu * f + pr;
+                    pr = pr * f;
+                }
+            lp += __logf(pr);
+            sr += __fdividef(nu, pr);
+        }
+    }
+    // Stirling series at alpha' >= 8
+    const float z = y + ap;
+    const float iz = __frcp_rn(z), iz2 = iz * iz;
+    const float Sz = iz * (1.f / 12 - iz2 * (1.f / 360 - iz2 * (1.f / 1260)));
+    const float Tz = -0.5f * iz - iz2 * (1.f / 12 - iz2 * (1.f / 120 - iz2 * (1.f / 252)));
+    const float l1 = log1pf(y * t[kDwIap]);
+    const float D = fmaf(y + t[kDwAph], l1, -y) + ((Sz + t[kDwCl]) - lp) + y * t[kDwLa];
+    const float dpsi = l1 + ((Tz + t[kDwCd]) - sr);
+    const float ay = alpha + y;
+    ll = (y * eta - ay * sp) + D;
+    r = y - ay * sig;
+    q = alpha * (dpsi - sp) - r;
+}
+
 
 }  // namespace tc

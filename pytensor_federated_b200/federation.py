@@ -103,9 +103,17 @@ class NodeFederation:
         rows: List[np.ndarray] = []
         chain_of: Dict[int, int] = {}
         shapes: Dict[int, tuple] = {}
-        for node, (intercept, beta) in requests.items():
+        disp_shapes: Dict[int, tuple] = {}
+        for node, inputs in requests.items():
+            # families with a dispersion parameter: (intercept, beta, log_dispersion), the last one part of the key
+            intercept, beta = inputs[0], inputs[1]
             ic = np.asarray(intercept, dtype=np.float32)
-            vec = np.concatenate([ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features * C)])
+            parts = [ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features * C)]
+            if m.dispersion:
+                ld = np.asarray(inputs[2], dtype=np.float32)
+                parts.append(ld.reshape(1))
+                disp_shapes[node] = ld.shape
+            vec = np.concatenate(parts)
             key = vec.tobytes()
             if key not in chains:
                 if len(rows) == K:
@@ -122,13 +130,21 @@ class NodeFederation:
             ic_shape = (m.n_groups, C)
             inputs = ([theta[:, :G].reshape((K,) + ic_shape), theta[:, G:].reshape((K,) + beta_shape)] if K > 1
                       else [theta[0, :G].reshape(ic_shape), theta[0, G:].reshape(beta_shape)])
+        elif m.dispersion:
+            P = m.n_features
+            inputs = ([theta[:, :G], theta[:, G : G + P], theta[:, G + P]] if K > 1
+                      else [theta[0, :G], theta[0, G : G + P], theta[0, G + P]])
         else:
             inputs = [theta[:, :G], theta[:, G:]] if K > 1 else [theta[0, :G], theta[0, G:]]
-        per = m.per_node(self.engine.evaluate_raw(inputs))                         # [n_nodes, K, 1 + G + P]
+        per = m.per_node(self.engine.evaluate_raw(inputs))                         # [n_nodes, K, 1 + G + P (+ 1)]
         out = {}
         for node in requests:
             v = per[node, chain_of[node]]
-            out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].reshape(beta_shape).copy()])
+            if m.dispersion:
+                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G : -1].copy(),
+                                              v[-1].reshape(disp_shapes[node]).copy()])
+            else:
+                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].reshape(beta_shape).copy()])
         return out
 
     def evaluate_node(self, node: int, *inputs) -> Tuple[np.ndarray, List[np.ndarray]]:
@@ -154,7 +170,9 @@ class NodeFederation:
         * linear regression: ``f(intercepts, slopes) -> (logp, [d_intercepts, d_slopes])``, each argument a vector
           ``[n_nodes]`` or a scalar shared by all nodes (its gradient is then the sum over the nodes);
         * ODE: ``f(theta[n_nodes, n_params]) -> (logp, [d_theta])``;
-        * GLM (parameters shared by the nodes): ``f(intercept, beta) -> (logp, [d_intercept, d_beta])``.
+        * GLM (parameters shared by the nodes): ``f(intercept, beta) -> (logp, [d_intercept, d_beta])``; families
+          with a dispersion parameter: ``f(intercept, beta, log_dispersion) -> (logp, [d_intercept, d_beta,
+          d_log_dispersion])``.
 
         With :meth:`all_nodes_op` the model graph has ONE federated node instead of one per data holder, so the
         Python cost of a model evaluation no longer grows with the size of the federation."""
@@ -174,6 +192,12 @@ class NodeFederation:
                     th = np.broadcast_to(np.asarray(theta, dtype=np.float64), (self.n_nodes, m.n_params))
                     per = m.per_node(eng.evaluate_raw([th]))
                     return np.asarray(per[:, 0].sum()), [per[:, 1:].copy()]
+        elif getattr(eng.model, "dispersion", False):
+            def func(intercept, beta, log_dispersion):
+                with self._lock:
+                    self.n_launches += 1
+                    logp, *grads = eng.evaluate(intercept, beta, log_dispersion)
+                    return logp, grads
         else:
             def func(intercept, beta):
                 with self._lock:

@@ -16,7 +16,9 @@ import numpy as np
 
 from .base import ShardModel
 
-FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3}
+FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5}
+#: families with a learned dispersion parameter (one more input, ``log_dispersion``)
+DISPERSION_FAMILIES = ("gaussian_scale", "negative_binomial")
 
 
 def _family_code(family) -> int:
@@ -82,6 +84,21 @@ class GlmShards(ShardModel):
         This full parameterisation is not identified without priors: adding one vector to every class column of
         ``(intercept, beta)`` leaves LL unchanged (its gradients sum to 0 over the classes).  A reference-category
         model is obtained by fixing one column (say class 0) at 0 and ignoring its gradient.
+
+        ``"gaussian_scale"`` and ``"negative_binomial"`` learn a dispersion parameter: the inputs per call are
+        ``(intercept, beta, log_dispersion)`` — ``intercept[G]`` (a scalar when G = 1), ``beta[P]`` and a scalar, batched
+        ``[K, G]``, ``[K, P]`` and ``[K]`` — and the gradients come back in the same shapes.  With
+        ``eta = intercept[group] + x' beta + o``:
+
+            gaussian_scale, s = log sigma:   ll = -(d / sigma)^2 / 2 - s - log(2 pi) / 2,      d = y - eta
+            negative_binomial, a = log alpha (NB2: mean mu = exp(eta), variance mu + mu^2 / alpha):
+                ll = lgamma(y + alpha) - lgamma(alpha) + alpha log(alpha / (alpha + mu)) + y log(mu / (alpha + mu))
+
+        The negative-binomial LL omits ``-lgamma(y + 1)``, as the Poisson family does, so as alpha -> inf it tends to
+        the Poisson family's ``y eta - mu`` exactly (the Gaussian one keeps ``-log(2 pi) / 2`` like ``"gaussian"``,
+        which it equals at s = 0).  Offsets (``log t`` exposures of count models) and weights work as for every family.
+        Counts must be integers in ``[0, 2^24]`` on every row of non-zero weight.  Only the bf16 tensor-core kernel
+        evaluates these families, with the shape limits of the multinomial one; ``n_classes`` is rejected.
     """
 
     def __init__(
@@ -144,10 +161,14 @@ class GlmShards(ShardModel):
         #: classes per chain (multinomial family; 1 for every other family)
         self.n_classes = 1
         self.multinomial = isinstance(family, str) and family == "multinomial"
+        #: the family has a log-dispersion parameter after beta (``gaussian_scale``, ``negative_binomial``)
+        self.dispersion = isinstance(family, str) and family in DISPERSION_FAMILIES
         if self.multinomial:
             self._init_multinomial(n_classes)
         elif n_classes is not None:
             raise ValueError("n_classes is for family='multinomial' only")
+        if self.dispersion:
+            self._init_dispersion()
 
     def _init_multinomial(self, n_classes) -> None:
         """Checks of the multinomial family, then its sizes: C (G + P) parameters per chain, and the kernel's
@@ -176,6 +197,26 @@ class GlmShards(ShardModel):
         self.n_params = C * (self.n_groups + self.n_features)
         self.n_theta_words = self.n_chains * self.n_params
         self.n_vals = self.n_nodes * self.n_chains * C * (1 + self.n_groups + self.n_features)
+
+    def _init_dispersion(self) -> None:
+        """Checks of the families with a dispersion parameter, then their sizes: theta per chain is
+        ``[intercept[G], beta[P], log_dispersion]`` and the output block ``[LL, d intercept[G], d beta[P], d log_dispersion]``."""
+        import torch
+
+        if self.kernel not in ("auto", "tc"):
+            raise ValueError(f"kernel={self.kernel!r}: the {self.family} family runs on the bf16 tensor-core kernel only "
+                             "(kernel='tc' or 'auto')")
+        if self.family == "negative_binomial":
+            for si, (y, w) in enumerate(zip(self.ys, self.weights)):
+                bad = ~((y == torch.floor(y)) & (y >= 0) & (y <= 2.0 ** 24))   # NaN fails every comparison
+                if w is not None:
+                    bad &= w != 0   # a masked row may carry anything
+                if bool(torch.any(bad)):
+                    raise ValueError(f"counts of segment {si} must be integers in [0, 2^24] on every row of non-zero weight")
+        self.n_inputs = 3
+        self.n_params = self.n_groups + self.n_features + 1
+        self.n_theta_words = self.n_chains * self.n_params
+        self.n_vals = self.n_nodes * self.n_chains * (1 + self.n_params)
 
     def _row_data(self, entries, name: str) -> list:
         """One contiguous float32 tensor (or None) per segment, on the device of the segment's X."""
@@ -213,7 +254,10 @@ class GlmShards(ShardModel):
     # -- packing ---------------------------------------------------------------------------
     def call_context(self, inputs):
         """``(batched, intercept shape)`` of one call: a 2-D ``beta`` means one row per chain (multinomial: a 3-D
-        ``beta[K, P, C]``)."""
+        ``beta[K, P, C]``); families with a dispersion parameter add the shape of ``log_dispersion``."""
+        if self.dispersion:
+            intercept, beta, log_disp = inputs
+            return (np.ndim(beta) == 2, np.shape(intercept), np.shape(log_disp))
         intercept, beta = inputs
         return (np.ndim(beta) == (3 if self.multinomial else 2), np.shape(intercept))
 
@@ -222,6 +266,8 @@ class GlmShards(ShardModel):
     def pack_theta(self, inputs, out: np.ndarray):
         if self.multinomial:
             return self._pack_theta_multinomial(inputs, out)
+        if self.dispersion:
+            return self._pack_theta_dispersion(inputs, out)
         intercept, beta = inputs
         views = self._pack_views
         if views is None or views[0] is not out:
@@ -254,20 +300,38 @@ class GlmShards(ShardModel):
         views[2][...] = bt.reshape(K, P, C).transpose(0, 2, 1)
         return ctx
 
+    def _pack_theta_dispersion(self, inputs, out: np.ndarray):
+        """Theta words as ``[K][G + P + 1]``: ``(intercept, beta, log_dispersion)`` of each chain."""
+        intercept, beta, log_disp = inputs
+        K, G, P = self.n_chains, self.n_groups, self.n_features
+        th = out.view(np.float32).reshape(K, G + P + 1)
+        ic, bt, ld = np.asarray(intercept), np.asarray(beta), np.asarray(log_disp)
+        ctx = (bt.ndim == 2, ic.shape, ld.shape)
+        self._batched, self._icpt_shape = ctx[:2]
+        self._disp_shape = ctx[2]
+        th[:, :G] = ic.reshape(K, G)
+        th[:, G : G + P] = bt.reshape(K, P)
+        th[:, G + P] = ld.reshape(K)
+        return ctx
+
     _batched = False
     _icpt_shape = ()
+    _disp_shape = ()
 
     def _note_shapes(self, inputs):
         # single-threaded convenience state (tests call reference_partial then unpack_result);
         # the engine passes the context explicitly instead
         ctx = self.call_context(inputs)
-        self._batched, self._icpt_shape = ctx
+        self._batched, self._icpt_shape = ctx[:2]
+        if self.dispersion:
+            self._disp_shape = ctx[2]
         return ctx
 
     def per_node(self, vals: np.ndarray) -> np.ndarray:
         """The reduced vector as ``[n_nodes, n_chains, 1 + G + P]`` (``[LL, d intercepts, d beta]`` per block).
         Multinomial: ``[n_nodes, n_chains, 1 + G C + P C]``, ``[LL, d intercept (G, C), d beta (P, C)]`` with the
-        matrices row-major, summed from the kernel's blocks of the chain's C classes."""
+        matrices row-major, summed from the kernel's blocks of the chain's C classes.  Families with a dispersion
+        parameter: ``[n_nodes, n_chains, 2 + G + P]``, ``[LL, d intercepts, d beta, d log_dispersion]``."""
         if self.multinomial:
             n, K, C, G = self.n_nodes, self.n_chains, self.n_classes, self.n_groups
             raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C, 1 + G + self.n_features)
@@ -279,6 +343,8 @@ class GlmShards(ShardModel):
     def unpack_result(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
         if self.multinomial:
             return self._unpack_multinomial(vals, ctx)
+        if self.dispersion:
+            return self._unpack_dispersion(vals, ctx)
         v = self.per_node(vals).sum(axis=0) if self.n_nodes > 1 else np.asarray(vals, dtype=np.float64).reshape(self.n_chains, 1 + self.n_params)
         G = self.n_groups
         batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
@@ -286,6 +352,16 @@ class GlmShards(ShardModel):
             return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
                     v[:, 1 + G :].copy()]
         return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G :].copy()]
+
+    def _unpack_dispersion(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
+        v = self.per_node(vals).sum(axis=0)                         # [K, 2 + G + P]
+        G, P = self.n_groups, self.n_features
+        batched, icpt_shape, disp_shape = ctx if ctx is not None else (self._batched, self._icpt_shape, self._disp_shape)
+        if batched:
+            return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
+                    v[:, 1 + G : 1 + G + P].copy(), v[:, 1 + G + P].reshape(disp_shape).copy()]
+        return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G : 1 + G + P].copy(),
+                v[0, 1 + G + P].reshape(disp_shape).copy()]
 
     def _unpack_multinomial(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
         v = self.per_node(vals).sum(axis=0)                         # [K, 1 + G C + P C]
@@ -309,12 +385,12 @@ class GlmShards(ShardModel):
             if X0.dtype not in (torch.bfloat16, torch.float32) or self.n_chains != 1 or self.n_features > 1024:
                 raise ValueError("custom likelihoods need a bf16/fp32 design matrix, one chain and P <= 1024")
             return 3 if X0.dtype == torch.bfloat16 else 4
-        if self.multinomial:   # the bf16 tensor-core kernel or nothing: no other kernel has this family
+        if self.multinomial or self.dispersion:   # the bf16 tensor-core kernel or nothing: no other kernel has these
             if not (X0.dtype == torch.bfloat16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384
-                    and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0):
-                raise ValueError(f"the multinomial family runs on the bf16 tensor-core kernel only, which needs a bf16 "
+                    and self.n_chains <= 16 and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0):
+                raise ValueError(f"the {self.family} family runs on the bf16 tensor-core kernel only, which needs a bf16 "
                                  f"design matrix with P % 8 == 0, 8 <= P <= 384 and 16-byte aligned rows (got "
-                                 f"{X0.dtype}, P = {self.n_features}, row stride {self.ld})")
+                                 f"{X0.dtype}, P = {self.n_features}, row stride {self.ld}) and at most 16 chains")
             return 1
         if self.kernel == "fp8":
             return 2
@@ -391,6 +467,8 @@ class GlmShards(ShardModel):
         dtype = dtype or torch.float32
         if self.multinomial:
             return self._multinomial_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
+        if self.dispersion:
+            return self._dispersion_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(self.n_chains, -1)
@@ -481,6 +559,46 @@ class GlmShards(ShardModel):
                 out[:, 1 + G :] += (rT.to(torch.bfloat16) @ Xf if bf16_gemms else rT @ Xf).double()
         return full.reshape(-1).cpu().numpy()
 
+    def _dispersion_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
+        """The partial of the families with a dispersion parameter, ``[n_nodes][K][LL, gi[G], g[P], q]`` with
+        ``q = dll/dlog_dispersion``.  ``bf16_gemms``: the collective baseline, two bf16 GEMMs and fp32 elementwise
+        work; else the oracle in ``dtype``."""
+        import torch
+
+        intercept, beta, log_disp = inputs
+        self._note_shapes(inputs)
+        K, G, P = self.n_chains, self.n_groups, self.n_features
+        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G).to(self.device, dtype)
+        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P)
+        ld = torch.as_tensor(np.asarray(log_disp, dtype=np.float64)).reshape(K).to(self.device, dtype)
+        B = bt.T.to(self.device, torch.bfloat16 if bf16_gemms else dtype)       # [P, K]
+        full = torch.zeros(self.n_nodes, K, 2 + G + P, dtype=torch.float64, device=self.device)
+        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
+            out = full[self.node_ids[si] if self.node_ids is not None else 0]
+            for r0 in range(0, X.shape[0], chunk_rows):
+                r1 = min(X.shape[0], r0 + chunk_rows)
+                if bf16_gemms:
+                    Xf = X[r0:r1]
+                    eta = (Xf @ B).to(dtype)
+                else:
+                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
+                    eta = Xf @ B
+                eta = eta + ic[:, g]
+                if self.offsets[si] is not None:
+                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
+                yy = y[r0:r1].to(dtype).unsqueeze(1)
+                if self.family == "gaussian_scale":
+                    ll, r, q = _gaussian_scale_terms(yy, eta, ld)
+                else:
+                    ll, r, q = _negative_binomial_terms(yy, eta, ld)
+                ll, r = self._weigh(si, r0, r1, ll, r)
+                _, q = self._weigh(si, r0, r1, ll, q)
+                out[:, 0] += ll.double().sum(0)
+                out[:, 1 + g] += r.double().sum(0)
+                out[:, 1 + G : 1 + G + P] += (r.T.to(torch.bfloat16) @ Xf if bf16_gemms else r.T @ Xf).double()
+                out[:, 1 + G + P] += q.double().sum(0)
+        return full.reshape(-1).cpu().numpy()
+
     def _dequant_rows(self, seg: int, r0: int, r1: int):
         """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
         return self.Xs[seg][r0:r1]
@@ -498,6 +616,8 @@ class GlmShards(ShardModel):
             return self.reference_partial(inputs)
         if self.multinomial:
             return self._multinomial_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
+        if self.dispersion:
+            return self._dispersion_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float32)).reshape(self.n_chains, -1).to(self.device)
@@ -534,6 +654,51 @@ class GlmShards(ShardModel):
 
     def flops_per_eval(self) -> int:
         return int(4 * self.n_rows * self.n_features * self.n_chains * self.n_classes)
+
+
+_LOG_SQRT_2PI = 0.918938533204672742
+
+
+def _gaussian_scale_terms(y, eta, s):
+    """``(ll, dll/deta, dll/ds)`` of the Gaussian with ``sigma = exp(s)`` (``s`` per chain, broadcast over rows)."""
+    import torch
+
+    dn = (y - eta) * torch.exp(-s)
+    return -0.5 * dn * dn - s - _LOG_SQRT_2PI, dn * torch.exp(-s), dn * dn - 1.0
+
+
+def _negative_binomial_terms(y, eta, a):
+    """``(ll, dll/deta, dll/da)`` of the NB2 negative binomial with ``alpha = exp(a)``, ``mu = exp(eta)``, without
+    ``-lgamma(y + 1)``.  ``lgamma(y + alpha) - lgamma(alpha) - y a`` and ``psi(y + alpha) - psi(alpha)`` are taken
+    from their Stirling-series differences (written with ``log1p(y / alpha)``) where alpha is large, so that the
+    y log alpha terms and the lgamma values of size alpha log alpha cancel analytically, not in floating point."""
+    import torch
+
+    alpha = torch.exp(a)
+    x = eta - a
+    sp = torch.nn.functional.softplus(x)
+    big = alpha >= (8.0 if eta.dtype == torch.float32 else 1e3)   # the series' error: < 1e-9 (fp32), < 1e-25 (fp64)
+    yb = torch.where(torch.isfinite(y) & (y >= 0), y, torch.zeros_like(y))   # masked rows: keep every branch finite
+    ab = torch.where(big, alpha, torch.full_like(alpha, 1e3))
+    z = yb + ab
+    l1 = torch.log1p(yb / ab)
+
+    def stirling(v):   # lgamma(v) - ((v - 1/2) log v - v + log(2 pi) / 2)
+        return (1.0 / 12 - (1.0 / 360 - 1.0 / (1260 * v * v)) / (v * v)) / v
+
+    def psi_tail(v):   # psi(v) - log v
+        i2 = 1.0 / (v * v)
+        return -0.5 / v - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 / 252))
+
+    d_big = (z - 0.5) * l1 - yb + stirling(z) - stirling(ab)
+    dpsi_big = l1 + psi_tail(z) - psi_tail(ab)
+    d_small = torch.lgamma(y + alpha) - torch.lgamma(alpha) - y * a
+    dpsi_small = torch.digamma(y + alpha) - torch.digamma(alpha)
+    D = torch.where(big, d_big, d_small)
+    dpsi = torch.where(big, dpsi_big, dpsi_small)
+    ll = D + y * eta - (alpha + y) * sp
+    r = y - (alpha + y) * torch.sigmoid(x)
+    return ll, r, alpha * (dpsi - sp) - r
 
 
 def quantize_block_fp8(X, block: int = 32):
@@ -671,6 +836,29 @@ def synth_multinomial_shard(n_rows: int, n_features: int, n_classes: int, *, see
         X[r0:r1] = xb
         p = torch.softmax(xb.float() @ beta_true + b_true, dim=1)
         y[r0:r1] = torch.multinomial(p, 1, generator=gen).squeeze(1).float()
+    return X, y, beta_true
+
+
+def synth_negative_binomial_shard(n_rows: int, n_features: int, *, alpha: float, seed: int, device,
+                                  chunk_rows: int = 1 << 20, beta_scale: float = 0.05, intercept: float = 0.5):
+    """Synthetic over-dispersed count shard generated on the device in chunks: bf16 ``X ~ N(0,1)``,
+    ``y ~ NegativeBinomial(mean mu = exp(X beta* + intercept), variance mu + mu^2 / alpha)`` drawn as a gamma-Poisson
+    mixture (``lambda ~ Gamma(alpha, scale mu / alpha)``, ``y ~ Poisson(lambda)``), stored as float32.
+    Returns ``(X, y, beta*)``."""
+    import torch
+
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        mu = torch.exp(xb.float() @ beta_true + intercept).double()
+        lam = torch._standard_gamma(torch.full_like(mu, float(alpha)), generator=gen) * (mu / alpha)
+        y[r0:r1] = torch.poisson(lam, generator=gen).float()
     return X, y, beta_true
 
 

@@ -523,6 +523,14 @@ def default_inputs_from_words(model: ShardModel, words: np.ndarray):
         if model.n_chains == 1:
             return ic[0].copy(), bt[0].copy()
         return ic.copy(), bt.copy()
+    if isinstance(model, GlmShards) and model.dispersion:
+        # words [K][G + P + 1] -> intercept [K, G], beta [K, P], log_dispersion [K] (one chain: [G], [P], scalar)
+        th = words.view(np.float32).reshape(model.n_chains, model.n_params)
+        G, P = model.n_groups, model.n_features
+        ic, bt, ld = th[:, :G], th[:, G : G + P], th[:, G + P]
+        if model.n_chains == 1:
+            return ic[0].copy(), bt[0].copy(), ld[0].copy()
+        return ic.copy(), bt.copy(), ld.copy()
     if isinstance(model, GlmShards):
         th = words.view(np.float32).reshape(model.n_chains, model.n_params)
         if model.n_chains == 1:

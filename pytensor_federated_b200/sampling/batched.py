@@ -164,21 +164,26 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
     data instead of sixty-four.
 
     A multinomial engine (``family="multinomial"``, C classes) takes ``theta = [intercept (G, C), beta (P, C)]`` per
-    chain, both flattened row-major."""
+    chain, both flattened row-major; one with a dispersion parameter (``"gaussian_scale"``, ``"negative_binomial"``)
+    takes ``theta = [intercept[G], beta[P], log_dispersion]``.  Gradients come back in the order of theta."""
     cap = int(getattr(engine.model, "n_chains", 1))
     n_classes = int(getattr(engine.model, "n_classes", 1)) if getattr(engine.model, "multinomial", False) else 1
+    dispersion = bool(getattr(engine.model, "dispersion", False))
     split = n_groups * n_classes   # theta columns that are intercepts
 
     def shaped(ic: np.ndarray, beta: np.ndarray):
-        """Inputs of ``engine.evaluate``; ``ic`` / ``beta`` have the chains (if any) in their leading axis."""
+        """Inputs of ``engine.evaluate``; ``ic`` / ``beta`` have the chains (if any) in their leading axis (with a
+        dispersion parameter, ``beta``'s last column is ``log_dispersion``)."""
+        if dispersion:
+            return ic, beta[..., :-1], beta[..., -1]
         if n_classes == 1:
             return ic, beta
         lead = ic.shape[:-1]
         return ic.reshape(lead + (n_groups, n_classes)), beta.reshape(lead + (-1, n_classes))
 
     def tile(theta: np.ndarray):
-        logp, d_ic, d_beta = engine.evaluate(*shaped(theta[:, :split], theta[:, split:]))
-        return np.asarray(logp).reshape(-1), np.concatenate([np.asarray(d_ic).reshape(cap, -1), np.asarray(d_beta).reshape(cap, -1)], axis=1)
+        logp, *grads = engine.evaluate(*shaped(theta[:, :split], theta[:, split:]))
+        return np.asarray(logp).reshape(-1), np.concatenate([np.asarray(g).reshape(cap, -1) for g in grads], axis=1)
 
     def fn(theta: np.ndarray):
         theta = np.asarray(theta)
@@ -192,8 +197,8 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
             if k < cap:
                 block = np.concatenate([block, np.repeat(block[-1:], cap - k, axis=0)], axis=0)
             if cap == 1:   # single-chain engines take unbatched inputs
-                logp, d_ic, d_beta = engine.evaluate(*shaped(block[0, :split], block[0, split:]))
-                lp, gr = np.asarray(logp).reshape(1), np.concatenate([np.asarray(d_ic).reshape(-1), np.asarray(d_beta).reshape(-1)])[None]
+                logp, *outs = engine.evaluate(*shaped(block[0, :split], block[0, split:]))
+                lp, gr = np.asarray(logp).reshape(1), np.concatenate([np.asarray(g).reshape(-1) for g in outs])[None]
             else:
                 lp, gr = tile(block)
             logps.append(lp[:k])

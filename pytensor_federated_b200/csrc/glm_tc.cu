@@ -83,7 +83,10 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
 // with a learned dispersion parameter (codes 4 and 5, tc::gaussian_scale_loglik / tc::negbin_loglik): theta rows
 // have stride G + P + 1, the intercept table is followed by kDispWords per-chain constants, the epilogue produces a
 // third per-row value q = dll/dlog_dispersion next to ll and r, and each chain's output block is
-// [LL, gi[G], g[P], dlog_dispersion].  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// [LL, gi[G], g[P], dlog_dispersion]; ORD = the ordinal (cumulative-logit) family (code 6), whose C - 1 cutpoints
+// ride along N like the multinomial classes: column v = k (C - 1) + j is cutpoint j of chain k, its intercept table
+// row holds intercept - c_j (packed by the host), so MMA #1 gives z_j = eta - c_j, and the columns of one row are
+// coupled only through tc::ordinal_loglik.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -106,7 +109,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS, bool SOFTMAX, bool DISP>
+template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -317,6 +320,19 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                     sm_cls[s] = (float)(v % NC);
                 }
             }
+            // ORD: chain and cutpoint of this thread's columns (chain -1: past K (C - 1))
+            int od_chain[2 * NJ], od_cut[2 * NJ];
+            int od_chains = 0, od_ncut = 1;
+            if constexpr (ORD) {
+                od_ncut = prm.n_classes - 1;
+                od_chains = nch / od_ncut;
+#pragma unroll
+                for (int s = 0; s < 2 * NJ; ++s) {
+                    const int v = 8 * (s >> 1) + 2 * q + (s & 1);
+                    od_chain[s] = v < nch ? v / od_ncut : -1;
+                    od_cut[s] = v % od_ncut;
+                }
+            }
             Ring stage;
             uint32_t rb = 0;                        // R buffer of the current tile (alternates)
             for (int j = 0;; ++j) {
@@ -397,6 +413,24 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                             }
                             softmax_loglik<2 * NJ, KC / 2>(sm_eta, sm_chain, sm_cls, sm_chains, y, sm_ll, sm_r);
                         }
+                        // ORD: z = eta - c_j (+ offset, as in ROWS) of every column, coupled per chain over the quad;
+                        // every lane takes part, valid row or not.  The label is clamped into [0, C - 1], so a masked
+                        // row's NaN or out-of-range y (dropped below) still indexes inside the intercept table.
+                        float od_ll[2 * NJ], od_r[2 * NJ];
+                        if constexpr (ORD) {
+                            float z[2 * NJ];
+#pragma unroll
+                            for (int s = 0; s < 2 * NJ; ++s) {
+                                const int jc = s >> 1, e = s & 1;
+                                const int k = od_chain[s] >= 0 ? 8 * jc + 2 * q + e : 0;   // as in SOFTMAX
+                                z[s] = ((eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
+                                        eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k * G + seg_group];
+                                if constexpr (ROWS) z[s] = __fadd_rn(z[s], o);
+                            }
+                            const int yi = min(max(__float2int_rz(y), 0), od_ncut);   // NaN -> 0
+                            ordinal_loglik<2 * NJ, KC>(z, od_chain, od_cut, od_chains, od_ncut, yi, icpt + seg_group, G,
+                                                       od_ll, od_r);
+                        }
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc)
 #pragma unroll
@@ -417,6 +451,14 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                             ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
                                             r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
                                             dq = wt == 0.f ? 0.f : __fmul_rn(wt, dq);
+                                        }
+                                    } else if constexpr (ORD) {
+                                        // offset already in z; weight as in ROWS
+                                        ll = od_ll[2 * jc + e];
+                                        r = od_r[2 * jc + e];
+                                        if constexpr (ROWS) {
+                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
                                         }
                                     } else if constexpr (SOFTMAX) {
                                         // weight as in ROWS (offsets are rejected for this family)
@@ -624,12 +666,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP)                                                                         \
+#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD)                                                                    \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
                                                  prm->n_groups + (DISP ? tc::kDispWords : 0), KC);                 \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -640,27 +682,34 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP>, *comm, segs_dev, *prm, maps,            \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD>, *comm, segs_dev, *prm, maps,       \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
     if (prm->family == 3) {                 // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
         if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false); else LAUNCH_TC(4, false, true, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false); else LAUNCH_TC(8, false, true, false); }
-        else { if (rows) LAUNCH_TC(16, true, true, false); else LAUNCH_TC(16, false, true, false); }
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false); else LAUNCH_TC(4, false, true, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false); else LAUNCH_TC(8, false, true, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, true, false, false); else LAUNCH_TC(16, false, true, false, false); }
+    }
+    else if (prm->family == 6) {            // ordinal: K (C - 1) cutpoint columns; C = 2, K = 1 runs the KC = 1 bucket
+        if (prm->n_classes < 2 || prm->n_chains % (prm->n_classes - 1) != 0) return -3;
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true); else LAUNCH_TC(1, false, false, false, true); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true); else LAUNCH_TC(4, false, false, false, true); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true); else LAUNCH_TC(8, false, false, false, true); }
+        else { if (rows) LAUNCH_TC(16, true, false, false, true); else LAUNCH_TC(16, false, false, false, true); }
     }
     else if (prm->family == 4 || prm->family == 5) {   // learned dispersion: theta rows [G + P + 1]
         if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true); else LAUNCH_TC(1, false, false, true); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true); else LAUNCH_TC(4, false, false, true); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true); else LAUNCH_TC(8, false, false, true); }
-        else { if (rows) LAUNCH_TC(16, true, false, true); else LAUNCH_TC(16, false, false, true); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false); else LAUNCH_TC(1, false, false, true, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false); else LAUNCH_TC(4, false, false, true, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false); else LAUNCH_TC(8, false, false, true, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, true, false); else LAUNCH_TC(16, false, false, true, false); }
     }
-    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false); else LAUNCH_TC(1, false, false, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false); else LAUNCH_TC(4, false, false, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false); else LAUNCH_TC(8, false, false, false); }
-    else { if (rows) LAUNCH_TC(16, true, false, false); else LAUNCH_TC(16, false, false, false); }
+    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false); else LAUNCH_TC(1, false, false, false, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false); else LAUNCH_TC(4, false, false, false, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false); else LAUNCH_TC(8, false, false, false, false); }
+    else { if (rows) LAUNCH_TC(16, true, false, false, false); else LAUNCH_TC(16, false, false, false, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

@@ -34,13 +34,16 @@ struct GlmParams {
                           // 3 = multinomial (softmax over n_classes columns; tensor-core bf16 kernel only),
                           // 4 = Gaussian with unknown scale (log_dispersion = log sigma), 5 = negative binomial (NB2,
                           // log link, log_dispersion = log alpha); 4 and 5: tensor-core bf16 kernel only, output
-                          // block per chain [LL, gi[G], g[P], dLL/dlog_dispersion]
+                          // block per chain [LL, gi[G], g[P], dLL/dlog_dispersion], 6 = ordinal (cumulative logit,
+                          // n_classes = C categories, C - 1 cutpoint columns per chain; tensor-core bf16 kernel only)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)
     int row_data;         // kGlmRowOffsets | kGlmRowWeights when any segment has them: selects the kernel instantiation
     int n_classes;        // multinomial: C classes per chain, n_chains = K C "virtual chains" (column k C + c is class
-                          // c of chain k; theta row k C + c = (intercept[:, c], beta[:, c]) of chain k); else 1
+                          // c of chain k; theta row k C + c = (intercept[:, c], beta[:, c]) of chain k); ordinal: C
+                          // categories, n_chains = K (C - 1) (column k (C - 1) + j is cutpoint j of chain k; theta row
+                          // k (C - 1) + j = (intercept - c_j, beta) of chain k); else 1
 };
 
 constexpr int kGlmRowOffsets = 1;

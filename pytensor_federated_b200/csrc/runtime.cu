@@ -573,8 +573,27 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
                 g_last_error = "the multinomial family takes no offsets (one common to all classes cancels)";
                 return -37;
             }
+    } else if (family == 6) {
+        // family 6 (ordinal): the C - 1 cutpoints of each chain are columns of a K (C - 1)-chain launch, so like
+        // family 3 it exists in the bf16 tensor-core kernel only; checked before any engine state changes
+        if (use_tensor_cores != 1) {
+            g_last_error = "the ordinal family runs on the bf16 tensor-core kernel only";
+            return -34;
+        }
+        if (n_classes < 2 || n_classes > 17) {
+            g_last_error = "the ordinal family needs 2 <= n_classes <= 17";
+            return -35;
+        }
+        if (n_chains % (n_classes - 1) != 0) {
+            g_last_error = "the ordinal family needs n_chains = K x (n_classes - 1) (one column per chain and cutpoint)";
+            return -36;
+        }
+        if ((long long)(n_out > 0 ? n_out : 1) * n_chains * (1 + n_groups + n_features) != e->n_vals) {
+            g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
+            return -33;
+        }
     } else if (n_classes != 1) {
-        g_last_error = "n_classes must be 1 for every family but the multinomial one";
+        g_last_error = "n_classes must be 1 for every family but the multinomial and ordinal ones";
         return -38;
     }
     // families 4 and 5 (Gaussian with unknown scale, negative binomial) carry a log-dispersion parameter after

@@ -274,6 +274,73 @@ __device__ __forceinline__ void softmax_loglik(const float (&eta)[NS], const int
         }
 }
 
+// The cumulative-logit terms of one row and chain, with u = z_up = eta - c_y (up: y <= C - 2), l = z_lo =
+// eta - c_{y-1} (lo: y >= 1) and the gap d = l - u > 0 (used when both are present):
+//   y = 0:      ll = -softplus(u),                                 r_up = -sigmoid(u)
+//   y = C - 1:  ll = -softplus(-l),                                r_lo = sigmoid(-l)
+//   otherwise:  ll = -softplus(u) - softplus(-l) + log(1 - e^-d),  r_up = -sigmoid(u) - 1 / expm1(d),
+//                                                                  r_lo = sigmoid(-l) + 1 / expm1(d)
+// softplus, sigmoid and log(1 - e^-d) use expf / log1pf / expm1f, which stay relatively accurate in the tails
+// (|c - eta| of 30 and more, gaps of a few hundredths), where __logf(1 + e) would return 0 or log(d) would cancel.
+__device__ __forceinline__ void ordinal_terms(float u, float l, float d, bool up, bool lo, float& ll, float& ru, float& rl) {
+    const float eu = expf(-fabsf(u)), el = expf(-fabsf(l));
+    const float spu = fmaxf(u, 0.f) + log1pf(eu);              // softplus(u)
+    const float spl = fmaxf(-l, 0.f) + log1pf(el);             // softplus(-l)
+    const float sgu = __fdividef(u >= 0.f ? 1.f : eu, 1.f + eu);   // sigmoid(u)
+    const float sgl = __fdividef(l <= 0.f ? 1.f : el, 1.f + el);   // sigmoid(-l)
+    const bool mid = up && lo;
+    const float lg = d > 0.693147181f ? log1pf(-expf(-d)) : logf(-expm1f(-d));   // log(1 - e^-d)
+    const float t = mid ? __frcp_rn(expm1f(d)) : 0.f;          // 0 once expm1 overflows (d > 88)
+    ll = ((up ? -spu : 0.f) - (lo ? spl : 0.f)) + (mid ? lg : 0.f);
+    ru = -sgu - t;
+    rl = sgl + t;
+}
+
+// Ordinal (cumulative-logit) likelihood of one row, family 6.  The C - 1 = n_cut cutpoints of chain k are columns
+// v = k n_cut + j, and column v holds z_j = eta - c_j (the intercept table row v is intercept - c_j).  As in
+// softmax_loglik, the row's columns sit in the four lanes of a quad, this lane holds NS of them (chain[s]: its chain,
+// -1 past K n_cut; cut[s]: its cutpoint j).  For label yi (clamped to [0, n_cut]) the row couples only the columns
+// up = yi (if yi < n_cut) and lo = yi - 1 (if yi > 0): per chain, their z are summed over the quad with xor-1 / xor-2
+// shuffles, which every lane runs for every chain below n_chains (warp-uniform); a lane holding neither column
+// adds 0, so the sums are exact and all four lanes get the same bits.  The gap l - u is taken from the intercept
+// table, icpt[(k, yi - 1)] - icpt[(k, yi)] of the row's group (icpt_g points at column g of the [KC][G] table): the
+// difference of two packed fp32 values, > 0 whenever the host accepted the cutpoints as ordered, and accurate to
+// ulp(|intercept - c|) rather than ulp(|z|).  Results: ll[s] = the chain's ll in column min(yi, n_cut - 1) and 0
+// elsewhere, r[s] = r_up / r_lo in the up / lo columns and 0 elsewhere.
+template <int NS, int MAX_CHAINS>
+__device__ __forceinline__ void ordinal_loglik(const float (&z)[NS], const int (&chain)[NS], const int (&cut)[NS],
+                                               int n_chains, int n_cut, int yi, const float* icpt_g, int G,
+                                               float (&ll)[NS], float (&r)[NS]) {
+    const bool up = yi < n_cut, lo = yi > 0;
+    const int credit = up ? yi : yi - 1;
+#pragma unroll
+    for (int s = 0; s < NS; ++s) ll[s] = r[s] = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAX_CHAINS; ++k) {
+        if (k >= n_chains) break;
+        float zu = 0.f, zl = 0.f;
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) {
+                if (cut[s] == yi) zu = z[s];
+                if (cut[s] == yi - 1) zl = z[s];
+            }
+        zu += __shfl_xor_sync(0xffffffffu, zu, 1);
+        zl += __shfl_xor_sync(0xffffffffu, zl, 1);
+        zu += __shfl_xor_sync(0xffffffffu, zu, 2);
+        zl += __shfl_xor_sync(0xffffffffu, zl, 2);
+        const float d = (up && lo) ? icpt_g[(k * n_cut + yi - 1) * G] - icpt_g[(k * n_cut + yi) * G] : 1.f;
+        float llk, ru, rl;
+        ordinal_terms(zu, zl, d, up, lo, llk, ru, rl);
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+            if (chain[s] == k) {
+                ll[s] = cut[s] == credit ? llk : 0.f;
+                r[s] = cut[s] == yi ? ru : (cut[s] == yi - 1 ? rl : 0.f);
+            }
+    }
+}
+
 // Families with a learned dispersion parameter: theta per chain is [intercept[G], beta[P], log_dispersion], and
 // the per-chain constants below, derived from log_dispersion at setup (in double), sit in a table of kDispWords
 // floats per chain behind the intercepts.

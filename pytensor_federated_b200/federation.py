@@ -96,7 +96,7 @@ class NodeFederation:
     def _evaluate_glm(self, requests):
         m = self.engine.model
         # multinomial models: intercept (G, C) and beta (P, C) per chain, flattened row-major
-        C = m.n_classes
+        C = m.n_classes if m.multinomial else 1
         G, K = m.n_groups * C, m.n_chains
         beta_shape = (m.n_features, C) if m.multinomial else (m.n_features,)
         chains: Dict[bytes, int] = {}      # distinct parameter vector -> chain
@@ -104,14 +104,16 @@ class NodeFederation:
         chain_of: Dict[int, int] = {}
         shapes: Dict[int, tuple] = {}
         disp_shapes: Dict[int, tuple] = {}
+        n_third = 1 if m.dispersion else (m.n_classes - 1 if m.ordinal else 0)   # log_dispersion / cutpoints
         for node, inputs in requests.items():
-            # families with a dispersion parameter: (intercept, beta, log_dispersion), the last one part of the key
+            # families with a dispersion parameter: (intercept, beta, log_dispersion), the last one part of the key;
+            # ordinal: (intercept, beta, cutpoints), likewise
             intercept, beta = inputs[0], inputs[1]
             ic = np.asarray(intercept, dtype=np.float32)
             parts = [ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features * C)]
-            if m.dispersion:
+            if n_third:
                 ld = np.asarray(inputs[2], dtype=np.float32)
-                parts.append(ld.reshape(1))
+                parts.append(ld.reshape(n_third))
                 disp_shapes[node] = ld.shape
             vec = np.concatenate(parts)
             key = vec.tobytes()
@@ -134,15 +136,21 @@ class NodeFederation:
             P = m.n_features
             inputs = ([theta[:, :G], theta[:, G : G + P], theta[:, G + P]] if K > 1
                       else [theta[0, :G], theta[0, G : G + P], theta[0, G + P]])
+        elif m.ordinal:
+            P = m.n_features
+            inputs = ([theta[:, :G], theta[:, G : G + P], theta[:, G + P :]] if K > 1
+                      else [theta[0, :G], theta[0, G : G + P], theta[0, G + P :]])
         else:
             inputs = [theta[:, :G], theta[:, G:]] if K > 1 else [theta[0, :G], theta[0, G:]]
-        per = m.per_node(self.engine.evaluate_raw(inputs))                         # [n_nodes, K, 1 + G + P (+ 1)]
+        # [n_nodes, K, 1 + G + P (+ 1, or + C - 1 cutpoints)]; the ordinal family's call context marks unordered chains
+        per = m.per_node(self.engine.evaluate_raw(inputs), m.call_context(inputs) if m.ordinal else None)
         out = {}
         for node in requests:
             v = per[node, chain_of[node]]
-            if m.dispersion:
-                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G : -1].copy(),
-                                              v[-1].reshape(disp_shapes[node]).copy()])
+            if n_third:
+                P = m.n_features
+                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G : 1 + G + P].copy(),
+                                              v[1 + G + P :].reshape(disp_shapes[node]).copy()])
             else:
                 out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].reshape(beta_shape).copy()])
         return out
@@ -172,7 +180,7 @@ class NodeFederation:
         * ODE: ``f(theta[n_nodes, n_params]) -> (logp, [d_theta])``;
         * GLM (parameters shared by the nodes): ``f(intercept, beta) -> (logp, [d_intercept, d_beta])``; families
           with a dispersion parameter: ``f(intercept, beta, log_dispersion) -> (logp, [d_intercept, d_beta,
-          d_log_dispersion])``.
+          d_log_dispersion])``; ordinal: ``f(intercept, beta, cutpoints) -> (logp, [d_intercept, d_beta, d_cutpoints])``.
 
         With :meth:`all_nodes_op` the model graph has ONE federated node instead of one per data holder, so the
         Python cost of a model evaluation no longer grows with the size of the federation."""
@@ -192,11 +200,11 @@ class NodeFederation:
                     th = np.broadcast_to(np.asarray(theta, dtype=np.float64), (self.n_nodes, m.n_params))
                     per = m.per_node(eng.evaluate_raw([th]))
                     return np.asarray(per[:, 0].sum()), [per[:, 1:].copy()]
-        elif getattr(eng.model, "dispersion", False):
-            def func(intercept, beta, log_dispersion):
+        elif getattr(eng.model, "dispersion", False) or getattr(eng.model, "ordinal", False):
+            def func(intercept, beta, third):   # log_dispersion or cutpoints
                 with self._lock:
                     self.n_launches += 1
-                    logp, *grads = eng.evaluate(intercept, beta, log_dispersion)
+                    logp, *grads = eng.evaluate(intercept, beta, third)
                     return logp, grads
         else:
             def func(intercept, beta):

@@ -16,7 +16,8 @@ import numpy as np
 
 from .base import ShardModel
 
-FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5}
+FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
+            "ordinal": 6}
 #: families with a learned dispersion parameter (one more input, ``log_dispersion``)
 DISPERSION_FAMILIES = ("gaussian_scale", "negative_binomial")
 
@@ -99,6 +100,25 @@ class GlmShards(ShardModel):
         which it equals at s = 0).  Offsets (``log t`` exposures of count models) and weights work as for every family.
         Counts must be integers in ``[0, 2^24]`` on every row of non-zero weight.  Only the bf16 tensor-core kernel
         evaluates these families, with the shape limits of the multinomial one; ``n_classes`` is rejected.
+
+        ``"ordinal"`` with ``n_classes=C`` is cumulative-logit (proportional-odds) regression over C ordered categories
+        (PyMC's ``OrderedLogistic``, brms' ``cumulative("logit")``): Likert scales, severity grades, ratings.  ``ys``
+        holds the categories ``0 .. C-1`` as float32, with the same label rules as the multinomial family.  The inputs
+        per call are ``(intercept, beta, cutpoints)`` — ``intercept[G]`` (a scalar when G = 1), ``beta[P]`` and
+        ``cutpoints[C-1]``, batched ``[K, G]``, ``[K, P]`` and ``[K, C-1]`` — and the gradients come back in the same
+        shapes.  With ``eta = intercept[group] + x' beta + o``, ``c_{-1} = -inf`` and ``c_{C-1} = +inf``:
+
+            P(y <= j) = sigmoid(c_j - eta),     LL = sum_i w_i log(sigmoid(c_{y_i} - eta_i) - sigmoid(c_{y_i - 1} - eta_i)).
+
+        ``2 <= C <= 17`` and ``K * (C - 1) <= 16``; the kernel and shape limits are those of the multinomial family.
+        Offsets and weights work as for every family (an offset shifts eta and does not cancel).  The intercepts and
+        the cutpoints are not identified together: adding one number to all of them leaves LL unchanged, so with
+        G = 1 one normally fixes ``intercept = 0``.  The kernel sees only ``intercept[g] - c_j``, rounded to float32:
+        a chain whose rounded values are not strictly decreasing in j for every group (cutpoints that are not
+        strictly increasing, or NaN) gets ``LL = -inf`` and zero gradients, and the other chains of the call are
+        unaffected.  Nothing is raised, so a sampler can step there and reject the proposal.  To sample, use an
+        ordered transform such as ``c = cumsum([c0, exp(d_1), ..., exp(d_{C-2})])`` and apply the chain rule to the
+        cutpoint gradient on the host: ``dLL/dc0 = sum_j dLL/dc_j``, ``dLL/dd_m = exp(d_m) sum_{j >= m} dLL/dc_j``.
     """
 
     def __init__(
@@ -163,10 +183,16 @@ class GlmShards(ShardModel):
         self.multinomial = isinstance(family, str) and family == "multinomial"
         #: the family has a log-dispersion parameter after beta (``gaussian_scale``, ``negative_binomial``)
         self.dispersion = isinstance(family, str) and family in DISPERSION_FAMILIES
+        #: cumulative-logit family: one more input, ``cutpoints[C - 1]``
+        self.ordinal = isinstance(family, str) and family == "ordinal"
+        #: columns of one launch: K, times C for the multinomial family, times C - 1 for the ordinal one
+        self.kernel_chains = self.n_chains
         if self.multinomial:
             self._init_multinomial(n_classes)
+        elif self.ordinal:
+            self._init_ordinal(n_classes)
         elif n_classes is not None:
-            raise ValueError("n_classes is for family='multinomial' only")
+            raise ValueError("n_classes is for family='multinomial' or 'ordinal' only")
         if self.dispersion:
             self._init_dispersion()
 
@@ -194,9 +220,37 @@ class GlmShards(ShardModel):
             if bool(torch.any(bad)):
                 raise ValueError(f"labels of segment {si} must be integers in [0, {C}) on every row of non-zero weight")
         self.n_classes = C
+        self.kernel_chains = self.n_chains * C
         self.n_params = C * (self.n_groups + self.n_features)
         self.n_theta_words = self.n_chains * self.n_params
         self.n_vals = self.n_nodes * self.n_chains * C * (1 + self.n_groups + self.n_features)
+
+    def _init_ordinal(self, n_classes) -> None:
+        """Checks of the ordinal family, then its sizes: G + P + C - 1 parameters per chain, and the kernel's output
+        of K (C - 1) virtual chains (one ``[LL, gi[G], g[P]]`` block per chain and cutpoint)."""
+        import torch
+
+        if self.kernel not in ("auto", "tc"):
+            raise ValueError(f"kernel={self.kernel!r}: the ordinal family runs on the bf16 tensor-core kernel only "
+                             "(kernel='tc' or 'auto')")
+        if n_classes is None or not 2 <= int(n_classes) <= 17:
+            raise ValueError(f"the ordinal family needs n_classes in [2, 17], got {n_classes}")
+        C = int(n_classes)
+        if self.n_chains * (C - 1) > 16:
+            raise ValueError(f"n_chains x (n_classes - 1) must be <= 16 (the tensor-core kernel's columns per launch), "
+                             f"got {self.n_chains} x {C - 1}")
+        for si, (y, w) in enumerate(zip(self.ys, self.weights)):
+            bad = ~((y == torch.floor(y)) & (y >= 0) & (y < C))   # NaN fails every comparison
+            if w is not None:
+                bad &= w != 0   # a masked row may carry anything
+            if bool(torch.any(bad)):
+                raise ValueError(f"labels of segment {si} must be integers in [0, {C}) on every row of non-zero weight")
+        self.n_classes = C
+        self.kernel_chains = self.n_chains * (C - 1)
+        self.n_inputs = 3
+        self.n_params = self.n_groups + self.n_features + C - 1
+        self.n_theta_words = self.kernel_chains * (self.n_groups + self.n_features)
+        self.n_vals = self.n_nodes * self.kernel_chains * (1 + self.n_groups + self.n_features)
 
     def _init_dispersion(self) -> None:
         """Checks of the families with a dispersion parameter, then their sizes: theta per chain is
@@ -258,6 +312,8 @@ class GlmShards(ShardModel):
         if self.dispersion:
             intercept, beta, log_disp = inputs
             return (np.ndim(beta) == 2, np.shape(intercept), np.shape(log_disp))
+        if self.ordinal:
+            return self._ordinal_table(inputs)[1]
         intercept, beta = inputs
         return (np.ndim(beta) == (3 if self.multinomial else 2), np.shape(intercept))
 
@@ -268,6 +324,8 @@ class GlmShards(ShardModel):
             return self._pack_theta_multinomial(inputs, out)
         if self.dispersion:
             return self._pack_theta_dispersion(inputs, out)
+        if self.ordinal:
+            return self._pack_theta_ordinal(inputs, out)
         intercept, beta = inputs
         views = self._pack_views
         if views is None or views[0] is not out:
@@ -314,9 +372,35 @@ class GlmShards(ShardModel):
         th[:, G + P] = ld.reshape(K)
         return ctx
 
+    def _ordinal_table(self, inputs):
+        """``(T, ctx)``: the kernel's intercept table ``T[K, C - 1, G] = float32(intercept[g] - c_j)`` (the difference
+        taken in double, rounded once) and the call context ``(batched, intercept shape, cutpoints shape, bad)``, with
+        ``bad`` the chains whose table is not strictly decreasing in j for every group."""
+        intercept, beta, cutpoints = inputs
+        K, G, C1 = self.n_chains, self.n_groups, self.n_classes - 1
+        ic = np.asarray(intercept, dtype=np.float64).reshape(K, G)
+        cp = np.asarray(cutpoints, dtype=np.float64).reshape(K, C1)
+        T = (ic[:, None, :] - cp[:, :, None]).astype(np.float32)
+        ordered = np.all(T[:, 1:, :] < T[:, :-1, :], axis=(1, 2))   # NaN fails the comparison
+        bad = tuple(int(k) for k in np.flatnonzero(~ordered))
+        return T, (np.ndim(beta) == 2, np.shape(intercept), np.shape(cutpoints), bad)
+
+    def _pack_theta_ordinal(self, inputs, out: np.ndarray):
+        """Theta words as ``[K (C - 1)][G + P]``: row ``k (C - 1) + j`` is ``(intercept - c_j, beta)`` of chain k, the
+        kernel's virtual chain of cutpoint j."""
+        K, C1, G, P = self.n_chains, self.n_classes - 1, self.n_groups, self.n_features
+        T, ctx = self._ordinal_table(inputs)
+        th = out.view(np.float32).reshape(K, C1, G + P)
+        th[:, :, :G] = T
+        th[:, :, G:] = np.asarray(inputs[1]).reshape(K, 1, P)
+        self._batched, self._icpt_shape, self._cut_shape, self._ord_bad = ctx
+        return ctx
+
     _batched = False
     _icpt_shape = ()
     _disp_shape = ()
+    _cut_shape = ()
+    _ord_bad = ()
 
     def _note_shapes(self, inputs):
         # single-threaded convenience state (tests call reference_partial then unpack_result);
@@ -325,13 +409,28 @@ class GlmShards(ShardModel):
         self._batched, self._icpt_shape = ctx[:2]
         if self.dispersion:
             self._disp_shape = ctx[2]
+        if self.ordinal:
+            self._cut_shape, self._ord_bad = ctx[2], ctx[3]
         return ctx
 
-    def per_node(self, vals: np.ndarray) -> np.ndarray:
+    def per_node(self, vals: np.ndarray, ctx=None) -> np.ndarray:
         """The reduced vector as ``[n_nodes, n_chains, 1 + G + P]`` (``[LL, d intercepts, d beta]`` per block).
         Multinomial: ``[n_nodes, n_chains, 1 + G C + P C]``, ``[LL, d intercept (G, C), d beta (P, C)]`` with the
         matrices row-major, summed from the kernel's blocks of the chain's C classes.  Families with a dispersion
-        parameter: ``[n_nodes, n_chains, 2 + G + P]``, ``[LL, d intercepts, d beta, d log_dispersion]``."""
+        parameter: ``[n_nodes, n_chains, 2 + G + P]``, ``[LL, d intercepts, d beta, d log_dispersion]``.  Ordinal:
+        ``[n_nodes, n_chains, 1 + G + P + C - 1]``, ``[LL, d intercepts, d beta, d cutpoints]`` from the kernel's blocks
+        ``[LL_j, gi_j[G], g_j[P]]`` of the chain's C - 1 cutpoints (``d c_j = -sum_g gi_j[g]``); the chains that
+        ``ctx`` (the call context, by default that of the last ``pack_theta``) marks as unordered get ``LL = -inf``
+        and zero gradients."""
+        if self.ordinal:
+            n, K, C1, G = self.n_nodes, self.n_chains, self.n_classes - 1, self.n_groups
+            raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C1, 1 + G + self.n_features)
+            out = np.concatenate([raw[..., 0].sum(axis=2)[..., None], raw[..., 1:].sum(axis=2),
+                                  -raw[..., 1 : 1 + G].sum(axis=3)], axis=2)
+            bad = list(ctx[3] if ctx is not None else self._ord_bad)
+            out[:, bad, 0] = -np.inf
+            out[:, bad, 1:] = 0.0
+            return out
         if self.multinomial:
             n, K, C, G = self.n_nodes, self.n_chains, self.n_classes, self.n_groups
             raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C, 1 + G + self.n_features)
@@ -345,6 +444,8 @@ class GlmShards(ShardModel):
             return self._unpack_multinomial(vals, ctx)
         if self.dispersion:
             return self._unpack_dispersion(vals, ctx)
+        if self.ordinal:
+            return self._unpack_ordinal(vals, ctx)
         v = self.per_node(vals).sum(axis=0) if self.n_nodes > 1 else np.asarray(vals, dtype=np.float64).reshape(self.n_chains, 1 + self.n_params)
         G = self.n_groups
         batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
@@ -362,6 +463,17 @@ class GlmShards(ShardModel):
                     v[:, 1 + G : 1 + G + P].copy(), v[:, 1 + G + P].reshape(disp_shape).copy()]
         return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G : 1 + G + P].copy(),
                 v[0, 1 + G + P].reshape(disp_shape).copy()]
+
+    def _unpack_ordinal(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
+        ctx = ctx if ctx is not None else (self._batched, self._icpt_shape, self._cut_shape, self._ord_bad)
+        v = self.per_node(vals, ctx).sum(axis=0)                    # [K, 1 + G + P + C - 1]
+        G, P = self.n_groups, self.n_features
+        batched, icpt_shape, cut_shape, _ = ctx
+        if batched:
+            return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
+                    v[:, 1 + G : 1 + G + P].copy(), v[:, 1 + G + P :].reshape(cut_shape).copy()]
+        return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G : 1 + G + P].copy(),
+                v[0, 1 + G + P :].reshape(cut_shape).copy()]
 
     def _unpack_multinomial(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
         v = self.per_node(vals).sum(axis=0)                         # [K, 1 + G C + P C]
@@ -385,7 +497,7 @@ class GlmShards(ShardModel):
             if X0.dtype not in (torch.bfloat16, torch.float32) or self.n_chains != 1 or self.n_features > 1024:
                 raise ValueError("custom likelihoods need a bf16/fp32 design matrix, one chain and P <= 1024")
             return 3 if X0.dtype == torch.bfloat16 else 4
-        if self.multinomial or self.dispersion:   # the bf16 tensor-core kernel or nothing: no other kernel has these
+        if self.multinomial or self.dispersion or self.ordinal:   # the bf16 tensor-core kernel or nothing: no other kernel has these
             if not (X0.dtype == torch.bfloat16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384
                     and self.n_chains <= 16 and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0):
                 raise ValueError(f"the {self.family} family runs on the bf16 tensor-core kernel only, which needs a bf16 "
@@ -449,7 +561,7 @@ class GlmShards(ShardModel):
         native.check(
             lib.b200_engine_set_glm(
                 handle, n, Xp, yp, sp, rows, grp, self.n_features, self.ld, self.n_groups,
-                self.n_chains * self.n_classes, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
+                self.kernel_chains, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
                 self.n_classes,
             ),
             "set_glm",
@@ -469,6 +581,8 @@ class GlmShards(ShardModel):
             return self._multinomial_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
         if self.dispersion:
             return self._dispersion_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
+        if self.ordinal:
+            return self._ordinal_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(self.n_chains, -1)
@@ -599,6 +713,62 @@ class GlmShards(ShardModel):
                 out[:, 1 + G + P] += q.double().sum(0)
         return full.reshape(-1).cpu().numpy()
 
+    def _ordinal_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
+        """The ordinal family's partial in the kernel's layout ``[n_nodes][K (C - 1)][1 + G + P]``: block
+        ``k (C - 1) + j`` is ``[LL_kj, gi_kj[G], g_kj[P]]`` with ``r_ikj = dll_i / dz_j`` at ``z_j = eta - c_j`` (non-zero
+        only for ``j = y_i`` and ``j = y_i - 1``) and each row's ``w ll`` credited to ``j = min(y_i, C - 2)``, as the
+        kernel does.  ``bf16_gemms``: the collective baseline, eta from one bf16 GEMM with ``beta`` as ``[P, K]``, then
+        ``X' (sum_j r_j)`` per chain in the block of cutpoint 0 (the host sums the cutpoints' blocks), fp32 elementwise
+        work; else the oracle in ``dtype``, which keeps every column's gradient block."""
+        import torch
+
+        intercept, beta, cutpoints = inputs
+        self._note_shapes(inputs)
+        K, C1, G, P = self.n_chains, self.n_classes - 1, self.n_groups, self.n_features
+        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G).to(self.device, dtype)
+        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P)
+        cp = torch.as_tensor(np.asarray(cutpoints, dtype=np.float64)).reshape(K, C1).to(self.device, dtype)
+        inf = torch.full((K, 1), float("inf"), dtype=dtype, device=self.device)
+        cpad = torch.cat([-inf, cp, inf], dim=1)                     # [K, C + 1]: c_{-1} = -inf, ..., c_{C-1} = +inf
+        B = bt.T.to(self.device, torch.bfloat16 if bf16_gemms else dtype)   # [P, K]
+        full = torch.zeros(self.n_nodes, K, C1, 1 + G + P, dtype=torch.float64, device=self.device)
+        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
+            out = full[self.node_ids[si] if self.node_ids is not None else 0]
+            w = self.weights[si]
+            for r0 in range(0, X.shape[0], chunk_rows):
+                r1 = min(X.shape[0], r0 + chunk_rows)
+                if bf16_gemms:
+                    Xf = X[r0:r1]
+                    eta = (Xf @ B).to(dtype)
+                else:
+                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
+                    eta = Xf @ B
+                eta = eta + ic[:, g]                                  # [n, K]
+                if self.offsets[si] is not None:
+                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
+                lab = y[r0:r1]
+                if w is not None:   # masked rows may carry NaN or out-of-range labels: any valid category will do
+                    lab = torch.where(w[r0:r1] != 0, lab, torch.zeros_like(lab))
+                lab = lab.long()
+                a = cpad[:, lab + 1].T - eta                          # c_y - eta = -z_up
+                b = cpad[:, lab].T - eta                              # c_{y-1} - eta = -z_lo
+                t = 1.0 / torch.expm1(a - b)                          # 1 / expm1(gap), 0 at the infinite ends
+                ll = torch.nn.functional.logsigmoid(a) + torch.nn.functional.logsigmoid(-b) + torch.log(-torch.expm1(b - a))
+                r_up = -torch.sigmoid(-a) - t
+                r_lo = torch.sigmoid(b) + t
+                hot = lambda j: torch.nn.functional.one_hot(j.clamp(0, C1 - 1), C1).to(dtype).unsqueeze(1)   # [n, 1, C1]
+                up, lo = (lab <= C1 - 1).to(dtype), (lab >= 1).to(dtype)
+                ll = ll.unsqueeze(2) * hot(torch.clamp(lab, max=C1 - 1))
+                r = (r_up * up.unsqueeze(1)).unsqueeze(2) * hot(lab) + (r_lo * lo.unsqueeze(1)).unsqueeze(2) * hot(lab - 1)
+                ll, r = self._weigh(si, r0, r1, ll, r)                # [n, K, C1]
+                out[:, :, 0] += ll.double().sum(0)
+                out[:, :, 1 + g] += r.double().sum(0)
+                if bf16_gemms:
+                    out[:, 0, 1 + G :] += (r.sum(2).T.to(torch.bfloat16) @ Xf).double()
+                else:
+                    out[:, :, 1 + G :] += (r.reshape(-1, K * C1).T @ Xf).double().reshape(K, C1, P)
+        return full.reshape(-1).cpu().numpy()
+
     def _dequant_rows(self, seg: int, r0: int, r1: int):
         """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
         return self.Xs[seg][r0:r1]
@@ -618,6 +788,8 @@ class GlmShards(ShardModel):
             return self._multinomial_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
         if self.dispersion:
             return self._dispersion_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
+        if self.ordinal:
+            return self._ordinal_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
         intercept, beta = inputs
         self._note_shapes(inputs)
         ic = torch.as_tensor(np.asarray(intercept, dtype=np.float32)).reshape(self.n_chains, -1).to(self.device)
@@ -653,7 +825,7 @@ class GlmShards(ShardModel):
         return int(sum(X.shape[0] * (self.n_features * X.element_size() + 4) for X in self.Xs)) + self._row_data_bytes()
 
     def flops_per_eval(self) -> int:
-        return int(4 * self.n_rows * self.n_features * self.n_chains * self.n_classes)
+        return int(4 * self.n_rows * self.n_features * self.kernel_chains)
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -860,6 +1032,33 @@ def synth_negative_binomial_shard(n_rows: int, n_features: int, *, alpha: float,
         lam = torch._standard_gamma(torch.full_like(mu, float(alpha)), generator=gen) * (mu / alpha)
         y[r0:r1] = torch.poisson(lam, generator=gen).float()
     return X, y, beta_true
+
+
+def synth_ordinal_shard(n_rows: int, n_features: int, n_classes: int, *, seed: int, device, chunk_rows: int = 1 << 20,
+                        beta_scale: float = 0.05, cutpoints=None):
+    """Synthetic ordinal (cumulative-logit) shard generated on the device in chunks: bf16 ``X ~ N(0,1)`` and labels
+    ``y = #{j : U > sigmoid(c_j - X beta*)}`` with ``U ~ Uniform(0, 1)``, so ``P(y <= j) = sigmoid(c_j - X beta*)``,
+    stored as float32 ``0 .. C-1``.  ``cutpoints`` (increasing, ``C - 1`` of them) default to evenly spaced values
+    in [-1.5, 1.5].  Returns ``(X, y, beta*, cutpoints)``."""
+    import torch
+
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    cuts = np.linspace(-1.5, 1.5, n_classes - 1) if cutpoints is None else np.asarray(cutpoints, dtype=np.float64)
+    if cuts.shape != (n_classes - 1,) or not np.all(np.diff(cuts) > 0):
+        raise ValueError(f"cutpoints must be {n_classes - 1} strictly increasing values")
+    c = torch.as_tensor(cuts, dtype=torch.float32, device=device)
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        cdf = torch.sigmoid(c[None, :] - (xb.float() @ beta_true)[:, None])   # [n, C - 1], P(y <= j)
+        u = torch.rand(r1 - r0, 1, generator=gen, device=device)
+        y[r0:r1] = (u > cdf).sum(1).float()
+    return X, y, beta_true, cuts.astype(np.float32)
 
 
 def synth_logistic_shard_fp8(n_rows: int, n_features: int, *, seed: int, device, chunk_rows: int = 1 << 20):

@@ -531,6 +531,18 @@ def default_inputs_from_words(model: ShardModel, words: np.ndarray):
         if model.n_chains == 1:
             return ic[0].copy(), bt[0].copy(), ld[0].copy()
         return ic.copy(), bt.copy(), ld.copy()
+    if isinstance(model, GlmShards) and model.ordinal:
+        # words [K (C - 1)][G + P], row k (C - 1) + j = (intercept - c_j, beta) of chain k.  Only the differences
+        # travel, so the inputs come back shifted to c_0 = 0 (the likelihood does not see the shift):
+        # intercept[g] = T[0, g], c_j = T[0, 0] - T[j, 0], in double, which packs back to the same words
+        G, P, C1 = model.n_groups, model.n_features, model.n_classes - 1
+        th = words.view(np.float32).reshape(model.n_chains, C1, G + P)
+        ic = th[:, 0, :G].copy()
+        cp = th[:, 0, :1].astype(np.float64) - th[:, :, 0].astype(np.float64)
+        bt = th[:, 0, G:].copy()
+        if model.n_chains == 1:
+            return ic[0], bt[0], cp[0]
+        return ic, bt, cp
     if isinstance(model, GlmShards):
         th = words.view(np.float32).reshape(model.n_chains, model.n_params)
         if model.n_chains == 1:

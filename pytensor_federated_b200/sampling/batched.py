@@ -165,17 +165,23 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
 
     A multinomial engine (``family="multinomial"``, C classes) takes ``theta = [intercept (G, C), beta (P, C)]`` per
     chain, both flattened row-major; one with a dispersion parameter (``"gaussian_scale"``, ``"negative_binomial"``)
-    takes ``theta = [intercept[G], beta[P], log_dispersion]``.  Gradients come back in the order of theta."""
+    takes ``theta = [intercept[G], beta[P], log_dispersion]``, and an ordinal one (``"ordinal"``, C categories)
+    ``theta = [intercept[G], beta[P], cutpoints[C-1]]``.  Gradients come back in the order of theta."""
     cap = int(getattr(engine.model, "n_chains", 1))
     n_classes = int(getattr(engine.model, "n_classes", 1)) if getattr(engine.model, "multinomial", False) else 1
     dispersion = bool(getattr(engine.model, "dispersion", False))
+    # trailing theta columns that form the third input: log_dispersion, or the ordinal family's C - 1 cutpoints
+    n_third = 1 if dispersion else (int(engine.model.n_classes) - 1 if getattr(engine.model, "ordinal", False) else 0)
     split = n_groups * n_classes   # theta columns that are intercepts
 
     def shaped(ic: np.ndarray, beta: np.ndarray):
         """Inputs of ``engine.evaluate``; ``ic`` / ``beta`` have the chains (if any) in their leading axis (with a
-        dispersion parameter, ``beta``'s last column is ``log_dispersion``)."""
+        dispersion parameter, ``beta``'s last column is ``log_dispersion``; ordinal: its last C - 1 columns are the
+        cutpoints)."""
         if dispersion:
             return ic, beta[..., :-1], beta[..., -1]
+        if n_third:
+            return ic, beta[..., :-n_third], beta[..., -n_third:]
         if n_classes == 1:
             return ic, beta
         lead = ic.shape[:-1]

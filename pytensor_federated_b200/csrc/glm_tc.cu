@@ -2,7 +2,8 @@
 //
 // Per 128-row tile of the bf16 design matrix X (read from HBM exactly ONCE per evaluation):
 //
-//   TMA        X[128 x P] -> smem, 128B-swizzled 64-feature panels (cp.async.bulk.tensor)
+//   TMA        X[128 x P] -> smem, 128B-swizzled 64-feature panels (cp.async.bulk.tensor), and the tile's
+//              128 responses (offsets, weights) -> the stage's row slot, on the same mbarrier
 //   MMA #1     eta[128 x N1] = X_tile (A, K-major) . Theta^T (B, K-major)      -> registers
 //              Theta holds, per MCMC chain, a 3-way bf16 split (hi, mid, lo) of the fp32
 //              coefficients, so eta keeps ~fp32 accuracy although the operands are bf16.
@@ -44,36 +45,50 @@ constexpr int kRing = 16;            // published chunks the consumers may lag b
 constexpr int kLLRows = 16;          // per-warp log-likelihood slot rows (>= kConsumerWarps)
 
 struct SmemLayout {
-    uint32_t stages, stage_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_theta_f, off_icpt, off_ring,
-        off_bars, total, preload;
+    uint32_t stages, stage_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_rows, row_bytes, off_theta_f,
+        off_disp, off_ring, off_bars, total, preload;
 };
-__host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_theta, int n_groups, int chains) {
+// chain_words: per-chain fp32 constants kept in shared memory next to the chunk's intercept column (kDispWords for
+// the dispersion families, else 0);
+// row_arrays: fp32 per-row arrays a tile carries (y, and the offsets / weights the launch has: 1 to 3)
+__host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_theta, int chain_words, int chains,
+                                                  int row_arrays) {
     SmemLayout L;
     const uint32_t panels = P / kPanel;
     L.stage_bytes = panels * kPanelBytes;
     L.theta_b_bytes = panels * n1 * 128;
     L.r_bytes = kTileM * n2 * 2;
+    // the row slot of a stage (its tile's y, offset, weight) lies outside the ring, whose last stage the fp32
+    // theta staging aliases; it is paid for per stage when the stage count is chosen
+    L.row_bytes = (uint32_t)row_arrays * kTileM * 4;
     // theta (fp32) is staged inside the TMA stage ring and is dead once the bf16 B operand and the intercept
     // table are built, so it costs no shared memory of its own.
-    const uint32_t fixed = L.theta_b_bytes + 2 * L.r_bytes + ((chains * n_groups * 4 + 15) & ~15) + kRing * 24 + 192 +
+    const uint32_t fixed = L.theta_b_bytes + 2 * L.r_bytes + ((chains * (1 + chain_words) * 4 + 15) & ~15) + kRing * 24 + 192 +
                            1024 /*alignment slack*/;
-    uint32_t stages = (227u * 1024u - fixed) / L.stage_bytes;
+    uint32_t stages = (227u * 1024u - fixed) / (L.stage_bytes + L.row_bytes);
     if (stages > 4) stages = 4;
     L.stages = stages;
     uint32_t o = stages * L.stage_bytes;
     L.off_theta_b = o; o += L.theta_b_bytes;
     L.off_r = o; o += 2 * L.r_bytes;
+    L.off_rows = o; o += stages * L.row_bytes;   // 512-byte multiples: 16-byte aligned like every TMA destination
     // theta (fp32) sits in the LAST stage when it fits into one: the TMA warp fills the first stages - 1 stages
     // with this CTA's first tiles BEFORE theta has arrived (`preload`), the last stage is free once the B
     // operand is built.  (larger theta: stage 0 onwards, needs n_theta * 4 <= stages * stage_bytes, no preload)
     const bool theta_in_last = (uint32_t)n_theta * 4u <= L.stage_bytes && stages >= 2;
     L.off_theta_f = theta_in_last ? (stages - 1) * L.stage_bytes : 0;
     L.preload = theta_in_last ? stages - 1 : 0;
-    L.off_icpt = o; o += (chains * n_groups * 4 + 15) & ~15;
+    L.off_disp = o; o += (chains * (1 + chain_words) * 4 + 15) & ~15;   // intercept column, then the constants
     L.off_ring = o; o += kRing * 24;   // published chunks + one mbarrier per ring slot
     L.off_bars = o; o += 192;
     L.total = o + 1024;
     return L;
+}
+
+// fp32 arrays in a stage's row slot (host and device agree through this): y, then the offsets and the weights
+// when ROWS and some segment of the launch has them (GlmParams::row_data)
+__host__ __device__ inline int row_arrays(bool rows, int row_data) {
+    return 1 + (rows && (row_data & kGlmRowOffsets) ? 1 : 0) + (rows && (row_data & kGlmRowWeights) ? 1 : 0);
 }
 
 // KC = chains per launch; ROWS = some segment has per-row offsets or weights (GlmSegment::offset / weight), so
@@ -98,8 +113,13 @@ struct Cfg {
 // doubles per CTA row of the partial array: (hi, lo) pairs of the n_vals outputs, then the per-warp slots of
 // the values that a whole warp contributes to — [kLLRows][n_out][KC][1 + G + disp]: log-likelihood, the G
 // intercept gradients and (disp = 1: families with a dispersion parameter) its gradient, of every (output block, chain)
-__host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int n_out, int n_groups, int disp = 0) {
+// — the part the launch sums (`partial_sum_doubles`) —, then the CTA's intercept table [KC][G] as floats, padded to
+// an even number of doubles so that every row stays 16-byte aligned
+__host__ __device__ constexpr size_t partial_sum_doubles(int n_vals, int kc, int n_out, int n_groups, int disp = 0) {
     return 2 * ((size_t)n_vals + (size_t)kLLRows * n_out * kc * (1 + n_groups + disp));
+}
+__host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int n_out, int n_groups, int disp = 0) {
+    return partial_sum_doubles(n_vals, kc, n_out, n_groups, disp) + ((size_t)kc * n_groups + 3) / 4 * 2;
 }
 
 // Work is handed out in CHUNKS of consecutive tiles of one segment (host-built table: 32 tiles while much
@@ -126,8 +146,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                       // Theta rows are zero and their gradient rows are never stored
     const int G = prm.n_groups;
     const int panels = PP / kPanel;
-    // DISP: the intercept table [KC][G] is followed by the per-chain dispersion constants [KC][kDispWords]
-    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, G + (DISP ? kDispWords : 0), KC);
+    // row slot of a stage: y, then the offsets and the weights when some segment of the launch has them
+    const int o_slot = 1, w_slot = ROWS && (prm.row_data & kGlmRowOffsets) ? 2 : 1;
+    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, DISP ? kDispWords : 0, KC, row_arrays(ROWS, prm.row_data));
     const int S = (int)L.stages;
     const int nch = prm.n_chains < KC ? prm.n_chains : KC;  // chains actually present in theta
     const int NV1 = 1 + G + P + DISP; // outputs per chain: [LL, gi[G], g[P]] (DISP: and dlog_dispersion)
@@ -135,9 +156,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     unsigned char* theta_b = smem + L.off_theta_b;
     unsigned char* r_buf = smem + L.off_r;
     float* theta_f = reinterpret_cast<float*>(smem + L.off_theta_f);  // valid until the setup barrier only
-    float* icpt = reinterpret_cast<float*>(smem + L.off_icpt);        // [KC][G] intercepts
-    float* disp = icpt + KC * G;                                        // DISP: [KC][kDispWords] per-chain constants
-    int4* ring = reinterpret_cast<int4*>(smem + L.off_ring);          // (segment or -1, first row, tiles, -)
+    float* icpt = reinterpret_cast<float*>(smem + L.off_disp);        // [KC]: intercepts of the current chunk's group
+    float* disp = icpt + KC;                                            // DISP: [KC][kDispWords] per-chain constants
+    int4* ring = reinterpret_cast<int4*>(smem + L.off_ring);          // (segment or -1, first row, tiles, group)
     uint64_t* bar_ring = reinterpret_cast<uint64_t*>(smem + L.off_ring + kRing * 16);   // slot j % kRing: chunk j published
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
     uint64_t* bar_full = bars;            // [4] X stage landed
@@ -154,8 +175,32 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (int i = 0; i < 4; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 32 * kConsumerWarps); }
         fence_barrier_init();
     }
+    // tmaps[4 s + a]: X, y, offset, weight of segment s (the last two only where the segment has them)
     if (warp == 0 && lane == 0)
-        for (int i = 0; i < prm.n_segments; ++i) tma_prefetch_desc(&tmaps[i]);
+        for (int i = 0; i < prm.n_segments; ++i) {
+            tma_prefetch_desc(&tmaps[4 * i]);
+            tma_prefetch_desc(&tmaps[4 * i + 1]);
+            if (ROWS && segs_g[i].offset) tma_prefetch_desc(&tmaps[4 * i + 2]);
+            if (ROWS && segs_g[i].weight) tma_prefetch_desc(&tmaps[4 * i + 3]);
+        }
+    // One tile into stage st, issued by one lane: the X panels and the tile's row data (y, then, ROWS, offset and
+    // weight where the segment has them: bit 0 / bit 1 of `rows`) into the stage's row slot, all counted on full[st].
+    // TMA zero-fills rows past the segment's end.
+    auto load_tile = [&](int st, int seg, int row0, int rows) {
+        const CUtensorMap* m = tmaps + 4 * seg;
+        float* slot = reinterpret_cast<float*>(smem + L.off_rows + (size_t)st * L.row_bytes);
+        mbar_expect_tx(&bar_full[st], L.stage_bytes + kTileM * 4 * (1 + (rows & 1) + (rows >> 1)));
+        for (int pnl = 0; pnl < panels; ++pnl)
+            tma_load_2d(smem + (size_t)st * L.stage_bytes + pnl * kPanelBytes, m, pnl * kPanel, row0, &bar_full[st]);
+        tma_load_1d(slot, m + 1, row0, &bar_full[st]);
+        if (rows & 1) tma_load_1d(slot + o_slot * kTileM, m + 2, row0, &bar_full[st]);
+        if (rows & 2) tma_load_1d(slot + w_slot * kTileM, m + 3, row0, &bar_full[st]);
+    };
+    // the row arrays of segment seg that the producer loads (bit 0: offset, bit 1: weight)
+    auto seg_row_mask = [&](int seg) -> int {
+        if constexpr (!ROWS) return 0;
+        return (segs_g[seg].offset ? 1 : 0) | (segs_g[seg].weight ? 2 : 0);
+    };
     // Early loads: X does not depend on theta.  The TMA warp waits for the previous evaluation to retire (its
     // last CTA re-arms the work counter), claims this CTA's first chunk and fills all stages but the one theta
     // is staged in, so the tensor core has `preload` tiles waiting when theta arrives (peers see theta several
@@ -171,14 +216,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             const GlmChunk ch = chunks[claim0];
             preloaded = ch.n_tiles < (int)L.preload ? ch.n_tiles : (int)L.preload;
             if (!prm.early_loads) preloaded = 0;
-            if (elect_one()) {
-                for (int t = 0; t < preloaded; ++t) {
-                    mbar_expect_tx(&bar_full[t], L.stage_bytes);
-                    for (int pnl = 0; pnl < panels; ++pnl)
-                        tma_load_2d(smem + (size_t)t * L.stage_bytes + pnl * kPanelBytes, &tmaps[ch.seg], pnl * kPanel,
-                                    (ch.first_tile + t) * kTileM, &bar_full[t]);
-                }
-            }
+            const int rows = seg_row_mask(ch.seg);
+            if (elect_one())
+                for (int t = 0; t < preloaded; ++t) load_tile(t, ch.seg, (ch.first_tile + t) * kTileM, rows);
             __syncwarp();
         }
     }
@@ -189,13 +229,17 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     const int NS1 = 1 + G + DISP;     // warp-level values per (block, chain): LL, the G intercept gradients (and q)
     const size_t row_doubles = partial_row_doubles(comm.n_vals, KC, NOUT, G, DISP);
     double* out = comm.cta_partials + (size_t)blockIdx.x * row_doubles;   // this CTA's running sums, (hi, lo) pairs
+    const size_t sum_doubles = partial_sum_doubles(comm.n_vals, KC, NOUT, G, DISP);
+    // [KC][G] intercepts, in global memory so that the shared memory budget does not grow with G: written in the
+    // setup below, read by this CTA only (after __syncthreads), one column into `icpt` per chunk
+    float* icpt_table = reinterpret_cast<float*>(out + sum_doubles);
     double* ll_slots = out + 2 * (size_t)comm.n_vals;                     // [kLLRows][NOUT][KC][NS1] pairs
 
     if (active) {
         // ---------------- theta-dependent setup --------------------------------------------------
-        for (size_t i = threadIdx.x; i < row_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
+        for (size_t i = threadIdx.x; i < sum_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
-            icpt[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
+            icpt_table[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
         if constexpr (DISP)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
@@ -244,6 +288,10 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             mbar_wait(&bar_ring[slot], (uint32_t)((j / kRing) & 1));
             named_sync(1, 256);
             if (threadIdx.x == 128) *chunk_decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[slot];
+            // the intercepts of the chunk's group (ring entry .w); every reader of the previous column has passed the
+            // barrier above
+            if (threadIdx.x >= 128 && threadIdx.x < 128 + KC && !*pipeline_fault() && ring[slot].x >= 0)
+                icpt[threadIdx.x - 128] = __ldcg(icpt_table + (threadIdx.x - 128) * G + ring[slot].w);
             named_sync(1, 256);
             return *chunk_decided;
         };
@@ -259,12 +307,14 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 GlmChunk ch{};
                 if (have) ch = chunks[claim];
                 if (lane == 0) {
-                    ring[j & (kRing - 1)] = have ? make_int4(ch.seg, ch.first_tile * kTileM, ch.n_tiles, 0) : make_int4(-1, 0, 0, 0);
+                    ring[j & (kRing - 1)] = have ? make_int4(ch.seg, ch.first_tile * kTileM, ch.n_tiles, segs_g[ch.seg].group)
+                                                 : make_int4(-1, 0, 0, 0);
                     mbar_arrive(&bar_ring[j & (kRing - 1)]);
                     if (have) ahead = atomicAdd(work_counter, 1u);   // next claim: the round trip hides behind this chunk
                 }
                 __syncwarp();
                 if (!have) break;
+                const int rows = seg_row_mask(ch.seg);
                 for (int t = 0; t < ch.n_tiles; ++t) {
                     const int st = stage.idx;
                     if (j == 0 && t < preloaded) {   // already in flight (early loads)
@@ -273,13 +323,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                     }
                     mbar_wait(&bar_empty[st], stage.phase ^ 1);
                     if (j == 0 && t == preloaded && lane == 0) fed::stamp(comm, 3);
-                    const int row0 = (ch.first_tile + t) * kTileM;
-                    unsigned char* dst = smem + (size_t)st * L.stage_bytes;
-                    if (elect_one()) {
-                        mbar_expect_tx(&bar_full[st], L.stage_bytes);
-                        for (int pnl = 0; pnl < panels; ++pnl)
-                            tma_load_2d(dst + pnl * kPanelBytes, &tmaps[ch.seg], pnl * kPanel, row0, &bar_full[st]);
-                    }
+                    if (elect_one()) load_tile(st, ch.seg, (ch.first_tile + t) * kTileM, rows);
                     __syncwarp();
                     stage.advance(S);
                 }
@@ -338,9 +382,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             for (int j = 0;; ++j) {
                 const int4 ch = consumer_chunk(j);
                 if (ch.x < 0) break;
-                const float* __restrict__ seg_y = segs_g[ch.x].y;   // segment table: global, read once per chunk
-                const float* __restrict__ seg_o = ROWS ? segs_g[ch.x].offset : nullptr;   // null: absent (chunk-uniform)
-                const float* __restrict__ seg_w = ROWS ? segs_g[ch.x].weight : nullptr;
+                // segment table: global, read once per chunk; an absent offset / weight reads as 0 / 1 (chunk-uniform)
+                const bool has_o = ROWS && segs_g[ch.x].offset != nullptr;
+                const bool has_w = ROWS && segs_g[ch.x].weight != nullptr;
                 const long long seg_rows = segs_g[ch.x].n_rows;
                 const int seg_group = segs_g[ch.x].group;
                 const int og = segs_g[ch.x].out_group;               // output block of this chunk's segment
@@ -348,21 +392,10 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                 for (int s = 0; s < 2 * NJ; ++s) ll_acc[s] = gi_acc[s] = ds_acc[s] = 0.f;
                 for (int t = 0; t < ch.z; ++t) {
-                    // row data: y, offset and weight of this thread's two rows, loaded before the tile is waited for
-                    // and MMA #1 runs, so three dependent global reads do not sit between the two GEMMs
-                    float y_r[2], o_r[2], w_r[2];
-                    if constexpr (ROWS) {
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const long long grow = (long long)ch.y + (long long)t * kTileM + 64 * c + 16 * w + (lane >> 2) + 8 * h;
-                            const bool valid = grow < seg_rows;
-                            y_r[h] = valid ? __ldg(seg_y + grow) : 0.f;
-                            o_r[h] = valid && seg_o ? __ldg(seg_o + grow) : 0.f;
-                            w_r[h] = valid && seg_w ? __ldg(seg_w + grow) : 1.f;
-                        }
-                    }
                     mbar_wait(&bar_full[stage.idx], stage.phase);
                     const uint32_t x_a = x_base_a + (uint32_t)stage.idx * L.stage_bytes;
+                    // y, offset, weight of the tile's rows: landed with X (the TMA producer loads them into the stage's slot)
+                    const float* row_slot = reinterpret_cast<const float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
                     // ---- MMA #1: eta of this group's 64 rows
                     float eacc[N1 / 2];
 #pragma unroll
@@ -387,13 +420,12 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                         const int row = 64 * c + 16 * w + (lane >> 2) + 8 * h;   // row of the tile
                         const long long grow = (long long)ch.y + (long long)t * kTileM + row;
                         const bool valid = grow < seg_rows;
-                        float y, o = 0.f, wt = 1.f;   // response, offset and weight of the row
+                        // response, offset and weight of the row
+                        const float y = valid ? row_slot[row] : 0.f;
+                        float o = 0.f, wt = 1.f;
                         if constexpr (ROWS) {
-                            y = y_r[h];
-                            o = o_r[h];
-                            wt = w_r[h];
-                        } else {
-                            y = valid ? __ldg(seg_y + grow) : 0.f;
+                            o = valid && has_o ? row_slot[o_slot * kTileM + row] : 0.f;
+                            wt = valid && has_w ? row_slot[w_slot * kTileM + row] : 1.f;
                         }
                         // SOFTMAX: the row's log-sum-exp per chain over the quad; every lane takes part, whether its
                         // row is valid or not (a row past the segment is dropped below, as in the other families)
@@ -408,7 +440,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 // index stays inside the table whatever G is
                                 const int k = sm_chain[s] >= 0 ? 8 * jc + 2 * q + e : 0;
                                 sm_eta[s] = ((eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
-                                             eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k * G + seg_group];
+                                             eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k];
                                 sm_ll[s] = sm_r[s] = 0.f;
                             }
                             softmax_loglik<2 * NJ, KC / 2>(sm_eta, sm_chain, sm_cls, sm_chains, y, sm_ll, sm_r);
@@ -424,11 +456,11 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 const int jc = s >> 1, e = s & 1;
                                 const int k = od_chain[s] >= 0 ? 8 * jc + 2 * q + e : 0;   // as in SOFTMAX
                                 z[s] = ((eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
-                                        eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k * G + seg_group];
+                                        eacc[4 * (2 * NJ + jc) + 2 * h + e]) + icpt[k];
                                 if constexpr (ROWS) z[s] = __fadd_rn(z[s], o);
                             }
                             const int yi = min(max(__float2int_rz(y), 0), od_ncut);   // NaN -> 0
-                            ordinal_loglik<2 * NJ, KC>(z, od_chain, od_cut, od_chains, od_ncut, yi, icpt + seg_group, G,
+                            ordinal_loglik<2 * NJ, KC>(z, od_chain, od_cut, od_chains, od_ncut, yi, icpt, 1,
                                                        od_ll, od_r);
                         }
 #pragma unroll
@@ -442,7 +474,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                 if (valid && k < nch) {
                                     if constexpr (DISP) {
                                         // offset and weight as in ROWS, the weight applied to all three values
-                                        float et = eta + icpt[k * G + seg_group];
+                                        float et = eta + icpt[k];
                                         if constexpr (ROWS) et = __fadd_rn(et, o);
                                         const float* dt = disp + k * kDispWords;   // k < nch <= KC: inside the table
                                         if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
@@ -472,11 +504,11 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                         // offset after the intercept, weight after the likelihood, both rounded on their
                                         // own (no FMA contraction): w = 1, o = 0 gives the bits of the plain model; a
                                         // zero weight selects 0, so a masked row's non-finite y or o never reaches a sum
-                                        link_loglik(prm.family, y, __fadd_rn(eta + icpt[k * G + seg_group], o), ll, r);
+                                        link_loglik(prm.family, y, __fadd_rn(eta + icpt[k], o), ll, r);
                                         ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
                                         r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
                                     } else {
-                                        link_loglik(prm.family, y, eta + icpt[k * G + seg_group], ll, r);
+                                        link_loglik(prm.family, y, eta + icpt[k], ll, r);
                                     }
                                 }
                                 ll_acc[2 * jc + e] += ll;
@@ -602,8 +634,9 @@ EncodeTiledFn get_encode() {
 int chains_bucket(int k) { return k <= 1 ? 1 : (k <= 4 ? 4 : (k <= 8 ? 8 : (k <= 16 ? 16 : 0))); }
 }  // namespace
 
-// Builds one TMA descriptor per segment ([n_rows, P] bf16, box = 64 features x 128 rows, 128B swizzle) and
-// the chunk table.
+// Builds the TMA descriptors of every segment, [n_segments][4]: X ([n_rows, P] bf16, box = 64 features x 128 rows,
+// 128B swizzle), then y, offset and weight ([n_rows] fp32, box = 128 rows; an absent offset / weight keeps a zeroed
+// descriptor the kernel never uses), and the chunk table.  Every check comes before the first device allocation.
 extern "C" int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count,
                                    void** tmaps_dev, void** chunks_dev, int* n_chunks) {
     if (prm->n_features % 8 != 0 || prm->n_features > 384 || prm->n_features < 8) return -11;   // padded to 128s by TMA
@@ -611,24 +644,36 @@ extern "C" int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, 
     if ((prm->ld * 2) % 16 != 0) return -14;
     EncodeTiledFn encode = get_encode();
     if (!encode) return -15;
-    for (int s = 0; s < n_segments; ++s)
-        if (segs_host[s].n_rows + tc::kTileM >= (1ll << 31)) return -18;   // row coordinates are 32-bit
-    CUtensorMap* host = new CUtensorMap[n_segments];
     for (int s = 0; s < n_segments; ++s) {
-        if (((uintptr_t)segs_host[s].X & 15) != 0) { delete[] host; return -16; }
+        const GlmSegment& g = segs_host[s];
+        if (g.n_rows + tc::kTileM >= (1ll << 31)) return -18;   // row coordinates are 32-bit
+        if (((uintptr_t)g.X & 15) != 0) return -16;            // TMA reads from 16-byte aligned addresses only
+        if ((((uintptr_t)g.y | (uintptr_t)g.offset | (uintptr_t)g.weight) & 15) != 0) return -19;
+    }
+    std::vector<CUtensorMap> host((size_t)n_segments * 4);   // value-initialised: zeroed
+    for (int s = 0; s < n_segments; ++s) {
         cuuint64_t dims[2] = {(cuuint64_t)prm->n_features, (cuuint64_t)segs_host[s].n_rows};
         cuuint64_t strides[1] = {(cuuint64_t)prm->ld * 2};
         cuuint32_t box[2] = {(cuuint32_t)tc::kPanel, (cuuint32_t)tc::kTileM};
         cuuint32_t estr[2] = {1, 1};
-        CUresult r = encode(&host[s], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(segs_host[s].X), dims, strides,
+        CUresult r = encode(&host[4 * s], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(segs_host[s].X), dims, strides,
                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { delete[] host; return -17; }
+        const float* rows[3] = {segs_host[s].y, segs_host[s].offset, segs_host[s].weight};
+        for (int a = 0; a < 3 && r == CUDA_SUCCESS; ++a) {
+            if (!rows[a]) continue;
+            cuuint64_t rdims[1] = {(cuuint64_t)segs_host[s].n_rows};
+            cuuint64_t rstrides[1] = {4};   // unused at rank 1
+            cuuint32_t rbox[1] = {(cuuint32_t)tc::kTileM};
+            r = encode(&host[4 * s + 1 + a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, const_cast<float*>(rows[a]), rdims, rstrides,
+                       rbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                       CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        }
+        if (r != CUDA_SUCCESS) return -17;
     }
     if (*tmaps_dev) cudaFree(*tmaps_dev);
-    cudaError_t e = cudaMalloc(tmaps_dev, sizeof(CUtensorMap) * n_segments);
-    if (e == cudaSuccess) e = cudaMemcpy(*tmaps_dev, host, sizeof(CUtensorMap) * n_segments, cudaMemcpyHostToDevice);
-    delete[] host;
+    cudaError_t e = cudaMalloc(tmaps_dev, sizeof(CUtensorMap) * host.size());
+    if (e == cudaSuccess) e = cudaMemcpy(*tmaps_dev, host.data(), sizeof(CUtensorMap) * host.size(), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) return (int)e;
     const std::vector<GlmChunk> chunks = build_chunks(segs_host, n_segments, sm_count > 0 ? sm_count : 132, tc::kTileM, 2,
                                                         tc::kMaxChunk, tc::kMinChunk);
@@ -660,6 +705,17 @@ extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int 
     return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups, dispersion ? 1 : 0);
 }
 
+// Stages of the TMA ring the launch of this shape gets (host only; tests/test_glm_row_stream.py).  The launch
+// needs at least 2.
+extern "C" int b200_glm_tc_stages(int n_features, int n_chains, int n_groups, int family, int row_data) {
+    const int kc = chains_bucket(n_chains);
+    if (kc == 0) return 0;
+    const int n1 = kc <= 8 ? 24 : 48, n2 = ((2 * kc + 7) / 8) * 8;   // Cfg<kc>
+    const bool disp = family == 4 || family == 5;
+    return (int)tc::smem_layout((n_features + 127) & ~127, n1, n2, 0, disp ? tc::kDispWords : 0, kc,
+                                tc::row_arrays(row_data != 0, row_data)).stages;
+}
+
 extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps,
                                   const void* chunks_dev, int n_chunks, unsigned int* work_counter, int grid,
                                   cudaStream_t stream) {
@@ -669,7 +725,7 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
 #define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD)                                                                    \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
-                                                 prm->n_groups + (DISP ? tc::kDispWords : 0), KC);                 \
+                                                 DISP ? tc::kDispWords : 0, KC, tc::row_arrays(ROWS, prm->row_data)); \
         if (L.stages < 2) return -2;                                                                               \
         cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \

@@ -610,7 +610,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         return -33;
     }
     const int tile_rows = (use_tensor_cores == 1 || use_tensor_cores == 2) ? 128 : 8;
-    e->glm_segs.resize(n_segments);
+    std::vector<GlmSegment> segs(n_segments);   // the engine's model changes only once every check has passed
     long long tiles = 0;
     int row_data = 0;
     for (int s = 0; s < n_segments; ++s) {
@@ -630,15 +630,28 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
             g_last_error = "segment output block out of range";
             return -31;
         }
-        e->glm_segs[s] = g;
+        segs[s] = g;
         tiles += (n_rows[s] + tile_rows - 1) / tile_rows;
     }
-    e->glm = GlmParams{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
-                       early_loads_enabled() ? 1 : 0, row_data, n_classes};
-    if (!dispersion && (long long)e->glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
+    const GlmParams glm{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
+                        early_loads_enabled() ? 1 : 0, row_data, n_classes};
+    if (!dispersion && (long long)glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
         g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
         return -33;
     }
+    // the bf16 tensor-core kernel checks the shape and the alignment of every array it reads through TMA before
+    // anything is committed, so a refused model leaves the engine evaluating the one it had
+    if (use_tensor_cores == 1) {
+        int rc = b200_glm_tc_prepare(segs.data(), n_segments, &glm, e->sm_count, &e->glm_tmaps_dev, &e->glm_chunks_dev,
+                                     &e->glm_n_chunks);
+        if (rc != 0) {
+            g_last_error = rc == -19 ? "tensor-core GLM path: y, offsets and weights must be 16-byte aligned (rc=-19)"
+                                     : "tensor-core GLM path rejected this shape (rc=" + std::to_string(rc) + ")";
+            return rc;
+        }
+    }
+    e->glm_segs = segs;
+    e->glm = glm;
     if (e->glm_segs_dev) cudaFree(e->glm_segs_dev);
     CK(cudaMalloc((void**)&e->glm_segs_dev, sizeof(GlmSegment) * (n_segments > 0 ? n_segments : 1)));
     CK(cudaMemcpy(e->glm_segs_dev, e->glm_segs.data(), sizeof(GlmSegment) * n_segments, cudaMemcpyHostToDevice));
@@ -661,13 +674,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         e->kind = MODEL_GLM_FP8;
         e->grid = e->sm_count;
         if (e->glm_n_chunks > 0 && e->grid > e->glm_n_chunks) e->grid = e->glm_n_chunks;
-    } else if (use_tensor_cores) {
-        int rc = b200_glm_tc_prepare(e->glm_segs.data(), n_segments, &e->glm, e->sm_count, &e->glm_tmaps_dev,
-                                     &e->glm_chunks_dev, &e->glm_n_chunks);
-        if (rc != 0) {
-            g_last_error = "tensor-core GLM path rejected this shape (rc=" + std::to_string(rc) + ")";
-            return rc;
-        }
+    } else if (use_tensor_cores) {   // prepared above
         e->tc_row_doubles = b200_glm_tc_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups, dispersion ? 1 : 0);
         if (e->tc_partials) cudaFree(e->tc_partials);
         const size_t tc_doubles = (size_t)e->sm_count * e->tc_row_doubles + ((size_t)e->sm_count / 16 + 2) * e->n_vals * 2;

@@ -81,6 +81,13 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
         : "memory");
 }
+__device__ __forceinline__ void tma_load_1d(void* smem_dst, const CUtensorMap* map, int c0, uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2}], [%3];" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(map), "r"(c0), "r"(smem_u32(bar))
+        : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
@@ -303,7 +310,7 @@ __device__ __forceinline__ void ordinal_terms(float u, float l, float d, bool up
 // up = yi (if yi < n_cut) and lo = yi - 1 (if yi > 0): per chain, their z are summed over the quad with xor-1 / xor-2
 // shuffles, which every lane runs for every chain below n_chains (warp-uniform); a lane holding neither column
 // adds 0, so the sums are exact and all four lanes get the same bits.  The gap l - u is taken from the intercept
-// table, icpt[(k, yi - 1)] - icpt[(k, yi)] of the row's group (icpt_g points at column g of the [KC][G] table): the
+// table, icpt[(k, yi - 1)] - icpt[(k, yi)] of the row's group (icpt_g[v * G]: intercept row v of the row's group): the
 // difference of two packed fp32 values, > 0 whenever the host accepted the cutpoints as ordered, and accurate to
 // ulp(|intercept - c|) rather than ulp(|z|).  Results: ll[s] = the chain's ll in column min(yi, n_cut - 1) and 0
 // elsewhere, r[s] = r_up / r_lo in the up / lo columns and 0 elsewhere.

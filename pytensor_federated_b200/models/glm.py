@@ -26,6 +26,12 @@ def _family_code(family) -> int:
     return family.code_id if hasattr(family, "code_id") else FAMILIES[family]
 
 
+def _aligned16(t):
+    """``t``, or a copy of it when its storage does not start on a 16-byte boundary (a view such as ``y[1:]``): the
+    tensor-core kernel streams per-row arrays with TMA, which reads from 16-byte aligned addresses only."""
+    return t.clone() if t.data_ptr() % 16 != 0 else t
+
+
 class GlmShards(ShardModel):
     """The GLM segments that live on ONE GPU.
 
@@ -52,8 +58,8 @@ class GlmShards(ShardModel):
         one-Op-per-node pattern (``demo_model.py:28-36``) answered by one launch.
     offsets, weights
         Per-row data, ``None`` or one entry per segment: ``None`` (no offset / weight 1 for that segment) or a 1-D
-        tensor of the segment's ``n_rows`` (converted once to contiguous float32; a tensor must already live on the
-        device of X).  Every kernel evaluates
+        tensor of the segment's ``n_rows`` (converted once to contiguous, 16-byte aligned float32, as ``ys`` are; a
+        tensor must already live on the device of X).  Every kernel evaluates
 
             eta_i = intercept[group] + x_i' beta + o_i,     LL = sum_i w_i ll(y_i, eta_i),
             dLL/dbeta = sum_i w_i r_i x_i,   dLL/dintercept[g] = sum_{i in g} w_i r_i,   r_i = dll/deta at eta_i,
@@ -143,7 +149,7 @@ class GlmShards(ShardModel):
         if len(Xs) != len(ys):
             raise ValueError("Xs and ys must have the same length")
         self.Xs = list(Xs)
-        self.ys = [y.to(torch.float32).contiguous() for y in ys]
+        self.ys = [_aligned16(y.to(torch.float32).contiguous()) for y in ys]
         self.weights = self._row_data(weights, "weights")
         self.offsets = self._row_data(offsets, "offsets")
         for si, (o, w) in enumerate(zip(self.offsets, self.weights)):
@@ -293,7 +299,7 @@ class GlmShards(ShardModel):
                 v = torch.as_tensor(np.asarray(v), device=X.device)
             if v.dim() != 1 or v.shape[0] != X.shape[0]:
                 raise ValueError(f"{name} of segment {si} must be 1-D with {X.shape[0]} rows, got shape {tuple(v.shape)}")
-            out.append(v.to(torch.float32).contiguous())
+            out.append(_aligned16(v.to(torch.float32).contiguous()))
         return out
 
     @property

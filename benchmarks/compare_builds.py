@@ -5,7 +5,8 @@ Each tree first builds its own library in place (``__graft_entry__.build()``).  
 runs as a subprocess alternately in the base tree and in this one, ``--rounds`` times each, so drift of a shared
 machine hits both sides alike.  Every run passes ``--dump-outputs`` to a temporary directory, and the dumps of all
 runs are compared bit for bit with the first base run's.  Prints one JSON line: per side the ``value`` (evals/s)
-and ``ms_per_step`` of every round with median / min / max, the median head / base ratio, each run's clocks
+and ``ms_per_step`` of every round with median / min / max, the same for ``e2e.value`` (the end-to-end rate, which
+includes the host's packing and unpacking), the median head / base ratios, each run's clocks
 block, whether the outputs are bitwise equal, and the card's name and power limit read in the same call.
 
     python benchmarks/compare_builds.py --base /path/to/parent-export [--rounds 5] [-- bench.py arguments]
@@ -69,9 +70,11 @@ def dumps_equal(a: str, b: str) -> bool:
 
 def summary(lines: list) -> dict:
     vals = [ln["value"] for ln in lines]
+    e2e = [ln["e2e"]["value"] for ln in lines]
     ms = [ln["ms_per_step"] for ln in lines]
     return {
         "value": vals, "value_median": statistics.median(vals), "value_min": min(vals), "value_max": max(vals),
+        "e2e_value": e2e, "e2e_median": statistics.median(e2e), "e2e_min": min(e2e), "e2e_max": max(e2e),
         "ms_per_step": ms, "ms_median": statistics.median(ms), "ms_min": min(ms), "ms_max": max(ms),
         "verified": all(ln.get("verified") for ln in lines),
         "clocks": [ln.get("clocks") for ln in lines],
@@ -115,6 +118,7 @@ def main() -> None:
         "base": b,
         "head": h,
         "ratio_head_over_base": h["value_median"] / b["value_median"],
+        "e2e_ratio_head_over_base": h["e2e_median"] / b["e2e_median"],
         "every_head_faster": min(h["value"]) > max(b["value"]),
         "outputs_bitwise_equal": equal,
         "card": card,

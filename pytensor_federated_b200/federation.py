@@ -95,27 +95,15 @@ class NodeFederation:
 
     def _evaluate_glm(self, requests):
         m = self.engine.model
-        # multinomial models: intercept (G, C) and beta (P, C) per chain, flattened row-major
-        C = m.n_classes if m.multinomial else 1
-        G, K = m.n_groups * C, m.n_chains
-        beta_shape = (m.n_features, C) if m.multinomial else (m.n_features,)
+        K = m.n_chains
         chains: Dict[bytes, int] = {}      # distinct parameter vector -> chain
         rows: List[np.ndarray] = []
         chain_of: Dict[int, int] = {}
-        shapes: Dict[int, tuple] = {}
-        disp_shapes: Dict[int, tuple] = {}
-        n_third = 1 if m.dispersion else (m.n_classes - 1 if m.ordinal else 0)   # log_dispersion / cutpoints
+        shapes: Dict[int, list] = {}
         for node, inputs in requests.items():
-            # families with a dispersion parameter: (intercept, beta, log_dispersion), the last one part of the key;
-            # ordinal: (intercept, beta, cutpoints), likewise
-            intercept, beta = inputs[0], inputs[1]
-            ic = np.asarray(intercept, dtype=np.float32)
-            parts = [ic.reshape(G), np.asarray(beta, dtype=np.float32).reshape(m.n_features * C)]
-            if n_third:
-                ld = np.asarray(inputs[2], dtype=np.float32)
-                parts.append(ld.reshape(n_third))
-                disp_shapes[node] = ld.shape
-            vec = np.concatenate(parts)
+            # every input is part of the key: the flat parameter vector of the model's layout
+            arrs = [np.asarray(x, dtype=np.float32) for x in inputs]
+            vec = np.concatenate([a.reshape(int(np.prod(s))) for a, s in zip(arrs, m.input_shapes)])
             key = vec.tobytes()
             if key not in chains:
                 if len(rows) == K:
@@ -126,33 +114,16 @@ class NodeFederation:
                 chains[key] = len(rows)
                 rows.append(vec)
             chain_of[node] = chains[key]
-            shapes[node] = ic.shape
+            shapes[node] = [a.shape for a in arrs]
         theta = np.stack(rows + [rows[0]] * (K - len(rows)))                       # unused chains repeat the first
-        if m.multinomial:
-            ic_shape = (m.n_groups, C)
-            inputs = ([theta[:, :G].reshape((K,) + ic_shape), theta[:, G:].reshape((K,) + beta_shape)] if K > 1
-                      else [theta[0, :G].reshape(ic_shape), theta[0, G:].reshape(beta_shape)])
-        elif m.dispersion:
-            P = m.n_features
-            inputs = ([theta[:, :G], theta[:, G : G + P], theta[:, G + P]] if K > 1
-                      else [theta[0, :G], theta[0, G : G + P], theta[0, G + P]])
-        elif m.ordinal:
-            P = m.n_features
-            inputs = ([theta[:, :G], theta[:, G : G + P], theta[:, G + P :]] if K > 1
-                      else [theta[0, :G], theta[0, G : G + P], theta[0, G + P :]])
-        else:
-            inputs = [theta[:, :G], theta[:, G:]] if K > 1 else [theta[0, :G], theta[0, G:]]
-        # [n_nodes, K, 1 + G + P (+ 1, or + C - 1 cutpoints)]; the ordinal family's call context marks unordered chains
-        per = m.per_node(self.engine.evaluate_raw(inputs), m.call_context(inputs) if m.ordinal else None)
+        inputs = m.inputs_from_theta(theta if K > 1 else theta[0])
+        per = m.per_node(self.engine.evaluate_raw(inputs), m.call_context(inputs))   # [n_nodes, K, 1 + n_params]
         out = {}
         for node in requests:
             v = per[node, chain_of[node]]
-            if n_third:
-                P = m.n_features
-                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G : 1 + G + P].copy(),
-                                              v[1 + G + P :].reshape(disp_shapes[node]).copy()])
-            else:
-                out[node] = (np.array(v[0]), [v[1 : 1 + G].reshape(shapes[node]).copy(), v[1 + G :].reshape(beta_shape).copy()])
+            # d_beta in the model's shape, the other gradients in the shapes this node passed
+            ic_shape, _, *rest = shapes[node]
+            out[node] = (np.array(v[0]), m.gradients_from_row(v, [ic_shape, None, *rest]))
         return out
 
     def evaluate_node(self, node: int, *inputs) -> Tuple[np.ndarray, List[np.ndarray]]:
@@ -200,17 +171,15 @@ class NodeFederation:
                     th = np.broadcast_to(np.asarray(theta, dtype=np.float64), (self.n_nodes, m.n_params))
                     per = m.per_node(eng.evaluate_raw([th]))
                     return np.asarray(per[:, 0].sum()), [per[:, 1:].copy()]
-        elif getattr(eng.model, "dispersion", False) or getattr(eng.model, "ordinal", False):
-            def func(intercept, beta, third):   # log_dispersion or cutpoints
-                with self._lock:
-                    self.n_launches += 1
-                    logp, *grads = eng.evaluate(intercept, beta, third)
-                    return logp, grads
         else:
-            def func(intercept, beta):
+            n_inputs = eng.model.n_inputs
+
+            def func(*inputs):
+                if len(inputs) != n_inputs:
+                    raise TypeError(f"the model takes {n_inputs} inputs, got {len(inputs)}")
                 with self._lock:
                     self.n_launches += 1
-                    logp, *grads = eng.evaluate(intercept, beta)
+                    logp, *grads = eng.evaluate(*inputs)
                     return logp, grads
         return func
 

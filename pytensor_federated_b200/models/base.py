@@ -5,6 +5,8 @@ reference node serves (``pytensor_federated/service.py:78-86``): it owns the
 node's private data (resident in HBM) and knows
 
 * how the client's input arrays are packed into the theta mailbox (32-bit words),
+* how those words are turned back into input arrays (``inputs_from_words(words)``, what the peers of the
+  collective backend evaluate; every model but ``LinregShards`` has it),
 * how the reduced ``[LL, dLL/dtheta ...]`` vector of doubles is unpacked into the flat
   ``(logp, *gradients)`` tuple of the ``wrap_logp_grad_func`` convention
   (``pytensor_federated/common.py:26-49``),

@@ -6,6 +6,10 @@ bf16 design matrix* and *hierarchical GLM, 8 partial-pooling groups, fp8 block-s
 matrix*.  ``theta = [intercept[G], beta[P]]`` (float32) per chain; a segment (shard) uses
 ``intercept[group]``, so G = 1 is the pooled GLM and G = #shards the partial-pooling one.
 Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
+
+How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
+oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
+``_Ordinal`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -18,8 +22,6 @@ from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
             "ordinal": 6}
-#: families with a learned dispersion parameter (one more input, ``log_dispersion``)
-DISPERSION_FAMILIES = ("gaussian_scale", "negative_binomial")
 
 
 def _family_code(family) -> int:
@@ -30,6 +32,17 @@ def _aligned16(t):
     """``t``, or a copy of it when its storage does not start on a 16-byte boundary (a view such as ``y[1:]``): the
     tensor-core kernel streams per-row arrays with TMA, which reads from 16-byte aligned addresses only."""
     return t.clone() if t.data_ptr() % 16 != 0 else t
+
+
+def _split(rows: np.ndarray, shapes) -> List[np.ndarray]:
+    """``rows[..., n]`` cut into consecutive pieces, piece i reshaped to ``rows.shape[:-1] + shapes[i]`` (views where
+    the reshape allows; never a cast)."""
+    lead, out, a = rows.shape[:-1], [], 0
+    for s in shapes:
+        n = int(np.prod(s))
+        out.append(rows[..., a : a + n].reshape(lead + tuple(s)))
+        a += n
+    return out
 
 
 class GlmShards(ShardModel):
@@ -174,109 +187,24 @@ class GlmShards(ShardModel):
             if X.dim() != 2 or X.shape[1] != self.n_features or X.stride(1) != 1 or X.stride(0) != self.ld:
                 raise ValueError("all design matrices must be row-major [n, P] with one row stride")
         self.device = X0.device
-        self.n_inputs = 2
-        self.n_params = self.n_groups + self.n_features
-        self.n_theta_words = self.n_chains * self.n_params
         if (node_ids is None) != (n_nodes is None):
             raise ValueError("node_ids and n_nodes come together")
         self.node_ids = list(node_ids) if node_ids is not None else None
         self.n_nodes = int(n_nodes) if n_nodes is not None else 1
         if self.node_ids is not None and (len(self.node_ids) != len(self.Xs) or not all(0 <= i < self.n_nodes for i in self.node_ids)):
             raise ValueError("node_ids needs one node index in [0, n_nodes) per segment")
-        self.n_vals = self.n_nodes * self.n_chains * (1 + self.n_params)
-        #: classes per chain (multinomial family; 1 for every other family)
-        self.n_classes = 1
-        self.multinomial = isinstance(family, str) and family == "multinomial"
-        #: the family has a log-dispersion parameter after beta (``gaussian_scale``, ``negative_binomial``)
-        self.dispersion = isinstance(family, str) and family in DISPERSION_FAMILIES
-        #: cumulative-logit family: one more input, ``cutpoints[C - 1]``
-        self.ordinal = isinstance(family, str) and family == "ordinal"
+        layout = _LAYOUTS.get(family, _Scalar) if isinstance(family, str) else _Scalar
+        self._layout = lay = layout(self, n_classes)
+        #: classes per chain (multinomial and ordinal families; 1 for every other family)
+        self.n_classes = lay.n_classes
+        #: per-chain shapes of the inputs, in order: ``(intercept, beta)`` or ``(intercept, beta, third)``
+        self.input_shapes = lay.shapes
+        self.n_inputs = len(lay.shapes)
+        self.n_params = sum(int(np.prod(s)) for s in lay.shapes)
         #: columns of one launch: K, times C for the multinomial family, times C - 1 for the ordinal one
-        self.kernel_chains = self.n_chains
-        if self.multinomial:
-            self._init_multinomial(n_classes)
-        elif self.ordinal:
-            self._init_ordinal(n_classes)
-        elif n_classes is not None:
-            raise ValueError("n_classes is for family='multinomial' or 'ordinal' only")
-        if self.dispersion:
-            self._init_dispersion()
-
-    def _init_multinomial(self, n_classes) -> None:
-        """Checks of the multinomial family, then its sizes: C (G + P) parameters per chain, and the kernel's
-        output of K C virtual chains (one ``[LL, gi[G], g[P]]`` block per chain and class)."""
-        import torch
-
-        if self.kernel not in ("auto", "tc"):
-            raise ValueError(f"kernel={self.kernel!r}: the multinomial family runs on the bf16 tensor-core kernel only "
-                             "(kernel='tc' or 'auto')")
-        if n_classes is None or not 2 <= int(n_classes) <= 16:
-            raise ValueError(f"the multinomial family needs n_classes in [2, 16], got {n_classes}")
-        C = int(n_classes)
-        if self.n_chains * C > 16:
-            raise ValueError(f"n_chains x n_classes must be <= 16 (the tensor-core kernel's columns per launch), got "
-                             f"{self.n_chains} x {C}")
-        if any(o is not None for o in self.offsets):
-            raise ValueError("offsets are not supported by the multinomial family: an offset common to all classes "
-                             "cancels in the softmax")
-        for si, (y, w) in enumerate(zip(self.ys, self.weights)):
-            bad = ~((y == torch.floor(y)) & (y >= 0) & (y < C))   # NaN fails every comparison
-            if w is not None:
-                bad &= w != 0   # a masked row may carry anything
-            if bool(torch.any(bad)):
-                raise ValueError(f"labels of segment {si} must be integers in [0, {C}) on every row of non-zero weight")
-        self.n_classes = C
-        self.kernel_chains = self.n_chains * C
-        self.n_params = C * (self.n_groups + self.n_features)
-        self.n_theta_words = self.n_chains * self.n_params
-        self.n_vals = self.n_nodes * self.n_chains * C * (1 + self.n_groups + self.n_features)
-
-    def _init_ordinal(self, n_classes) -> None:
-        """Checks of the ordinal family, then its sizes: G + P + C - 1 parameters per chain, and the kernel's output
-        of K (C - 1) virtual chains (one ``[LL, gi[G], g[P]]`` block per chain and cutpoint)."""
-        import torch
-
-        if self.kernel not in ("auto", "tc"):
-            raise ValueError(f"kernel={self.kernel!r}: the ordinal family runs on the bf16 tensor-core kernel only "
-                             "(kernel='tc' or 'auto')")
-        if n_classes is None or not 2 <= int(n_classes) <= 17:
-            raise ValueError(f"the ordinal family needs n_classes in [2, 17], got {n_classes}")
-        C = int(n_classes)
-        if self.n_chains * (C - 1) > 16:
-            raise ValueError(f"n_chains x (n_classes - 1) must be <= 16 (the tensor-core kernel's columns per launch), "
-                             f"got {self.n_chains} x {C - 1}")
-        for si, (y, w) in enumerate(zip(self.ys, self.weights)):
-            bad = ~((y == torch.floor(y)) & (y >= 0) & (y < C))   # NaN fails every comparison
-            if w is not None:
-                bad &= w != 0   # a masked row may carry anything
-            if bool(torch.any(bad)):
-                raise ValueError(f"labels of segment {si} must be integers in [0, {C}) on every row of non-zero weight")
-        self.n_classes = C
-        self.kernel_chains = self.n_chains * (C - 1)
-        self.n_inputs = 3
-        self.n_params = self.n_groups + self.n_features + C - 1
-        self.n_theta_words = self.kernel_chains * (self.n_groups + self.n_features)
-        self.n_vals = self.n_nodes * self.kernel_chains * (1 + self.n_groups + self.n_features)
-
-    def _init_dispersion(self) -> None:
-        """Checks of the families with a dispersion parameter, then their sizes: theta per chain is
-        ``[intercept[G], beta[P], log_dispersion]`` and the output block ``[LL, d intercept[G], d beta[P], d log_dispersion]``."""
-        import torch
-
-        if self.kernel not in ("auto", "tc"):
-            raise ValueError(f"kernel={self.kernel!r}: the {self.family} family runs on the bf16 tensor-core kernel only "
-                             "(kernel='tc' or 'auto')")
-        if self.family == "negative_binomial":
-            for si, (y, w) in enumerate(zip(self.ys, self.weights)):
-                bad = ~((y == torch.floor(y)) & (y >= 0) & (y <= 2.0 ** 24))   # NaN fails every comparison
-                if w is not None:
-                    bad &= w != 0   # a masked row may carry anything
-                if bool(torch.any(bad)):
-                    raise ValueError(f"counts of segment {si} must be integers in [0, 2^24] on every row of non-zero weight")
-        self.n_inputs = 3
-        self.n_params = self.n_groups + self.n_features + 1
-        self.n_theta_words = self.n_chains * self.n_params
-        self.n_vals = self.n_nodes * self.n_chains * (1 + self.n_params)
+        self.kernel_chains = self.n_chains * lay.columns
+        self.n_theta_words = self.kernel_chains * lay.words
+        self.n_vals = self.n_nodes * self.kernel_chains * (1 + lay.words)
 
     def _row_data(self, entries, name: str) -> list:
         """One contiguous float32 tensor (or None) per segment, on the device of the segment's X."""
@@ -312,185 +240,58 @@ class GlmShards(ShardModel):
         return int(sum(X.shape[0] for X in self.Xs))
 
     # -- packing ---------------------------------------------------------------------------
-    def call_context(self, inputs):
-        """``(batched, intercept shape)`` of one call: a 2-D ``beta`` means one row per chain (multinomial: a 3-D
-        ``beta[K, P, C]``); families with a dispersion parameter add the shape of ``log_dispersion``."""
-        if self.dispersion:
-            intercept, beta, log_disp = inputs
-            return (np.ndim(beta) == 2, np.shape(intercept), np.shape(log_disp))
-        if self.ordinal:
-            return self._ordinal_table(inputs)[1]
-        intercept, beta = inputs
-        return (np.ndim(beta) == (3 if self.multinomial else 2), np.shape(intercept))
+    #: call context of the most recent single-threaded ``pack_theta`` / ``reference_partial`` / ``eager_partial``
+    #: (before any: unbatched, scalar shapes, no unordered chains); the engine passes the context explicitly instead
+    _last_ctx = (False, (), (), ())
 
-    _pack_views = None
+    def call_context(self, inputs):
+        """``(batched, intercept shape)`` of one call: ``beta`` with one more axis than its per-chain shape means one
+        row per chain.  Three-input families add the shape of the third input; the ordinal family then adds the
+        chains whose cutpoints are not ordered."""
+        return self._layout.call_context(inputs)
 
     def pack_theta(self, inputs, out: np.ndarray):
-        if self.multinomial:
-            return self._pack_theta_multinomial(inputs, out)
-        if self.dispersion:
-            return self._pack_theta_dispersion(inputs, out)
-        if self.ordinal:
-            return self._pack_theta_ordinal(inputs, out)
-        intercept, beta = inputs
-        views = self._pack_views
-        if views is None or views[0] is not out:
-            # float32 windows into the staging buffer, built once per buffer (this runs on every evaluation)
-            th = out.view(np.float32).reshape(self.n_chains, self.n_params)
-            views = self._pack_views = (out, th[:, : self.n_groups], th[:, self.n_groups :])
-        ic = intercept if type(intercept) is np.ndarray else np.asarray(intercept)
-        bt = beta if type(beta) is np.ndarray else np.asarray(beta)
-        batched = bt.ndim == 2
-        ctx = (batched, ic.shape)
-        self._batched, self._icpt_shape = ctx
-        # the assignments convert to float32 while they copy
-        views[1][...] = ic.reshape(self.n_chains, -1) if batched else ic.reshape(1, -1)
-        views[2][...] = bt.reshape(self.n_chains, self.n_features)
+        ctx = self._last_ctx = self._layout.pack(inputs, out)
         return ctx
 
-    def _pack_theta_multinomial(self, inputs, out: np.ndarray):
-        """Theta words as ``[K C][G + P]``: row ``k C + c`` is ``(intercept[:, c], beta[:, c])`` of chain k, the
-        kernel's virtual chain of class c."""
-        intercept, beta = inputs
-        K, C, G, P = self.n_chains, self.n_classes, self.n_groups, self.n_features
-        views = self._pack_views
-        if views is None or views[0] is not out:
-            th = out.view(np.float32).reshape(K, C, G + P)
-            views = self._pack_views = (out, th[:, :, :G], th[:, :, G:])
-        ic, bt = np.asarray(intercept), np.asarray(beta)
-        ctx = (bt.ndim == 3, ic.shape)
-        self._batched, self._icpt_shape = ctx
-        views[1][...] = ic.reshape(K, G, C).transpose(0, 2, 1)
-        views[2][...] = bt.reshape(K, P, C).transpose(0, 2, 1)
-        return ctx
+    def inputs_from_words(self, words: np.ndarray):
+        """Theta words -> inputs of one call (the peers of the collective backend).  The ordinal family's words carry
+        only ``intercept - c_j``, so its inputs come back shifted to ``c_0 = 0`` (the likelihood does not see the
+        shift; they pack back to the same words)."""
+        return self._layout.inputs_from_words(words)
 
-    def _pack_theta_dispersion(self, inputs, out: np.ndarray):
-        """Theta words as ``[K][G + P + 1]``: ``(intercept, beta, log_dispersion)`` of each chain."""
-        intercept, beta, log_disp = inputs
-        K, G, P = self.n_chains, self.n_groups, self.n_features
-        th = out.view(np.float32).reshape(K, G + P + 1)
-        ic, bt, ld = np.asarray(intercept), np.asarray(beta), np.asarray(log_disp)
-        ctx = (bt.ndim == 2, ic.shape, ld.shape)
-        self._batched, self._icpt_shape = ctx[:2]
-        self._disp_shape = ctx[2]
-        th[:, :G] = ic.reshape(K, G)
-        th[:, G : G + P] = bt.reshape(K, P)
-        th[:, G + P] = ld.reshape(K)
-        return ctx
+    def inputs_from_theta(self, theta: np.ndarray) -> List[np.ndarray]:
+        """The inputs held in flat parameter rows ``theta[..., n_params]`` (each input flattened row-major, in
+        order): input i gets shape ``theta.shape[:-1] + input_shapes[i]``, so ``[K, n_params]`` gives a batched
+        call and ``[n_params]`` an unbatched one.  Views where possible; the dtype is kept."""
+        return _split(np.asarray(theta), self.input_shapes)
 
-    def _ordinal_table(self, inputs):
-        """``(T, ctx)``: the kernel's intercept table ``T[K, C - 1, G] = float32(intercept[g] - c_j)`` (the difference
-        taken in double, rounded once) and the call context ``(batched, intercept shape, cutpoints shape, bad)``, with
-        ``bad`` the chains whose table is not strictly decreasing in j for every group."""
-        intercept, beta, cutpoints = inputs
-        K, G, C1 = self.n_chains, self.n_groups, self.n_classes - 1
-        ic = np.asarray(intercept, dtype=np.float64).reshape(K, G)
-        cp = np.asarray(cutpoints, dtype=np.float64).reshape(K, C1)
-        T = (ic[:, None, :] - cp[:, :, None]).astype(np.float32)
-        ordered = np.all(T[:, 1:, :] < T[:, :-1, :], axis=(1, 2))   # NaN fails the comparison
-        bad = tuple(int(k) for k in np.flatnonzero(~ordered))
-        return T, (np.ndim(beta) == 2, np.shape(intercept), np.shape(cutpoints), bad)
-
-    def _pack_theta_ordinal(self, inputs, out: np.ndarray):
-        """Theta words as ``[K (C - 1)][G + P]``: row ``k (C - 1) + j`` is ``(intercept - c_j, beta)`` of chain k, the
-        kernel's virtual chain of cutpoint j."""
-        K, C1, G, P = self.n_chains, self.n_classes - 1, self.n_groups, self.n_features
-        T, ctx = self._ordinal_table(inputs)
-        th = out.view(np.float32).reshape(K, C1, G + P)
-        th[:, :, :G] = T
-        th[:, :, G:] = np.asarray(inputs[1]).reshape(K, 1, P)
-        self._batched, self._icpt_shape, self._cut_shape, self._ord_bad = ctx
-        return ctx
-
-    _batched = False
-    _icpt_shape = ()
-    _disp_shape = ()
-    _cut_shape = ()
-    _ord_bad = ()
-
-    def _note_shapes(self, inputs):
-        # single-threaded convenience state (tests call reference_partial then unpack_result);
-        # the engine passes the context explicitly instead
-        ctx = self.call_context(inputs)
-        self._batched, self._icpt_shape = ctx[:2]
-        if self.dispersion:
-            self._disp_shape = ctx[2]
-        if self.ordinal:
-            self._cut_shape, self._ord_bad = ctx[2], ctx[3]
-        return ctx
+    def gradients_from_row(self, row: np.ndarray, shapes) -> List[np.ndarray]:
+        """The gradients in result rows ``[..., 1 + n_params]`` (``[LL, gradients]`` as :meth:`per_node` gives
+        them), in the order of the inputs and as fresh arrays: gradient i gets ``shapes[i]``, or where that is None
+        the rows' leading axes and the input's per-chain shape."""
+        return [(g if s is None else g.reshape(s)).copy() for g, s in zip(_split(row[..., 1:], self.input_shapes), shapes)]
 
     def per_node(self, vals: np.ndarray, ctx=None) -> np.ndarray:
-        """The reduced vector as ``[n_nodes, n_chains, 1 + G + P]`` (``[LL, d intercepts, d beta]`` per block).
-        Multinomial: ``[n_nodes, n_chains, 1 + G C + P C]``, ``[LL, d intercept (G, C), d beta (P, C)]`` with the
-        matrices row-major, summed from the kernel's blocks of the chain's C classes.  Families with a dispersion
-        parameter: ``[n_nodes, n_chains, 2 + G + P]``, ``[LL, d intercepts, d beta, d log_dispersion]``.  Ordinal:
-        ``[n_nodes, n_chains, 1 + G + P + C - 1]``, ``[LL, d intercepts, d beta, d cutpoints]`` from the kernel's blocks
-        ``[LL_j, gi_j[G], g_j[P]]`` of the chain's C - 1 cutpoints (``d c_j = -sum_g gi_j[g]``); the chains that
-        ``ctx`` (the call context, by default that of the last ``pack_theta``) marks as unordered get ``LL = -inf``
-        and zero gradients."""
-        if self.ordinal:
-            n, K, C1, G = self.n_nodes, self.n_chains, self.n_classes - 1, self.n_groups
-            raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C1, 1 + G + self.n_features)
-            out = np.concatenate([raw[..., 0].sum(axis=2)[..., None], raw[..., 1:].sum(axis=2),
-                                  -raw[..., 1 : 1 + G].sum(axis=3)], axis=2)
-            bad = list(ctx[3] if ctx is not None else self._ord_bad)
-            out[:, bad, 0] = -np.inf
-            out[:, bad, 1:] = 0.0
-            return out
-        if self.multinomial:
-            n, K, C, G = self.n_nodes, self.n_chains, self.n_classes, self.n_groups
-            raw = np.asarray(vals, dtype=np.float64).reshape(n, K, C, 1 + G + self.n_features)
-            return np.concatenate([raw[..., 0].sum(axis=2)[..., None],
-                                   raw[..., 1 : 1 + G].transpose(0, 1, 3, 2).reshape(n, K, G * C),
-                                   raw[..., 1 + G :].transpose(0, 1, 3, 2).reshape(n, K, self.n_features * C)], axis=2)
-        return np.asarray(vals, dtype=np.float64).reshape(self.n_nodes, self.n_chains, 1 + self.n_params)
+        """The reduced vector as ``[n_nodes, n_chains, 1 + n_params]``: ``[LL, gradients]`` per node and chain, the
+        gradients flattened row-major in the order of the inputs (multinomial: ``[LL, d intercept (G, C), d beta
+        (P, C)]``, summed from the kernel's blocks of the chain's C classes; ordinal: ``[LL, d intercepts, d beta,
+        d cutpoints]`` from the kernel's blocks ``[LL_j, gi_j[G], g_j[P]]`` of the chain's C - 1 cutpoints, with
+        ``d c_j = -sum_g gi_j[g]``).  Ordinal chains that ``ctx`` (the call context, by default that of the last
+        ``pack_theta``) marks as unordered get ``LL = -inf`` and zero gradients."""
+        raw = np.asarray(vals, dtype=np.float64).reshape(self.n_nodes, self.kernel_chains, 1 + self._layout.words)
+        return self._layout.fold(raw, self._last_ctx if ctx is None else ctx)
 
     def unpack_result(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
-        if self.multinomial:
-            return self._unpack_multinomial(vals, ctx)
-        if self.dispersion:
-            return self._unpack_dispersion(vals, ctx)
-        if self.ordinal:
-            return self._unpack_ordinal(vals, ctx)
-        v = self.per_node(vals).sum(axis=0) if self.n_nodes > 1 else np.asarray(vals, dtype=np.float64).reshape(self.n_chains, 1 + self.n_params)
-        G = self.n_groups
-        batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
-        if batched:
-            return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
-                    v[:, 1 + G :].copy()]
-        return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G :].copy()]
-
-    def _unpack_dispersion(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
-        v = self.per_node(vals).sum(axis=0)                         # [K, 2 + G + P]
-        G, P = self.n_groups, self.n_features
-        batched, icpt_shape, disp_shape = ctx if ctx is not None else (self._batched, self._icpt_shape, self._disp_shape)
-        if batched:
-            return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
-                    v[:, 1 + G : 1 + G + P].copy(), v[:, 1 + G + P].reshape(disp_shape).copy()]
-        return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G : 1 + G + P].copy(),
-                v[0, 1 + G + P].reshape(disp_shape).copy()]
-
-    def _unpack_ordinal(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
-        ctx = ctx if ctx is not None else (self._batched, self._icpt_shape, self._cut_shape, self._ord_bad)
-        v = self.per_node(vals, ctx).sum(axis=0)                    # [K, 1 + G + P + C - 1]
-        G, P = self.n_groups, self.n_features
-        batched, icpt_shape, cut_shape, _ = ctx
-        if batched:
-            return [v[:, 0].copy(), v[:, 1 : 1 + G].reshape((self.n_chains,) + tuple(icpt_shape[1:])).copy(),
-                    v[:, 1 + G : 1 + G + P].copy(), v[:, 1 + G + P :].reshape(cut_shape).copy()]
-        return [np.asarray(v[0, 0]), v[0, 1 : 1 + G].reshape(icpt_shape).copy(), v[0, 1 + G : 1 + G + P].copy(),
-                v[0, 1 + G + P :].reshape(cut_shape).copy()]
-
-    def _unpack_multinomial(self, vals: np.ndarray, ctx=None) -> List[np.ndarray]:
-        v = self.per_node(vals).sum(axis=0)                         # [K, 1 + G C + P C]
-        K, GC, PC = self.n_chains, self.n_groups * self.n_classes, self.n_features * self.n_classes
-        batched, icpt_shape = ctx if ctx is not None else (self._batched, self._icpt_shape)
-        beta_shape = (self.n_features, self.n_classes)
-        if batched:
-            return [v[:, 0].copy(), v[:, 1 : 1 + GC].reshape((K,) + tuple(icpt_shape[1:])).copy(),
-                    v[:, 1 + GC : 1 + GC + PC].reshape((K,) + beta_shape).copy()]
-        return [np.asarray(v[0, 0]), v[0, 1 : 1 + GC].reshape(icpt_shape).copy(),
-                v[0, 1 + GC : 1 + GC + PC].reshape(beta_shape).copy()]
+        ctx = self._last_ctx if ctx is None else ctx
+        batched, icpt_shape = ctx[0], ctx[1]
+        v = self.per_node(vals, ctx).sum(axis=0)                    # [K, 1 + n_params]
+        if not batched:
+            v = v[0]
+        # the intercept's gradient in the shape it was passed (chains leading when batched), beta's in the model's
+        # shape, a third input's in its shape
+        shapes = [(self.n_chains,) + tuple(icpt_shape[1:]) if batched else icpt_shape, None, *ctx[2 : self.n_inputs]]
+        return [np.array(v[..., 0]), *self.gradients_from_row(v, shapes)]
 
     # -- native ----------------------------------------------------------------------------
     def use_tensor_cores(self):
@@ -503,9 +304,11 @@ class GlmShards(ShardModel):
             if X0.dtype not in (torch.bfloat16, torch.float32) or self.n_chains != 1 or self.n_features > 1024:
                 raise ValueError("custom likelihoods need a bf16/fp32 design matrix, one chain and P <= 1024")
             return 3 if X0.dtype == torch.bfloat16 else 4
-        if self.multinomial or self.dispersion or self.ordinal:   # the bf16 tensor-core kernel or nothing: no other kernel has these
-            if not (X0.dtype == torch.bfloat16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384
-                    and self.n_chains <= 16 and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0):
+        bf16 = X0.dtype == torch.bfloat16
+        tc_ok = (bf16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384 and self.n_chains <= 16
+                 and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0)
+        if self._layout.tc_only:   # the bf16 tensor-core kernel or nothing: no other kernel has these families
+            if not tc_ok:
                 raise ValueError(f"the {self.family} family runs on the bf16 tensor-core kernel only, which needs a bf16 "
                                  f"design matrix with P % 8 == 0, 8 <= P <= 384 and 16-byte aligned rows (got "
                                  f"{X0.dtype}, P = {self.n_features}, row stride {self.ld}) and at most 16 chains")
@@ -523,9 +326,6 @@ class GlmShards(ShardModel):
             return generic
         # auto: the tensor-core kernel wherever its shape constraints hold (it is faster even for one chain:
         # TMA streaming + the X tile reused from smem for both GEMMs), then SIMT, then the general kernel
-        bf16 = X0.dtype == torch.bfloat16
-        tc_ok = (bf16 and self.n_features % 8 == 0 and 8 <= self.n_features <= 384 and self.n_chains <= 16
-                 and all(X.data_ptr() % 16 == 0 for X in self.Xs) and self.ld % 8 == 0)
         if tc_ok:
             return 1
         if self.n_chains > 1:
@@ -578,209 +378,12 @@ class GlmShards(ShardModel):
     # -- eager oracle (also the compute step of the NCCL baseline) ---------------------------
     def reference_partial(self, inputs, *, dtype=None, chunk_rows: int = 1 << 20) -> np.ndarray:
         """This node's partial with stock PyTorch ops (oracle of the kernels, compute step of the CPU / gloo
-        path).  Rows are processed ``chunk_rows`` at a time (a multiple of 128), so an fp64 oracle of a
-        10M-row shard needs 2 GB of scratch, not 20."""
+        path), in the kernel's layout (:meth:`per_node` folds it).  Rows are processed ``chunk_rows`` at a time (a
+        multiple of 128), so an fp64 oracle of a 10M-row shard needs 2 GB of scratch, not 20."""
         import torch
 
-        dtype = dtype or torch.float32
-        if self.multinomial:
-            return self._multinomial_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
-        if self.dispersion:
-            return self._dispersion_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
-        if self.ordinal:
-            return self._ordinal_partial(inputs, dtype=dtype, chunk_rows=chunk_rows)
-        intercept, beta = inputs
-        self._note_shapes(inputs)
-        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(self.n_chains, -1)
-        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(self.n_chains, self.n_features)
-        full = torch.zeros(self.n_nodes, self.n_chains, 1 + self.n_params, dtype=torch.float64, device=self.device)
-        B = bt.to(self.device, dtype)                              # [K, P]
-        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
-            out = full[self.node_ids[si] if self.node_ids is not None else 0]
-            icg = ic[:, g].to(self.device, dtype)
-            for r0 in range(0, X.shape[0], chunk_rows):
-                r1 = min(X.shape[0], r0 + chunk_rows)
-                Xf = self._dequant_rows(si, r0, r1).to(dtype)
-                eta = Xf @ B.T + icg                                # [n, K]
-                if self.offsets[si] is not None:
-                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
-                yy = y[r0:r1].to(dtype).unsqueeze(1)
-                if hasattr(self.family, "code_id"):
-                    if self.family.torch_fn is None:
-                        raise ValueError("this CustomFamily has no torch_fn oracle")
-                    ll, r = self.family.torch_fn(yy, eta)
-                elif self.family == "logistic":
-                    ll = yy * eta - torch.nn.functional.softplus(eta)
-                    r = yy - torch.sigmoid(eta)
-                elif self.family == "poisson":
-                    mu = torch.exp(eta)
-                    ll = yy * eta - mu
-                    r = yy - mu
-                else:
-                    d = yy - eta
-                    ll = -0.5 * d * d - 0.918938533204672742
-                    r = d
-                ll, r = self._weigh(si, r0, r1, ll, r)
-                out[:, 0] += ll.double().sum(0)
-                out[:, 1 + g] += r.double().sum(0)
-                out[:, 1 + self.n_groups :] += (r.T @ Xf).double()
-        return full.reshape(-1).cpu().numpy()
-
-    def _weigh(self, seg: int, r0: int, r1: int, ll, r):
-        """``(w ll, w r)`` of rows ``[r0, r1)`` of segment ``seg``; rows of weight 0 give exactly 0 (a select, not
-        a product: their ``ll`` may be NaN)."""
-        import torch
-
-        w = self.weights[seg]
-        if w is None:
-            return ll, r
-        ww = w[r0:r1].to(ll.dtype).reshape((-1,) + (1,) * (ll.dim() - 1))   # broadcast over chains (and classes)
-        keep = ww != 0
-        return torch.where(keep, ww * ll, torch.zeros_like(ll)), torch.where(keep, ww * r, torch.zeros_like(r))
-
-    def _multinomial_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
-        """The multinomial family's partial in the kernel's layout ``[n_nodes][K C][1 + G + P]`` (block ``k C + c``:
-        ``[LL_kc, gi_kc[G], g_kc[P]]`` with ``LL_kc = sum_i w_i [y_i == c] log_softmax(eta_i)_c``,
-        ``r_ikc = [y_i == c] - softmax(eta_i)_c``).  ``bf16_gemms``: the collective baseline, two bf16 GEMMs
-        with ``beta`` as ``[P, K C]`` and fp32 elementwise work; else the oracle in ``dtype``."""
-        import torch
-
-        intercept, beta = inputs
-        self._note_shapes(inputs)
-        K, C, G, P = self.n_chains, self.n_classes, self.n_groups, self.n_features
-        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G, C).to(self.device, dtype)
-        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P, C)
-        B = bt.permute(1, 0, 2).reshape(P, K * C).to(self.device, torch.bfloat16 if bf16_gemms else dtype)   # column k C + c
-        full = torch.zeros(self.n_nodes, K * C, 1 + G + P, dtype=torch.float64, device=self.device)
-        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
-            out = full[self.node_ids[si] if self.node_ids is not None else 0]
-            w = self.weights[si]
-            for r0 in range(0, X.shape[0], chunk_rows):
-                r1 = min(X.shape[0], r0 + chunk_rows)
-                if bf16_gemms:
-                    Xf = X[r0:r1]
-                    eta = (Xf @ B).to(dtype)
-                else:
-                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
-                    eta = Xf @ B
-                n = r1 - r0
-                eta = eta.reshape(n, K, C) + ic[:, g, :]
-                lab = y[r0:r1]
-                if w is not None:   # masked rows may carry NaN or out-of-range labels: any valid class will do
-                    lab = torch.where(w[r0:r1] != 0, lab, torch.zeros_like(lab))
-                hit = torch.nn.functional.one_hot(lab.long(), C).bool().unsqueeze(1)   # [n, 1, C]
-                logp = torch.log_softmax(eta, dim=-1)
-                ll = torch.where(hit, logp, torch.zeros_like(logp))
-                r = hit.to(dtype) - torch.exp(logp)
-                ll, r = self._weigh(si, r0, r1, ll, r)
-                out[:, 0] += ll.double().sum(0).reshape(K * C)
-                out[:, 1 + g] += r.double().sum(0).reshape(K * C)
-                rT = r.reshape(n, K * C).T
-                out[:, 1 + G :] += (rT.to(torch.bfloat16) @ Xf if bf16_gemms else rT @ Xf).double()
-        return full.reshape(-1).cpu().numpy()
-
-    def _dispersion_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
-        """The partial of the families with a dispersion parameter, ``[n_nodes][K][LL, gi[G], g[P], q]`` with
-        ``q = dll/dlog_dispersion``.  ``bf16_gemms``: the collective baseline, two bf16 GEMMs and fp32 elementwise
-        work; else the oracle in ``dtype``."""
-        import torch
-
-        intercept, beta, log_disp = inputs
-        self._note_shapes(inputs)
-        K, G, P = self.n_chains, self.n_groups, self.n_features
-        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G).to(self.device, dtype)
-        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P)
-        ld = torch.as_tensor(np.asarray(log_disp, dtype=np.float64)).reshape(K).to(self.device, dtype)
-        B = bt.T.to(self.device, torch.bfloat16 if bf16_gemms else dtype)       # [P, K]
-        full = torch.zeros(self.n_nodes, K, 2 + G + P, dtype=torch.float64, device=self.device)
-        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
-            out = full[self.node_ids[si] if self.node_ids is not None else 0]
-            for r0 in range(0, X.shape[0], chunk_rows):
-                r1 = min(X.shape[0], r0 + chunk_rows)
-                if bf16_gemms:
-                    Xf = X[r0:r1]
-                    eta = (Xf @ B).to(dtype)
-                else:
-                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
-                    eta = Xf @ B
-                eta = eta + ic[:, g]
-                if self.offsets[si] is not None:
-                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
-                yy = y[r0:r1].to(dtype).unsqueeze(1)
-                if self.family == "gaussian_scale":
-                    ll, r, q = _gaussian_scale_terms(yy, eta, ld)
-                else:
-                    ll, r, q = _negative_binomial_terms(yy, eta, ld)
-                ll, r = self._weigh(si, r0, r1, ll, r)
-                _, q = self._weigh(si, r0, r1, ll, q)
-                out[:, 0] += ll.double().sum(0)
-                out[:, 1 + g] += r.double().sum(0)
-                out[:, 1 + G : 1 + G + P] += (r.T.to(torch.bfloat16) @ Xf if bf16_gemms else r.T @ Xf).double()
-                out[:, 1 + G + P] += q.double().sum(0)
-        return full.reshape(-1).cpu().numpy()
-
-    def _ordinal_partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
-        """The ordinal family's partial in the kernel's layout ``[n_nodes][K (C - 1)][1 + G + P]``: block
-        ``k (C - 1) + j`` is ``[LL_kj, gi_kj[G], g_kj[P]]`` with ``r_ikj = dll_i / dz_j`` at ``z_j = eta - c_j`` (non-zero
-        only for ``j = y_i`` and ``j = y_i - 1``) and each row's ``w ll`` credited to ``j = min(y_i, C - 2)``, as the
-        kernel does.  ``bf16_gemms``: the collective baseline, eta from one bf16 GEMM with ``beta`` as ``[P, K]``, then
-        ``X' (sum_j r_j)`` per chain in the block of cutpoint 0 (the host sums the cutpoints' blocks), fp32 elementwise
-        work; else the oracle in ``dtype``, which keeps every column's gradient block."""
-        import torch
-
-        intercept, beta, cutpoints = inputs
-        self._note_shapes(inputs)
-        K, C1, G, P = self.n_chains, self.n_classes - 1, self.n_groups, self.n_features
-        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float64)).reshape(K, G).to(self.device, dtype)
-        bt = torch.as_tensor(np.asarray(beta, dtype=np.float64)).reshape(K, P)
-        cp = torch.as_tensor(np.asarray(cutpoints, dtype=np.float64)).reshape(K, C1).to(self.device, dtype)
-        inf = torch.full((K, 1), float("inf"), dtype=dtype, device=self.device)
-        cpad = torch.cat([-inf, cp, inf], dim=1)                     # [K, C + 1]: c_{-1} = -inf, ..., c_{C-1} = +inf
-        B = bt.T.to(self.device, torch.bfloat16 if bf16_gemms else dtype)   # [P, K]
-        full = torch.zeros(self.n_nodes, K, C1, 1 + G + P, dtype=torch.float64, device=self.device)
-        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
-            out = full[self.node_ids[si] if self.node_ids is not None else 0]
-            w = self.weights[si]
-            for r0 in range(0, X.shape[0], chunk_rows):
-                r1 = min(X.shape[0], r0 + chunk_rows)
-                if bf16_gemms:
-                    Xf = X[r0:r1]
-                    eta = (Xf @ B).to(dtype)
-                else:
-                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
-                    eta = Xf @ B
-                eta = eta + ic[:, g]                                  # [n, K]
-                if self.offsets[si] is not None:
-                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
-                lab = y[r0:r1]
-                if w is not None:   # masked rows may carry NaN or out-of-range labels: any valid category will do
-                    lab = torch.where(w[r0:r1] != 0, lab, torch.zeros_like(lab))
-                lab = lab.long()
-                a = cpad[:, lab + 1].T - eta                          # c_y - eta = -z_up
-                b = cpad[:, lab].T - eta                              # c_{y-1} - eta = -z_lo
-                t = 1.0 / torch.expm1(a - b)                          # 1 / expm1(gap), 0 at the infinite ends
-                ll = torch.nn.functional.logsigmoid(a) + torch.nn.functional.logsigmoid(-b) + torch.log(-torch.expm1(b - a))
-                r_up = -torch.sigmoid(-a) - t
-                r_lo = torch.sigmoid(b) + t
-                hot = lambda j: torch.nn.functional.one_hot(j.clamp(0, C1 - 1), C1).to(dtype).unsqueeze(1)   # [n, 1, C1]
-                up, lo = (lab <= C1 - 1).to(dtype), (lab >= 1).to(dtype)
-                ll = ll.unsqueeze(2) * hot(torch.clamp(lab, max=C1 - 1))
-                r = (r_up * up.unsqueeze(1)).unsqueeze(2) * hot(lab) + (r_lo * lo.unsqueeze(1)).unsqueeze(2) * hot(lab - 1)
-                ll, r = self._weigh(si, r0, r1, ll, r)                # [n, K, C1]
-                out[:, :, 0] += ll.double().sum(0)
-                out[:, :, 1 + g] += r.double().sum(0)
-                if bf16_gemms:
-                    out[:, 0, 1 + G :] += (r.sum(2).T.to(torch.bfloat16) @ Xf).double()
-                else:
-                    out[:, :, 1 + G :] += (r.reshape(-1, K * C1).T @ Xf).double().reshape(K, C1, P)
-        return full.reshape(-1).cpu().numpy()
-
-    def _dequant_rows(self, seg: int, r0: int, r1: int):
-        """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
-        return self.Xs[seg][r0:r1]
-
-    def _dequant(self, X):
-        return X
+        self._last_ctx = self.call_context(inputs)
+        return self._partial(inputs, dtype=dtype or torch.float32, chunk_rows=chunk_rows)
 
     def eager_partial(self, inputs) -> np.ndarray:
         """Stock-PyTorch evaluation as a practitioner would write it: two bf16 GEMMs (X @ beta, then
@@ -790,38 +393,70 @@ class GlmShards(ShardModel):
 
         if self.Xs[0].dtype != torch.bfloat16:
             return self.reference_partial(inputs)
-        if self.multinomial:
-            return self._multinomial_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
-        if self.dispersion:
-            return self._dispersion_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
-        if self.ordinal:
-            return self._ordinal_partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
-        intercept, beta = inputs
-        self._note_shapes(inputs)
-        ic = torch.as_tensor(np.asarray(intercept, dtype=np.float32)).reshape(self.n_chains, -1).to(self.device)
-        bt = torch.as_tensor(np.asarray(beta, dtype=np.float32)).reshape(self.n_chains, self.n_features).to(self.device)
-        out = torch.zeros(self.n_chains, 1 + self.n_params, dtype=torch.float64, device=self.device)
+        self._last_ctx = self.call_context(inputs)
+        return self._layout.baseline(self, inputs)
+
+    def _partial(self, inputs, *, dtype, chunk_rows: int, bf16_gemms: bool = False) -> np.ndarray:
+        """The partial in the kernel's layout ``[n_nodes][kernel_chains][1 + G + P (+ 1)]``, from the family's
+        per-row terms (``_Layout.oracle``) in ``dtype``.  ``bf16_gemms``: the collective baseline, eta and the beta
+        gradient from bf16 GEMMs of the stored matrix (one per column of eta: the ordinal family puts
+        ``X' (sum_j r_j)`` in the block of cutpoint 0 and the host sums the blocks); else the oracle, from the
+        dequantised rows."""
+        import torch
+
+        lay = self._layout
+        icpt, beta, terms = lay.oracle(inputs, self.device, dtype)   # [G, E], [P, E]: E columns of eta
+        icpt = icpt.to(self.device, dtype)
+        B = beta.to(self.device, torch.bfloat16 if bf16_gemms else dtype)
+        G, P = self.n_groups, self.n_features
+        step = self.kernel_chains // B.shape[1]   # kernel columns per column of eta
+        full = torch.zeros(self.n_nodes, self.kernel_chains, 1 + lay.words, dtype=torch.float64, device=self.device)
         for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
-            eta = (X @ bt.T.to(torch.bfloat16)).float() + ic[:, g]          # [n, K]
-            if self.offsets[si] is not None:
-                eta = eta + self.offsets[si].unsqueeze(1)
-            yy = y.unsqueeze(1)
-            if self.family == "logistic":
-                ll = yy * eta - torch.nn.functional.softplus(eta)
-                r = yy - torch.sigmoid(eta)
-            elif self.family == "poisson":
-                mu = torch.exp(eta)
-                ll = yy * eta - mu
-                r = yy - mu
-            else:
-                d = yy - eta
-                ll = -0.5 * d * d - 0.918938533204672742
-                r = d
-            ll, r = self._weigh(si, 0, X.shape[0], ll, r)
-            out[:, 0] += ll.sum(0).double()
-            out[:, 1 + g] += r.sum(0).double()
-            out[:, 1 + self.n_groups :] += (r.T.to(torch.bfloat16) @ X).double()
-        return out.reshape(-1).cpu().numpy()
+            out = full[self.node_ids[si] if self.node_ids is not None else 0]
+            w = self.weights[si]
+            for r0 in range(0, X.shape[0], chunk_rows):
+                r1 = min(X.shape[0], r0 + chunk_rows)
+                if bf16_gemms:
+                    Xf = X[r0:r1]
+                    eta = (Xf @ B).to(dtype)
+                else:
+                    Xf = self._dequant_rows(si, r0, r1).to(dtype)
+                    eta = Xf @ B
+                eta = eta + icpt[g]
+                if self.offsets[si] is not None:
+                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
+                # ll, r (and the dispersion families' q = dll/dlog_dispersion), [n, K] or [n, K, columns]
+                ll, r, *q = self._weigh(si, r0, r1, *terms(y[r0:r1], None if w is None else w[r0:r1], eta))
+                out[:, 0] += ll.double().sum(0).reshape(-1)
+                out[:, 1 + g] += r.double().sum(0).reshape(-1)
+                if not bf16_gemms:
+                    out[:, 1 + G : 1 + G + P] += (r.reshape(r1 - r0, -1).T @ Xf).double()
+                elif step == 1:
+                    out[:, 1 + G : 1 + G + P] += (r.reshape(r1 - r0, -1).T.to(torch.bfloat16) @ Xf).double()
+                else:
+                    out[::step, 1 + G : 1 + G + P] += (r.sum(2).T.to(torch.bfloat16) @ Xf).double()
+                for t in q:
+                    out[:, 1 + G + P] += t.double().sum(0)
+        return full.reshape(-1).cpu().numpy()
+
+    def _weigh(self, seg: int, r0: int, r1: int, *terms):
+        """``w t`` for each per-row term ``t`` of rows ``[r0, r1)`` of segment ``seg``; rows of weight 0 give exactly 0
+        (a select, not a product: their terms may be NaN)."""
+        import torch
+
+        w = self.weights[seg]
+        if w is None:
+            return terms
+        ww = w[r0:r1].to(terms[0].dtype).reshape((-1,) + (1,) * (terms[0].dim() - 1))   # broadcast over chains
+        keep = ww != 0
+        return [torch.where(keep, ww * t, torch.zeros_like(t)) for t in terms]
+
+    def _dequant_rows(self, seg: int, r0: int, r1: int):
+        """Rows ``[r0, r1)`` of segment ``seg`` as stored values (dense kernels: the matrix itself)."""
+        return self.Xs[seg][r0:r1]
+
+    def _dequant(self, X):
+        return X
 
     def _row_data_bytes(self) -> int:
         """Bytes of offsets and weights read per evaluation (4 per row per vector present)."""
@@ -832,6 +467,324 @@ class GlmShards(ShardModel):
 
     def flops_per_eval(self) -> int:
         return int(4 * self.n_rows * self.n_features * self.kernel_chains)
+
+
+# -- family layouts ------------------------------------------------------------------------------
+def _f64(x):
+    import torch
+
+    return torch.as_tensor(np.asarray(x, dtype=np.float64))
+
+
+def _tc_kernel_only(m) -> None:
+    if m.kernel not in ("auto", "tc"):
+        raise ValueError(f"kernel={m.kernel!r}: the {m.family} family runs on the bf16 tensor-core kernel only "
+                         "(kernel='tc' or 'auto')")
+
+
+def _check_classes(m, n_classes, most: int, per_chain: int, columns_text: str) -> int:
+    """``n_classes`` as an int once it is in ``[2, most]`` and ``per_chain`` kernel columns of it fit K times."""
+    if n_classes is None or not 2 <= int(n_classes) <= most:
+        raise ValueError(f"the {m.family} family needs n_classes in [2, {most}], got {n_classes}")
+    cols = per_chain(int(n_classes))
+    if m.n_chains * cols > 16:
+        raise ValueError(f"n_chains x {columns_text} must be <= 16 (the tensor-core kernel's columns per launch), got "
+                         f"{m.n_chains} x {cols}")
+    return int(n_classes)
+
+
+def _check_integers(m, what: str, valid: str, below) -> None:
+    """Every row of non-zero weight holds an integer ``y >= 0`` with ``below(y)`` (``valid`` says so in words)."""
+    import torch
+
+    for si, (y, w) in enumerate(zip(m.ys, m.weights)):
+        bad = ~((y == torch.floor(y)) & (y >= 0) & below(y))   # NaN fails every comparison
+        if w is not None:
+            bad &= w != 0   # a masked row may carry anything
+        if bool(torch.any(bad)):
+            raise ValueError(f"{what} of segment {si} must be integers in {valid} on every row of non-zero weight")
+
+
+def _labels(y, w):
+    """Integer labels of a chunk; masked rows may carry NaN or out-of-range labels: any valid class will do."""
+    import torch
+
+    if w is not None:
+        y = torch.where(w != 0, y, torch.zeros_like(y))
+    return y.long()
+
+
+class _Layout:
+    """How one family's inputs map to the kernel.  A layout owns the per-chain input shapes, ``columns`` (kernel
+    columns per chain) and ``words`` (theta words per column), and converts inputs -> theta words (:meth:`pack`),
+    words -> inputs, the kernel's output blocks ``[n_nodes, kernel_chains, 1 + words]`` -> ``[n_nodes, K,
+    1 + n_params]`` (:meth:`fold`), and gives the oracle's per-row terms (:meth:`oracle`).  This base is the identity
+    layout: one column per chain whose theta row is the chain's inputs flattened in order."""
+
+    columns = 1
+    n_classes = 1
+    tc_only = True   # no kernel but the bf16 tensor-core one evaluates the family
+
+    def __init__(self, m) -> None:
+        self.family, self.K, self.G, self.P = m.family, m.n_chains, m.n_groups, m.n_features
+        self.shapes = [(self.G,), (self.P,)]
+        self.words = self.G + self.P
+        self._views = None
+
+    @staticmethod
+    def _no_classes(n_classes) -> None:
+        if n_classes is not None:
+            raise ValueError("n_classes is for family='multinomial' or 'ordinal' only")
+
+    def call_context(self, inputs):
+        batched = np.ndim(inputs[1]) == 1 + len(self.shapes[1])
+        return (batched, np.shape(inputs[0])) + tuple(np.shape(x) for x in inputs[2:])
+
+    def pack(self, inputs, out: np.ndarray):
+        views = self._views
+        if views is None or views[0] is not out:
+            # float32 windows into the staging buffer, built once per buffer (this runs on every evaluation)
+            th = out.view(np.float32).reshape(self.K, self.words)
+            views = self._views = (out, _split(th, [(n,) for n in (int(np.prod(s)) for s in self.shapes)]))
+        xs = [x if type(x) is np.ndarray else np.asarray(x) for x in inputs]
+        for view, x in zip(views[1], xs):
+            view[...] = x.reshape(view.shape)   # converts to float32 while it copies
+        return self.call_context(xs)
+
+    def _theta_rows(self, words: np.ndarray) -> np.ndarray:
+        """Words -> ``[K, n_params]``, each chain's inputs flattened in order."""
+        return words.view(np.float32).reshape(self.K, -1)
+
+    def inputs_from_words(self, words: np.ndarray):
+        th = self._theta_rows(words)
+        return [x.copy() for x in _split(th if self.K > 1 else th[0], self.shapes)]
+
+    def fold(self, raw: np.ndarray, ctx) -> np.ndarray:
+        return raw
+
+    def _matrices(self, inputs):
+        """``(intercepts [G, K], beta [P, K])`` of one call as float64 host tensors."""
+        return _f64(inputs[0]).reshape(self.K, self.G).T, _f64(inputs[1]).reshape(self.K, self.P).T
+
+    def oracle(self, inputs, device, dtype):
+        """``(intercepts [G, E], beta [P, E], terms)`` of one call, the first two float64 on the host, with E the
+        columns of eta; ``terms(y, w, eta)`` gives a chunk's per-row terms ``(ll, dll/deta)`` (dispersion families:
+        and ``dll/dlog_dispersion``) as ``[n, K]`` tensors, or ``[n, K, columns]`` where a chain has several kernel
+        columns, unweighted."""
+        raise NotImplementedError
+
+    def baseline(self, m, inputs) -> np.ndarray:
+        """The partial of the collective baseline (:meth:`GlmShards.eager_partial`)."""
+        import torch
+
+        return m._partial(inputs, dtype=torch.float32, chunk_rows=1 << 62, bf16_gemms=True)
+
+
+class _Scalar(_Layout):
+    """The logistic, Poisson and Gaussian families and :class:`CustomFamily`: inputs ``(intercept[G], beta[P])``."""
+
+    tc_only = False
+
+    def __init__(self, m, n_classes) -> None:
+        self._no_classes(n_classes)
+        super().__init__(m)
+
+    def oracle(self, inputs, device, dtype):
+        return (*self._matrices(inputs), self._terms)
+
+    def _terms(self, y, w, eta):
+        import torch
+
+        yy = y.to(eta.dtype).unsqueeze(1)
+        if hasattr(self.family, "code_id"):
+            if self.family.torch_fn is None:
+                raise ValueError("this CustomFamily has no torch_fn oracle")
+            return self.family.torch_fn(yy, eta)
+        if self.family == "logistic":
+            return yy * eta - torch.nn.functional.softplus(eta), yy - torch.sigmoid(eta)
+        if self.family == "poisson":
+            mu = torch.exp(eta)
+            return yy * eta - mu, yy - mu
+        d = yy - eta
+        return -0.5 * d * d - _LOG_SQRT_2PI, d
+
+    def baseline(self, m, inputs) -> np.ndarray:
+        """Whole segments at once, fp32 elementwise work and fp32 sums."""
+        import torch
+
+        ic = torch.as_tensor(np.asarray(inputs[0], dtype=np.float32)).reshape(self.K, -1).to(m.device)
+        bt = torch.as_tensor(np.asarray(inputs[1], dtype=np.float32)).reshape(self.K, self.P).to(m.device)
+        out = torch.zeros(self.K, 1 + m.n_params, dtype=torch.float64, device=m.device)
+        for si, (X, y, g) in enumerate(zip(m.Xs, m.ys, m.groups)):
+            eta = (X @ bt.T.to(torch.bfloat16)).float() + ic[:, g]          # [n, K]
+            if m.offsets[si] is not None:
+                eta = eta + m.offsets[si].unsqueeze(1)
+            ll, r = m._weigh(si, 0, X.shape[0], *self._terms(y, None, eta))
+            out[:, 0] += ll.sum(0).double()
+            out[:, 1 + g] += r.sum(0).double()
+            out[:, 1 + self.G :] += (r.T.to(torch.bfloat16) @ X).double()
+        return out.reshape(-1).cpu().numpy()
+
+
+class _Dispersion(_Layout):
+    """``gaussian_scale`` and ``negative_binomial``: inputs ``(intercept[G], beta[P], log_dispersion)``, one kernel
+    column per chain with the theta row ``[intercept, beta, log_dispersion]`` and the output block ``[LL,
+    d intercept[G], d beta[P], d log_dispersion]``."""
+
+    def __init__(self, m, n_classes) -> None:
+        self._no_classes(n_classes)
+        _tc_kernel_only(m)
+        if m.family == "negative_binomial":
+            _check_integers(m, "counts", "[0, 2^24]", lambda y: y <= 2.0 ** 24)
+        super().__init__(m)
+        self.shapes.append(())
+        self.words += 1
+
+    def oracle(self, inputs, device, dtype):
+        ld = _f64(inputs[2]).reshape(self.K).to(device, dtype)
+        fn = _gaussian_scale_terms if self.family == "gaussian_scale" else _negative_binomial_terms
+        return (*self._matrices(inputs), lambda y, w, eta: fn(y.to(eta.dtype).unsqueeze(1), eta, ld))
+
+
+class _Softmax(_Layout):
+    """``multinomial``: inputs ``(intercept[G, C], beta[P, C])``; chain k runs as kernel columns ``k C + c`` with the
+    theta rows ``(intercept[:, c], beta[:, c])``, one ``[LL, gi[G], g[P]]`` block per chain and class."""
+
+    def __init__(self, m, n_classes) -> None:
+        _tc_kernel_only(m)
+        C = _check_classes(m, n_classes, 16, lambda c: c, "n_classes")
+        if any(o is not None for o in m.offsets):
+            raise ValueError("offsets are not supported by the multinomial family: an offset common to all classes "
+                             "cancels in the softmax")
+        _check_integers(m, "labels", f"[0, {C})", lambda y: y < C)
+        super().__init__(m)
+        self.n_classes = self.columns = C
+        self.shapes = [(self.G, C), (self.P, C)]
+
+    def pack(self, inputs, out: np.ndarray):
+        K, C, G, P = self.K, self.n_classes, self.G, self.P
+        th = out.view(np.float32).reshape(K, C, G + P)
+        ic, bt = np.asarray(inputs[0]), np.asarray(inputs[1])
+        th[:, :, :G] = ic.reshape(K, G, C).transpose(0, 2, 1)
+        th[:, :, G:] = bt.reshape(K, P, C).transpose(0, 2, 1)
+        return self.call_context([ic, bt])
+
+    def _theta_rows(self, words: np.ndarray) -> np.ndarray:
+        th = words.view(np.float32).reshape(self.K, self.n_classes, self.G + self.P)
+        return th.transpose(0, 2, 1).reshape(self.K, -1)
+
+    def fold(self, raw: np.ndarray, ctx) -> np.ndarray:
+        n, K, C, G, P = raw.shape[0], self.K, self.n_classes, self.G, self.P
+        raw = raw.reshape(n, K, C, 1 + G + P)
+        return np.concatenate([raw[..., 0].sum(axis=2)[..., None],
+                               raw[..., 1 : 1 + G].transpose(0, 1, 3, 2).reshape(n, K, G * C),
+                               raw[..., 1 + G :].transpose(0, 1, 3, 2).reshape(n, K, P * C)], axis=2)
+
+    def oracle(self, inputs, device, dtype):
+        import torch
+
+        K, C, G, P = self.K, self.n_classes, self.G, self.P
+        icpt = _f64(inputs[0]).reshape(K, G, C).permute(1, 0, 2).reshape(G, K * C)   # column k C + c
+        beta = _f64(inputs[1]).reshape(K, P, C).permute(1, 0, 2).reshape(P, K * C)
+
+        def terms(y, w, eta):
+            n = eta.shape[0]
+            hit = torch.nn.functional.one_hot(_labels(y, w), C).bool().unsqueeze(1)   # [n, 1, C]
+            logp = torch.log_softmax(eta.reshape(n, K, C), dim=-1)
+            ll = torch.where(hit, logp, torch.zeros_like(logp))
+            r = hit.to(eta.dtype) - torch.exp(logp)
+            return ll, r
+
+        return icpt, beta, terms
+
+
+class _Ordinal(_Layout):
+    """``ordinal``: inputs ``(intercept[G], beta[P], cutpoints[C - 1])``; chain k runs as kernel columns
+    ``k (C - 1) + j`` with the theta rows ``(intercept - c_j, beta)``, one ``[LL_j, gi_j[G], g_j[P]]`` block per chain
+    and cutpoint."""
+
+    def __init__(self, m, n_classes) -> None:
+        _tc_kernel_only(m)
+        C = _check_classes(m, n_classes, 17, lambda c: c - 1, "(n_classes - 1)")
+        _check_integers(m, "labels", f"[0, {C})", lambda y: y < C)
+        super().__init__(m)
+        self.n_classes, self.columns = C, C - 1
+        self.shapes.append((C - 1,))
+
+    def _table(self, inputs):
+        """``(T, ctx)``: the kernel's intercept table ``T[K, C - 1, G] = float32(intercept[g] - c_j)`` (the difference
+        taken in double, rounded once) and the call context ``(batched, intercept shape, cutpoints shape, bad)``, with
+        ``bad`` the chains whose table is not strictly decreasing in j for every group."""
+        intercept, beta, cutpoints = inputs
+        ic = np.asarray(intercept, dtype=np.float64).reshape(self.K, self.G)
+        cp = np.asarray(cutpoints, dtype=np.float64).reshape(self.K, self.columns)
+        T = (ic[:, None, :] - cp[:, :, None]).astype(np.float32)
+        ordered = np.all(T[:, 1:, :] < T[:, :-1, :], axis=(1, 2))   # NaN fails the comparison
+        bad = tuple(int(k) for k in np.flatnonzero(~ordered))
+        return T, (np.ndim(beta) == 2, np.shape(intercept), np.shape(cutpoints), bad)
+
+    def call_context(self, inputs):
+        return self._table(inputs)[1]
+
+    def pack(self, inputs, out: np.ndarray):
+        T, ctx = self._table(inputs)
+        th = out.view(np.float32).reshape(self.K, self.columns, self.G + self.P)
+        th[:, :, : self.G] = T
+        th[:, :, self.G :] = np.asarray(inputs[1]).reshape(self.K, 1, self.P)
+        return ctx
+
+    def inputs_from_words(self, words: np.ndarray):
+        # only the differences travel: intercept[g] = T[0, g], c_j = T[0, 0] - T[j, 0], in double (which packs back
+        # to the same words)
+        G = self.G
+        th = words.view(np.float32).reshape(self.K, self.columns, G + self.P)
+        ic = th[:, 0, :G].copy()
+        cp = th[:, 0, :1].astype(np.float64) - th[:, :, 0].astype(np.float64)
+        bt = th[:, 0, G:].copy()
+        if self.K == 1:
+            return ic[0], bt[0], cp[0]
+        return ic, bt, cp
+
+    def fold(self, raw: np.ndarray, ctx) -> np.ndarray:
+        n, K, C1, G = raw.shape[0], self.K, self.columns, self.G
+        raw = raw.reshape(n, K, C1, 1 + G + self.P)
+        out = np.concatenate([raw[..., 0].sum(axis=2)[..., None], raw[..., 1:].sum(axis=2),
+                              -raw[..., 1 : 1 + G].sum(axis=3)], axis=2)
+        bad = list(ctx[3])
+        out[:, bad, 0] = -np.inf
+        out[:, bad, 1:] = 0.0
+        return out
+
+    def oracle(self, inputs, device, dtype):
+        import torch
+
+        K, C1 = self.K, self.columns
+        cp = _f64(inputs[2]).reshape(K, C1).to(device, dtype)
+        inf = torch.full((K, 1), float("inf"), dtype=dtype, device=device)
+        cpad = torch.cat([-inf, cp, inf], dim=1)                     # [K, C + 1]: c_{-1} = -inf, ..., c_{C-1} = +inf
+
+        def terms(y, w, eta):
+            # r_j = dll / dz_j at z_j = eta - c_j, non-zero only for j = y and j = y - 1; each row's ll is credited to
+            # j = min(y, C - 2), as the kernel does
+            dt = eta.dtype
+            lab = _labels(y, w)
+            a = cpad[:, lab + 1].T - eta                          # c_y - eta = -z_up
+            b = cpad[:, lab].T - eta                              # c_{y-1} - eta = -z_lo
+            t = 1.0 / torch.expm1(a - b)                          # 1 / expm1(gap), 0 at the infinite ends
+            ll = torch.nn.functional.logsigmoid(a) + torch.nn.functional.logsigmoid(-b) + torch.log(-torch.expm1(b - a))
+            r_up = -torch.sigmoid(-a) - t
+            r_lo = torch.sigmoid(b) + t
+            hot = lambda j: torch.nn.functional.one_hot(j.clamp(0, C1 - 1), C1).to(dt).unsqueeze(1)   # [n, 1, C1]
+            up, lo = (lab <= C1 - 1).to(dt), (lab >= 1).to(dt)
+            ll = ll.unsqueeze(2) * hot(torch.clamp(lab, max=C1 - 1))
+            r = (r_up * up.unsqueeze(1)).unsqueeze(2) * hot(lab) + (r_lo * lo.unsqueeze(1)).unsqueeze(2) * hot(lab - 1)
+            return ll, r
+
+        return (*self._matrices(inputs), terms)
+
+
+_LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_binomial": _Dispersion,
+            "ordinal": _Ordinal}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742

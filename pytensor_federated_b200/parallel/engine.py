@@ -421,10 +421,7 @@ class FederatedEngine:
 
     def _unpack_words(self, words: np.ndarray):
         """Inverse of ``pack_theta`` for peers of the collective path: models expose
-        ``inputs_from_words`` when their inputs are not simply the float32 words."""
-        fn = getattr(self.model, "inputs_from_words", None)
-        if fn is not None:
-            return fn(words)
+        ``inputs_from_words``."""
         return default_inputs_from_words(self.model, words)
 
     # ------------------------------------------------------------------ peers
@@ -508,46 +505,13 @@ class FederatedEngine:
 
 
 def default_inputs_from_words(model: ShardModel, words: np.ndarray):
-    """theta words -> model inputs for the families shipped here."""
-    from ..models.glm import GlmShards
+    """theta words -> model inputs: the model's ``inputs_from_words``, or the float64 pairs of :class:`LinregShards`."""
     from ..models.linreg import LinregShards
-    from ..models.ode import OdeShards
 
     if isinstance(model, LinregShards):
         th = words.view(np.float64).reshape(model.n_shards_total, 2)
         return th[:, 0].copy(), th[:, 1].copy()
-    if isinstance(model, GlmShards) and model.multinomial:
-        # words [K C][G + P] (row k C + c: class c of chain k) -> intercept [K, G, C], beta [K, P, C]
-        th = words.view(np.float32).reshape(model.n_chains, model.n_classes, model.n_groups + model.n_features)
-        ic, bt = th[:, :, : model.n_groups].transpose(0, 2, 1), th[:, :, model.n_groups :].transpose(0, 2, 1)
-        if model.n_chains == 1:
-            return ic[0].copy(), bt[0].copy()
-        return ic.copy(), bt.copy()
-    if isinstance(model, GlmShards) and model.dispersion:
-        # words [K][G + P + 1] -> intercept [K, G], beta [K, P], log_dispersion [K] (one chain: [G], [P], scalar)
-        th = words.view(np.float32).reshape(model.n_chains, model.n_params)
-        G, P = model.n_groups, model.n_features
-        ic, bt, ld = th[:, :G], th[:, G : G + P], th[:, G + P]
-        if model.n_chains == 1:
-            return ic[0].copy(), bt[0].copy(), ld[0].copy()
-        return ic.copy(), bt.copy(), ld.copy()
-    if isinstance(model, GlmShards) and model.ordinal:
-        # words [K (C - 1)][G + P], row k (C - 1) + j = (intercept - c_j, beta) of chain k.  Only the differences
-        # travel, so the inputs come back shifted to c_0 = 0 (the likelihood does not see the shift):
-        # intercept[g] = T[0, g], c_j = T[0, 0] - T[j, 0], in double, which packs back to the same words
-        G, P, C1 = model.n_groups, model.n_features, model.n_classes - 1
-        th = words.view(np.float32).reshape(model.n_chains, C1, G + P)
-        ic = th[:, 0, :G].copy()
-        cp = th[:, 0, :1].astype(np.float64) - th[:, :, 0].astype(np.float64)
-        bt = th[:, 0, G:].copy()
-        if model.n_chains == 1:
-            return ic[0], bt[0], cp[0]
-        return ic, bt, cp
-    if isinstance(model, GlmShards):
-        th = words.view(np.float32).reshape(model.n_chains, model.n_params)
-        if model.n_chains == 1:
-            return th[0, : model.n_groups].copy(), th[0, model.n_groups :].copy()
-        return th[:, : model.n_groups].copy(), th[:, model.n_groups :].copy()
-    if isinstance(model, OdeShards):
-        return model.inputs_from_words(words)
+    fn = getattr(model, "inputs_from_words", None)
+    if fn is not None:
+        return fn(words)
     raise FederationError(f"{type(model).__name__} must implement inputs_from_words()")

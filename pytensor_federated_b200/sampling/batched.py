@@ -163,32 +163,18 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
     short last tile is padded by repeating its last chain, so 64 chains on a K = 16 engine cost four passes over the
     data instead of sixty-four.
 
-    A multinomial engine (``family="multinomial"``, C classes) takes ``theta = [intercept (G, C), beta (P, C)]`` per
-    chain, both flattened row-major; one with a dispersion parameter (``"gaussian_scale"``, ``"negative_binomial"``)
-    takes ``theta = [intercept[G], beta[P], log_dispersion]``, and an ordinal one (``"ordinal"``, C categories)
-    ``theta = [intercept[G], beta[P], cutpoints[C-1]]``.  Gradients come back in the order of theta."""
-    cap = int(getattr(engine.model, "n_chains", 1))
-    n_classes = int(getattr(engine.model, "n_classes", 1)) if getattr(engine.model, "multinomial", False) else 1
-    dispersion = bool(getattr(engine.model, "dispersion", False))
-    # trailing theta columns that form the third input: log_dispersion, or the ordinal family's C - 1 cutpoints
-    n_third = 1 if dispersion else (int(engine.model.n_classes) - 1 if getattr(engine.model, "ordinal", False) else 0)
-    split = n_groups * n_classes   # theta columns that are intercepts
-
-    def shaped(ic: np.ndarray, beta: np.ndarray):
-        """Inputs of ``engine.evaluate``; ``ic`` / ``beta`` have the chains (if any) in their leading axis (with a
-        dispersion parameter, ``beta``'s last column is ``log_dispersion``; ordinal: its last C - 1 columns are the
-        cutpoints)."""
-        if dispersion:
-            return ic, beta[..., :-1], beta[..., -1]
-        if n_third:
-            return ic, beta[..., :-n_third], beta[..., -n_third:]
-        if n_classes == 1:
-            return ic, beta
-        lead = ic.shape[:-1]
-        return ic.reshape(lead + (n_groups, n_classes)), beta.reshape(lead + (-1, n_classes))
+    ``theta`` per chain is the model's inputs flattened row-major and concatenated
+    (:meth:`~pytensor_federated_b200.models.GlmShards.inputs_from_theta`): ``[intercept (G, C), beta (P, C)]`` for a
+    multinomial engine, ``[intercept[G], beta[P], log_dispersion]`` for one with a dispersion parameter and
+    ``[intercept[G], beta[P], cutpoints[C-1]]`` for an ordinal one.  ``n_groups`` is the model's G.  Gradients come
+    back in the order of theta."""
+    m = engine.model
+    if n_groups != m.n_groups:
+        raise ValueError(f"n_groups={n_groups} but the engine's model has {m.n_groups} intercept groups")
+    cap = int(m.n_chains)
 
     def tile(theta: np.ndarray):
-        logp, *grads = engine.evaluate(*shaped(theta[:, :split], theta[:, split:]))
+        logp, *grads = engine.evaluate(*m.inputs_from_theta(theta))
         return np.asarray(logp).reshape(-1), np.concatenate([np.asarray(g).reshape(cap, -1) for g in grads], axis=1)
 
     def fn(theta: np.ndarray):
@@ -203,7 +189,7 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
             if k < cap:
                 block = np.concatenate([block, np.repeat(block[-1:], cap - k, axis=0)], axis=0)
             if cap == 1:   # single-chain engines take unbatched inputs
-                logp, *outs = engine.evaluate(*shaped(block[0, :split], block[0, split:]))
+                logp, *outs = engine.evaluate(*m.inputs_from_theta(block[0]))
                 lp, gr = np.asarray(logp).reshape(1), np.concatenate([np.asarray(g).reshape(-1) for g in outs])[None]
             else:
                 lp, gr = tile(block)

@@ -101,7 +101,9 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 // [LL, gi[G], g[P], dlog_dispersion]; ORD = the ordinal (cumulative-logit) family (code 6), whose C - 1 cutpoints
 // ride along N like the multinomial classes: column v = k (C - 1) + j is cutpoint j of chain k, its intercept table
 // row holds intercept - c_j (packed by the host), so MMA #1 gives z_j = eta - c_j, and the columns of one row are
-// coupled only through tc::ordinal_loglik.  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// coupled only through tc::ordinal_loglik; SURV (with DISP) = the right-censored survival families (codes 7 and 8,
+// tc::weibull_loglik / tc::lognormal_loglik), which share DISP's layout and take each row's event from the sign of
+// its y (+t event, -t censored; log |y| is computed once per row).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -129,7 +131,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD>
+template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD, bool SURV>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -240,7 +242,10 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (size_t i = threadIdx.x; i < sum_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
             icpt_table[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
-        if constexpr (DISP)
+        if constexpr (SURV)
+            for (int k = threadIdx.x; k < KC; k += blockDim.x)
+                survival_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
+        else if constexpr (DISP)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = term * C8 + chain
@@ -427,6 +432,14 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                             o = valid && has_o ? row_slot[o_slot * kTileM + row] : 0.f;
                             wt = valid && has_w ? row_slot[w_slot * kTileM + row] : 1.f;
                         }
+                        // SURV: the row's event and log time, shared by its chains (a row past the segment reads y = 0,
+                        // -inf here, and is dropped below; a masked row's NaN is removed by the weight's select)
+                        bool sv_event = true;
+                        float sv_lt = 0.f;
+                        if constexpr (SURV) {
+                            sv_event = !signbit(y);
+                            sv_lt = logf(fabsf(y));
+                        }
                         // SOFTMAX: the row's log-sum-exp per chain over the quad; every lane takes part, whether its
                         // row is valid or not (a row past the segment is dropped below, as in the other families)
                         float sm_ll[2 * NJ], sm_r[2 * NJ];
@@ -477,8 +490,13 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                         float et = eta + icpt[k];
                                         if constexpr (ROWS) et = __fadd_rn(et, o);
                                         const float* dt = disp + k * kDispWords;   // k < nch <= KC: inside the table
-                                        if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
-                                        else negbin_loglik(y, et, dt, ll, r, dq);
+                                        if constexpr (SURV) {
+                                            if (prm.family == 7) weibull_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
+                                            else lognormal_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
+                                        } else {
+                                            if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
+                                            else negbin_loglik(y, et, dt, ll, r, dq);
+                                        }
                                         if constexpr (ROWS) {
                                             ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
                                             r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
@@ -700,7 +718,7 @@ extern "C" int b200_glm_tc_chunk_table(const long long* n_rows, int n_segments, 
 }
 
 // doubles in the partial array of the tensor-core kernel: one row of (hi, lo) pairs + per-warp LL slots per CTA
-// (dispersion = 1: families 4 and 5, whose slots also hold dlog_dispersion)
+// (dispersion = 1: families 4, 5, 7 and 8, whose slots also hold dlog_dispersion)
 extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int dispersion) {
     return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups, dispersion ? 1 : 0);
 }
@@ -711,7 +729,7 @@ extern "C" int b200_glm_tc_stages(int n_features, int n_chains, int n_groups, in
     const int kc = chains_bucket(n_chains);
     if (kc == 0) return 0;
     const int n1 = kc <= 8 ? 24 : 48, n2 = ((2 * kc + 7) / 8) * 8;   // Cfg<kc>
-    const bool disp = family == 4 || family == 5;
+    const bool disp = family == 4 || family == 5 || family == 7 || family == 8;
     return (int)tc::smem_layout((n_features + 127) & ~127, n1, n2, 0, disp ? tc::kDispWords : 0, kc,
                                 tc::row_arrays(row_data != 0, row_data)).stages;
 }
@@ -722,12 +740,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD)                                                                    \
+#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD, SURV)                                                                    \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
                                                  DISP ? tc::kDispWords : 0, KC, tc::row_arrays(ROWS, prm->row_data)); \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -738,34 +756,41 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD>, *comm, segs_dev, *prm, maps,       \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV>, *comm, segs_dev, *prm, maps,       \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
     if (prm->family == 3) {                 // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
         if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false); else LAUNCH_TC(4, false, true, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false); else LAUNCH_TC(8, false, true, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, true, false, false); else LAUNCH_TC(16, false, true, false, false); }
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false, false); else LAUNCH_TC(4, false, true, false, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false, false); else LAUNCH_TC(8, false, true, false, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, true, false, false, false); else LAUNCH_TC(16, false, true, false, false, false); }
     }
     else if (prm->family == 6) {            // ordinal: K (C - 1) cutpoint columns; C = 2, K = 1 runs the KC = 1 bucket
         if (prm->n_classes < 2 || prm->n_chains % (prm->n_classes - 1) != 0) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true); else LAUNCH_TC(1, false, false, false, true); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true); else LAUNCH_TC(4, false, false, false, true); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true); else LAUNCH_TC(8, false, false, false, true); }
-        else { if (rows) LAUNCH_TC(16, true, false, false, true); else LAUNCH_TC(16, false, false, false, true); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true, false); else LAUNCH_TC(1, false, false, false, true, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true, false); else LAUNCH_TC(4, false, false, false, true, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true, false); else LAUNCH_TC(8, false, false, false, true, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, false, true, false); else LAUNCH_TC(16, false, false, false, true, false); }
+    }
+    else if (prm->family == 7 || prm->family == 8) {   // right-censored survival: the dispersion layout, SURV epilogue
+        if (prm->n_classes != 1) return -3;
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, true); else LAUNCH_TC(1, false, false, true, false, true); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, true); else LAUNCH_TC(4, false, false, true, false, true); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, true); else LAUNCH_TC(8, false, false, true, false, true); }
+        else { if (rows) LAUNCH_TC(16, true, false, true, false, true); else LAUNCH_TC(16, false, false, true, false, true); }
     }
     else if (prm->family == 4 || prm->family == 5) {   // learned dispersion: theta rows [G + P + 1]
         if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false); else LAUNCH_TC(1, false, false, true, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false); else LAUNCH_TC(4, false, false, true, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false); else LAUNCH_TC(8, false, false, true, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, true, false); else LAUNCH_TC(16, false, false, true, false); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, false); else LAUNCH_TC(1, false, false, true, false, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, false); else LAUNCH_TC(4, false, false, true, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, false); else LAUNCH_TC(8, false, false, true, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, true, false, false); else LAUNCH_TC(16, false, false, true, false, false); }
     }
-    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false); else LAUNCH_TC(1, false, false, false, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false); else LAUNCH_TC(4, false, false, false, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false); else LAUNCH_TC(8, false, false, false, false); }
-    else { if (rows) LAUNCH_TC(16, true, false, false, false); else LAUNCH_TC(16, false, false, false, false); }
+    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false, false); else LAUNCH_TC(1, false, false, false, false, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false); else LAUNCH_TC(4, false, false, false, false, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false); else LAUNCH_TC(8, false, false, false, false, false); }
+    else { if (rows) LAUNCH_TC(16, true, false, false, false, false); else LAUNCH_TC(16, false, false, false, false, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

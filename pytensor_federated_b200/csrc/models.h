@@ -28,14 +28,16 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8: [.., log_dispersion])
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8: [K][G+P+1])
     int family;           // 0 = logistic (Bernoulli), 1 = Poisson (log link), 2 = Gaussian (identity, unit variance),
                           // 3 = multinomial (softmax over n_classes columns; tensor-core bf16 kernel only),
                           // 4 = Gaussian with unknown scale (log_dispersion = log sigma), 5 = negative binomial (NB2,
                           // log link, log_dispersion = log alpha); 4 and 5: tensor-core bf16 kernel only, output
                           // block per chain [LL, gi[G], g[P], dLL/dlog_dispersion], 6 = ordinal (cumulative logit,
-                          // n_classes = C categories, C - 1 cutpoint columns per chain; tensor-core bf16 kernel only)
+                          // n_classes = C categories, C - 1 cutpoint columns per chain; tensor-core bf16 kernel only),
+                          // 7 = Weibull, 8 = log-normal right-censored survival (AFT, log_dispersion = log sigma;
+                          // y = +t for an event, -t for a censored row; the layout and kernel of 4 and 5)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)

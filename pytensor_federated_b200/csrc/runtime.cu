@@ -596,12 +596,13 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         g_last_error = "n_classes must be 1 for every family but the multinomial and ordinal ones";
         return -38;
     }
-    // families 4 and 5 (Gaussian with unknown scale, negative binomial) carry a log-dispersion parameter after
-    // beta; like family 3 they exist in the bf16 tensor-core kernel only
-    const bool dispersion = family == 4 || family == 5;
+    // families 4 and 5 (Gaussian with unknown scale, negative binomial) and 7 and 8 (right-censored Weibull and
+    // log-normal survival, with s = log sigma) carry a log-dispersion parameter after beta; like family 3 they exist
+    // in the bf16 tensor-core kernel only
+    const bool dispersion = family == 4 || family == 5 || family == 7 || family == 8;
     if (dispersion && use_tensor_cores != 1) {
-        g_last_error = family == 4 ? "the gaussian_scale family runs on the bf16 tensor-core kernel only"
-                                   : "the negative_binomial family runs on the bf16 tensor-core kernel only";
+        static const char* const names[] = {"gaussian_scale", "negative_binomial", "", "weibull", "lognormal"};
+        g_last_error = std::string("the ") + names[family - 4] + " family runs on the bf16 tensor-core kernel only";
         return -39;
     }
     // checked before any engine state changes, so a refused call leaves the engine's model as it was

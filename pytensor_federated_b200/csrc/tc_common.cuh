@@ -467,5 +467,57 @@ __device__ __forceinline__ void negbin_loglik(float y, float eta, const float* t
     q = alpha * (dpsi - sp) - r;
 }
 
+// Right-censored survival, accelerated failure time: log T = eta + sigma eps, s = log sigma, z = (log t - eta) / sigma,
+// delta = 1 for an event and 0 for a censored row.  Family 7 (Weibull, eps standard minimum-Gumbel, shape 1 / sigma)
+// and family 8 (log-normal, eps ~ N(0, 1)) use the Gaussian's table words kDwSinv and kDwS.  The host stores each
+// row's time signed in y: +t for an event, -t for a censored row (times are > 0, so the sign bit is free), and the
+// kernel takes t = |y|, delta = !signbit(y); log t is a per-row value, computed once per row with logf.
+__device__ inline void survival_constants(float ld, float* t) {
+    t[kDwSinv] = (float)exp(-(double)ld);
+    t[kDwS] = ld;
+}
+
+// Family 7 of one row: ll = delta (z - s - log t) - e^z, r = dll/deta = (e^z - delta) / sigma,
+// q = dll/ds = z (e^z - delta) - delta.
+__device__ __forceinline__ void weibull_loglik(bool event, float lt, float eta, const float* t, float& ll, float& r,
+                                               float& q) {
+    const float sinv = t[kDwSinv];
+    const float z = (lt - eta) * sinv;
+    const float ez = expf(z);
+    const float d = event ? 1.f : 0.f;
+    ll = event ? ((z - ez) - t[kDwS]) - lt : -ez;
+    r = (ez - d) * sinv;
+    q = z * (ez - d) - d;
+}
+
+// Family 8 of one row.  Event: ll = -z^2 / 2 - s - log(2 pi) / 2 - log t, r = z / sigma, q = z^2 - 1.  Censored:
+// ll = log Phi(-z), r = lambda / sigma, q = z lambda with the inverse Mills ratio lambda = phi(z) / Phi(-z).  With
+// u = z / sqrt(2), Phi(-z) = erfc(u) / 2.  Both signs of u go through one erfcx(a) = e^{a^2} erfc(a) at a = |u|, which
+// neither underflows nor loses relative accuracy in the upper tail (fp32 Phi(-z) is subnormal from z ~ 13 and 0 from
+// z ~ 14, so log(normcdf(-z)) would give -inf there):
+//   u >= 0:  log Phi(-z) = log(erfcx(u) / 2) - u^2,   lambda = sqrt(2 / pi) / erfcx(u)
+//   u <  0:  log Phi(-z) = log1p(-h),                 lambda = phi(z) / (1 - h),   h = erfc(-u) / 2 = erfcx(a) e^{-a^2} / 2
+__device__ __forceinline__ void lognormal_loglik(bool event, float lt, float eta, const float* t, float& ll, float& r,
+                                                 float& q) {
+    const float sinv = t[kDwSinv];
+    const float z = (lt - eta) * sinv;
+    if (event) {
+        ll = ((-0.5f * z * z - 0.918938533204672742f) - t[kDwS]) - lt;
+        r = z * sinv;
+        q = z * z - 1.f;
+        return;
+    }
+    const float u = z * 0.707106781186547524f;
+    const float a2 = u * u;
+    const float ex = erfcxf(fabsf(u));
+    const float g = expf(-a2);                       // e^{-u^2} = sqrt(2 pi) phi(z)
+    const float h = 0.5f * ex * g;                   // u < 0: erfc(-u) / 2 = 1 - Phi(-z) <= 1/2
+    ll = u >= 0.f ? logf(0.5f * ex) - a2 : log1pf(-h);
+    const float lam = u >= 0.f ? 0.797884560802865356f / ex                  // sqrt(2 / pi) / erfcx(u)
+                               : 0.398942280401432678f * g / (1.f - h);      // phi(z) / Phi(-z)
+    r = lam * sinv;
+    q = z * lam;
+}
+
 
 }  // namespace tc

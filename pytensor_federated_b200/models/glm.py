@@ -9,7 +9,7 @@ Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
 
 How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
 oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
-``_Ordinal`` below); :class:`GlmShards` and its callers are generic over it.
+``_Ordinal``, ``_Survival`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ import numpy as np
 from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
-            "ordinal": 6}
+            "ordinal": 6, "weibull": 7, "lognormal": 8}
 
 
 def _family_code(family) -> int:
@@ -138,6 +138,30 @@ class GlmShards(ShardModel):
         unaffected.  Nothing is raised, so a sampler can step there and reject the proposal.  To sample, use an
         ordered transform such as ``c = cumsum([c0, exp(d_1), ..., exp(d_{C-2})])`` and apply the chain rule to the
         cutpoint gradient on the host: ``dLL/dc0 = sum_j dLL/dc_j``, ``dLL/dd_m = exp(d_m) sum_{j >= m} dLL/dc_j``.
+
+        ``"weibull"`` and ``"lognormal"`` are right-censored survival regression (accelerated failure time, as
+        ``survreg`` and lifelines fit them, PyMC's ``pm.Censored`` and brms' ``y | cens(c)``): ``ys`` holds the
+        times ``t > 0`` and ``events`` whether each row's event was observed.  With ``eta = intercept[group] + x' beta
+        + o``, ``log T = eta + sigma eps`` and ``s = log sigma`` learned, the inputs and gradients are those of
+        ``gaussian_scale``: ``(intercept, beta, log_dispersion)`` with ``log_dispersion = s``.  With ``z = (log t -
+        eta) / sigma`` and ``delta`` = 1 for an event, 0 for a censored row (the event had not happened by ``t``):
+
+            weibull (eps standard minimum-Gumbel):   ll = delta (z - s - log t) - e^z
+            lognormal (eps ~ N(0, 1)):               ll = delta (-z^2 / 2 - s - log(2 pi) / 2 - log t)
+                                                          + (1 - delta) log Phi(-z)
+
+        The event rows' LL is the density of T, ``-log t`` included, so it equals ``scipy.stats.weibull_min(c=1 /
+        sigma, scale=e^eta)`` and ``lognorm(s=sigma, scale=e^eta)``, ``logpdf`` for events and ``logsf`` for censored
+        rows.  The Weibull shape is ``k = e^{-s}`` and its scale ``e^eta``; as a proportional-hazards model its
+        coefficients are ``-beta / sigma``.  An offset shifts the location of log T; weights work as for every
+        family, and a row of weight 0 may carry any time and event.  Times must be finite and > 0 and events 0 or 1
+        on every row of non-zero weight.  ``events`` takes one entry per segment: ``None`` (every row an event) or a
+        1-D tensor or array of 0 / 1 of the segment's rows (on the device of X, like ``offsets``); it is rejected
+        for every other family.  The model keeps a float32 copy of the times with censored rows negated, which is
+        what the kernel reads (the tensors passed in are not modified).  Only the bf16 tensor-core kernel evaluates
+        these families, with the shape limits of the multinomial one; ``n_classes`` is rejected.
+    events
+        Per-row event indicators of the survival families (see ``family``).
     """
 
     def __init__(
@@ -156,6 +180,7 @@ class GlmShards(ShardModel):
         offsets: Optional[Sequence] = None,
         weights: Optional[Sequence] = None,
         n_classes: Optional[int] = None,
+        events: Optional[Sequence] = None,
     ) -> None:
         import torch
 
@@ -194,6 +219,10 @@ class GlmShards(ShardModel):
         if self.node_ids is not None and (len(self.node_ids) != len(self.Xs) or not all(0 <= i < self.n_nodes for i in self.node_ids)):
             raise ValueError("node_ids needs one node index in [0, n_nodes) per segment")
         layout = _LAYOUTS.get(family, _Scalar) if isinstance(family, str) else _Scalar
+        if events is not None and not layout.takes_events:
+            raise ValueError(f"events= is for family='weibull' or 'lognormal' only, not {family!r}")
+        #: per-row event indicators of the survival families (one float32 tensor or None per segment)
+        self.events = self._row_data(events, "events")
         self._layout = lay = layout(self, n_classes)
         #: classes per chain (multinomial and ordinal families; 1 for every other family)
         self.n_classes = lay.n_classes
@@ -344,7 +373,7 @@ class GlmShards(ShardModel):
 
         n = len(self.Xs)
         Xp = native.void_p_array([X.data_ptr() for X in self.Xs])
-        yp = native.void_p_array([y.data_ptr() for y in self.ys])
+        yp = native.void_p_array([y.data_ptr() for y in self._layout.kernel_ys])
         kernel_scales = getattr(self, "_kernel_scales", None) or self.scales   # fp8: packed per tile
         sp = native.void_p_array([s.data_ptr() for s in kernel_scales]) if kernel_scales else None
         rows = (C.c_longlong * n)(*[X.shape[0] for X in self.Xs])
@@ -411,7 +440,7 @@ class GlmShards(ShardModel):
         G, P = self.n_groups, self.n_features
         step = self.kernel_chains // B.shape[1]   # kernel columns per column of eta
         full = torch.zeros(self.n_nodes, self.kernel_chains, 1 + lay.words, dtype=torch.float64, device=self.device)
-        for si, (X, y, g) in enumerate(zip(self.Xs, self.ys, self.groups)):
+        for si, (X, y, g) in enumerate(zip(self.Xs, lay.kernel_ys, self.groups)):
             out = full[self.node_ids[si] if self.node_ids is not None else 0]
             w = self.weights[si]
             for r0 in range(0, X.shape[0], chunk_rows):
@@ -524,9 +553,12 @@ class _Layout:
     columns = 1
     n_classes = 1
     tc_only = True   # no kernel but the bf16 tensor-core one evaluates the family
+    takes_events = False   # the survival families' per-row event indicators
 
     def __init__(self, m) -> None:
         self.family, self.K, self.G, self.P = m.family, m.n_chains, m.n_groups, m.n_features
+        #: the per-row values the kernel and the oracle read as y (the model's ``ys`` but for the survival families)
+        self.kernel_ys = m.ys
         self.shapes = [(self.G,), (self.P,)]
         self.words = self.G + self.P
         self._views = None
@@ -642,8 +674,33 @@ class _Dispersion(_Layout):
 
     def oracle(self, inputs, device, dtype):
         ld = _f64(inputs[2]).reshape(self.K).to(device, dtype)
-        fn = _gaussian_scale_terms if self.family == "gaussian_scale" else _negative_binomial_terms
+        fn = _DISPERSION_TERMS[self.family]
         return (*self._matrices(inputs), lambda y, w, eta: fn(y.to(eta.dtype).unsqueeze(1), eta, ld))
+
+
+class _Survival(_Dispersion):
+    """``weibull`` and ``lognormal``: the layout of :class:`_Dispersion` with ``log_dispersion = log sigma``.  The
+    event indicator travels in the sign of the kernel's y: ``kernel_ys`` is a float32 copy of the times, negated on
+    censored rows (times are > 0, so negation is exact and frees the sign bit); the oracle decodes it the same way."""
+
+    takes_events = True
+
+    def __init__(self, m, n_classes) -> None:
+        import torch
+
+        super().__init__(m, n_classes)
+        signed = []
+        for si, (t, ev, w) in enumerate(zip(m.ys, m.events, m.weights)):
+            keep = torch.ones_like(t, dtype=torch.bool) if w is None else w != 0   # a masked row may carry anything
+            if bool(torch.any(keep & ~(torch.isfinite(t) & (t > 0)))):
+                raise ValueError(f"times of segment {si} must be finite and > 0 on every row of non-zero weight")
+            if ev is None:
+                signed.append(t)
+                continue
+            if bool(torch.any(keep & ~((ev == 0) | (ev == 1)))):
+                raise ValueError(f"events of segment {si} must be 0 or 1 on every row of non-zero weight")
+            signed.append(_aligned16(torch.where(ev == 0, -t, t).contiguous()))
+        self.kernel_ys = signed
 
 
 class _Softmax(_Layout):
@@ -784,7 +841,7 @@ class _Ordinal(_Layout):
 
 
 _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_binomial": _Dispersion,
-            "ordinal": _Ordinal}
+            "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -830,6 +887,47 @@ def _negative_binomial_terms(y, eta, a):
     ll = D + y * eta - (alpha + y) * sp
     r = y - (alpha + y) * torch.sigmoid(x)
     return ll, r, alpha * (dpsi - sp) - r
+
+
+def _survival_split(y, eta, s):
+    """``(delta, log t, z, 1 / sigma)`` of rows whose times carry the event in their sign (+t event, -t censored)."""
+    import torch
+
+    event = ~torch.signbit(y)
+    lt = torch.log(y.abs())
+    sinv = torch.exp(-s)
+    return event, lt, (lt - eta) * sinv, sinv
+
+
+def _weibull_terms(y, eta, s):
+    """``(ll, dll/deta, dll/ds)`` of the right-censored Weibull AFT model, ``sigma = exp(s)``: shape ``1 / sigma``,
+    scale ``exp(eta)``; ``y`` = +t for an event, -t for a censored row."""
+    import torch
+
+    event, lt, z, sinv = _survival_split(y, eta, s)
+    ez = torch.exp(z)
+    d = event.to(eta.dtype)
+    ll = torch.where(event, z - ez - s - lt, -ez)
+    return ll, (ez - d) * sinv, z * (ez - d) - d
+
+
+def _lognormal_terms(y, eta, s):
+    """``(ll, dll/deta, dll/ds)`` of the right-censored log-normal AFT model, ``sigma = exp(s)``; ``y`` as in
+    :func:`_weibull_terms`.  Censored rows use ``log_ndtr``, relatively accurate far into the upper tail, and the
+    inverse Mills ratio ``phi(z) / Phi(-z)`` as the exponential of a difference of logs."""
+    import torch
+
+    event, lt, z, sinv = _survival_split(y, eta, s)
+    log_sf = torch.special.log_ndtr(-z)
+    lam = torch.exp(-0.5 * z * z - _LOG_SQRT_2PI - log_sf)
+    ll = torch.where(event, -0.5 * z * z - s - _LOG_SQRT_2PI - lt, log_sf)
+    r = torch.where(event, z, lam) * sinv
+    q = torch.where(event, z * z - 1.0, z * lam)
+    return ll, r, q
+
+
+_DISPERSION_TERMS = {"gaussian_scale": _gaussian_scale_terms, "negative_binomial": _negative_binomial_terms,
+                     "weibull": _weibull_terms, "lognormal": _lognormal_terms}
 
 
 def quantize_block_fp8(X, block: int = 32):
@@ -1018,6 +1116,51 @@ def synth_ordinal_shard(n_rows: int, n_features: int, n_classes: int, *, seed: i
         u = torch.rand(r1 - r0, 1, generator=gen, device=device)
         y[r0:r1] = (u > cdf).sum(1).float()
     return X, y, beta_true, cuts.astype(np.float32)
+
+
+def synth_survival_shard(n_rows: int, n_features: int, *, family: str, sigma: float, censor_fraction: float, seed: int,
+                         device, chunk_rows: int = 1 << 20, beta_scale: float = 0.05, intercept: float = 0.5):
+    """Synthetic right-censored survival shard generated on the device in chunks: bf16 ``X ~ N(0,1)``, event times
+    ``log T = X beta* + intercept + sigma eps`` with ``eps`` standard minimum-Gumbel (``family="weibull"``) or
+    N(0, 1) (``"lognormal"``), and censoring times ``C`` drawn independently of T from the same family with the
+    location shifted by one constant, chosen (for the marginal of ``X beta*``) so that about ``censor_fraction`` of
+    the rows are censored.  The observed time is ``min(T, C)`` and the event ``T <= C``.  ``censor_fraction`` = 0
+    gives no censoring.  Returns ``(X, time, event, beta*)``, time and event float32."""
+    import torch
+
+    if family not in ("weibull", "lognormal"):
+        raise ValueError(f"family must be 'weibull' or 'lognormal', got {family!r}")
+    if not 0.0 <= censor_fraction < 1.0:
+        raise ValueError(f"censor_fraction must be in [0, 1), got {censor_fraction}")
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+
+    def eps(n):
+        u = torch.rand(n, generator=gen, device=device, dtype=torch.float64).clamp(1e-300, 1.0)
+        return torch.log(-torch.log(u)) if family == "weibull" else torch.randn(n, generator=gen, device=device,
+                                                                                 dtype=torch.float64)
+
+    shift = float("inf")
+    if censor_fraction > 0:
+        # log C - log T = shift + sigma (eps_c - eps_t), with x' beta* cancelled: P(C < T) is censor_fraction when
+        # -shift is that quantile of sigma (eps_c - eps_t), estimated from 2^20 pairs
+        diff = sigma * (eps(1 << 20) - eps(1 << 20))
+        shift = -float(torch.quantile(diff.cpu().float(), censor_fraction))
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    time = torch.empty(n_rows, dtype=torch.float32, device=device)
+    event = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        loc = (xb.float() @ beta_true + intercept).double()
+        log_t = loc + sigma * eps(r1 - r0)
+        log_c = loc + shift + sigma * eps(r1 - r0)
+        ev = log_t <= log_c
+        time[r0:r1] = torch.exp(torch.where(ev, log_t, log_c)).float()
+        event[r0:r1] = ev.float()
+    return X, time, event, beta_true
 
 
 def synth_logistic_shard_fp8(n_rows: int, n_features: int, *, seed: int, device, chunk_rows: int = 1 << 20):

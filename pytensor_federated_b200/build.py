@@ -92,6 +92,32 @@ def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) 
     return LIB
 
 
+def build_snippet_library(source: str, macro: str, snippet: str, defines: List[str], name: str, what: str) -> Path:
+    """Compiles ``csrc/<source>`` with a user's CUDA snippet as the body of ``macro`` into
+    ``csrc/build/custom/<name>.so`` (kept as a cache: ``name`` must cover everything the build depends on).
+
+    The snippet reaches nvcc through a generated header named after its content, which ``source`` includes
+    as ``B200FED_SNIPPET_HEADER``: nvcc splits ``-D`` values at commas, so a snippet such as
+    ``pow(y[0], 0.5f)`` cannot travel as one.  ``what`` names the snippet in the error nvcc's rejection raises."""
+    custom = BUILD / "custom"
+    custom.mkdir(parents=True, exist_ok=True)
+    so = custom / f"{name}.so"
+    if so.exists():
+        return so
+    text = f"// generated from a user snippet\n#define {macro} {' '.join(snippet.split())}\n"
+    header = custom / f"b200fed_snippet_{hashlib.sha256(text.encode()).hexdigest()[:16]}.h"
+    if not header.exists():
+        tmp = header.with_suffix(f".{os.getpid()}.tmp")
+        tmp.write_text(text)
+        os.replace(tmp, header)          # concurrent builds of the same snippet write the same bytes
+    cmd = [nvcc_path(), *ARCH, *NVCC_FLAGS, "-shared", "-I", str(CSRC), "-I", str(custom),
+           f"-DB200FED_SNIPPET_HEADER=<{header.name}>", *defines, str(CSRC / source), "-o", str(so), "-lcudart"]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if res.returncode != 0:
+        raise RuntimeError(f"nvcc rejected the {what}:\n{res.stderr[-3000:]}")
+    return so
+
+
 def dump_sass(out_dir: Optional[Path] = None) -> Path:
     """Writes ``cuobjdump -sass`` of the library (HGMMA / UTMALDG / multimem instructions) to ``out_dir``."""
     out_dir = Path(out_dir or BUILD)

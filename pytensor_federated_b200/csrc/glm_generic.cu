@@ -9,6 +9,9 @@
 #include <cuda_bf16.h>
 #include "fed_comm.cuh"
 #include "models.h"
+#ifdef B200FED_SNIPPET_HEADER
+#include B200FED_SNIPPET_HEADER   // defines B200FED_CUSTOM_LINK (models/custom.py, build.py)
+#endif
 
 namespace {
 

@@ -15,10 +15,14 @@
 // broadcast -> solve -> reduce through fed_comm.cuh like every other model.
 //
 // Compiled per system by models/ode.py (nvcc, cached by content hash) with
-//   -DB200FED_ODE_NS=<states> -DB200FED_ODE_NP=<parameters> -DB200FED_ODE_RHS=<snippet>
+//   -DB200FED_ODE_NS=<states> -DB200FED_ODE_NP=<parameters> and B200FED_ODE_RHS=<snippet> defined by a generated
+// header (B200FED_SNIPPET_HEADER, see build.py: nvcc would split a -D value at the snippet's commas).
 // Without those macros this file builds the Lotka-Volterra instance (used by the tests as a cross-check of ode.cu).
 #include "fed_comm.cuh"
 #include "models.h"
+#ifdef B200FED_SNIPPET_HEADER
+#include B200FED_SNIPPET_HEADER
+#endif
 
 #ifndef B200FED_ODE_NS
 #define B200FED_ODE_NS 2
@@ -88,7 +92,15 @@ __device__ __forceinline__ Dual cos(const Dual& a) { return chain1(cosf(a.v), -s
 __device__ __forceinline__ Dual tanh(const Dual& a) { const float t = tanhf(a.v); return chain1(t, 1.f - t * t, a); }
 __device__ __forceinline__ Dual pow(const Dual& a, float p) { return chain1(powf(a.v, p), p * powf(a.v, p - 1.f), a); }
 __device__ __forceinline__ Dual square(const Dual& a) { return chain1(a.v * a.v, 2.f * a.v, a); }
-// plain-float overloads so that a snippet may call the same names on constants
+// plain-float overloads so that a snippet may call the same names on constants and on `t` (the Dual overloads
+// above hide the global float functions inside this namespace)
+__device__ __forceinline__ float exp(float a) { return expf(a); }
+__device__ __forceinline__ float log(float a) { return logf(a); }
+__device__ __forceinline__ float sqrt(float a) { return sqrtf(a); }
+__device__ __forceinline__ float sin(float a) { return sinf(a); }
+__device__ __forceinline__ float cos(float a) { return cosf(a); }
+__device__ __forceinline__ float tanh(float a) { return tanhf(a); }
+__device__ __forceinline__ float pow(float a, float p) { return powf(a, p); }
 __device__ __forceinline__ float square(float a) { return a * a; }
 
 // The user's right-hand side.  `T` is Dual here; the snippet must not name the type.

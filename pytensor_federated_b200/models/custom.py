@@ -22,13 +22,11 @@ from __future__ import annotations
 
 import ctypes as C
 import hashlib
-import subprocess
 from pathlib import Path
 from typing import Callable, Optional
 
 _PKG = Path(__file__).resolve().parent.parent
 _CSRC = _PKG / "csrc"
-_CACHE = _CSRC / "build" / "custom"
 
 
 class CustomFamily:
@@ -55,17 +53,9 @@ class CustomFamily:
             return self._lib
         from .. import build as native_build
 
-        _CACHE.mkdir(parents=True, exist_ok=True)
-        so = _CACHE / f"libb200fed_custom_{self.digest()}.so"
-        if not so.exists():
-            cmd = [
-                native_build.nvcc_path(), *native_build.ARCH, *native_build.NVCC_FLAGS, "-shared", "-I", str(_CSRC),
-                f"-DB200FED_CUSTOM_LINK={self.cuda_code}", "-DB200FED_GENERIC_ENTRY=b200_launch_glm_custom",
-                str(_CSRC / "glm_generic.cu"), "-o", str(so), "-lcudart",
-            ]
-            res = subprocess.run(cmd, capture_output=True, text=True)
-            if res.returncode != 0:
-                raise RuntimeError(f"nvcc rejected the custom likelihood:\n{res.stderr[-3000:]}")
+        so = native_build.build_snippet_library(
+            "glm_generic.cu", "B200FED_CUSTOM_LINK", self.cuda_code, ["-DB200FED_GENERIC_ENTRY=b200_launch_glm_custom"],
+            f"libb200fed_custom_{self.digest()}", "custom likelihood")
         self._lib = C.CDLL(str(so))
         return self._lib
 

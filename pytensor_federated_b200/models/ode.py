@@ -15,7 +15,8 @@ from __future__ import annotations
 
 import ctypes as C
 import hashlib
-import subprocess
+import math
+import numbers
 from pathlib import Path
 from typing import Callable, List, Optional, Sequence
 
@@ -25,7 +26,6 @@ from .base import ShardModel
 
 _PKG = Path(__file__).resolve().parent.parent
 _CSRC = _PKG / "csrc"
-_CACHE = _CSRC / "build" / "custom"
 
 
 def lv_rhs(u, v, th):
@@ -38,8 +38,11 @@ class OdeSystem:
 
     ``rhs_cuda``
         CUDA C statements assigning ``dy[0..n_states)`` from ``y[...]``, ``th[...]`` and the float ``t``.
-        The operands are dual numbers: ``+ - * /``, unary minus, mixing with float literals, and
-        ``exp log sqrt sin cos tanh pow(x, p) square`` are available; do not name the scalar type.
+        ``y`` and ``th`` are dual numbers (value and d/dtheta); do not name their type.  ``+ - * /`` and unary
+        minus take two duals or a dual and a float, in either order.  ``exp log sqrt sin cos tanh square`` and
+        ``pow(x, p)`` take a dual ``x`` (then ``p`` is a float) or a float, such as ``t`` or a literal, and then
+        return a float: ``sin(1.5f * t)`` is a float forcing term, ``cos(th[2] * t)`` a dual.  ``pow`` of a
+        dual exponent is not available.
     ``rhs_torch``
         The same right-hand side for tensors: ``rhs_torch(y, th, t) -> sequence of n_states tensors`` with
         ``y`` a sequence of state tensors and ``th`` a 1-D tensor — used by the eager oracle, whose
@@ -79,18 +82,11 @@ class OdeSystem:
             return self._lib
         from .. import build as native_build
 
-        _CACHE.mkdir(parents=True, exist_ok=True)
-        so = _CACHE / f"libb200fed_ode_{self.digest()}.so"
-        if not so.exists():
-            cmd = [
-                native_build.nvcc_path(), *native_build.ARCH, *native_build.NVCC_FLAGS, "-shared", "-I", str(_CSRC),
-                f"-DB200FED_ODE_NS={self.n_states}", f"-DB200FED_ODE_NP={self.n_params}",
-                f"-DB200FED_ODE_RHS={self.rhs_cuda}", "-DB200FED_ODE_ENTRY=b200_launch_ode_custom",
-                str(_CSRC / "ode_generic.cu"), "-o", str(so), "-lcudart",
-            ]
-            res = subprocess.run(cmd, capture_output=True, text=True)
-            if res.returncode != 0:
-                raise RuntimeError(f"nvcc rejected the ODE right-hand side:\n{res.stderr[-3000:]}")
+        so = native_build.build_snippet_library(
+            "ode_generic.cu", "B200FED_ODE_RHS", self.rhs_cuda,
+            [f"-DB200FED_ODE_NS={self.n_states}", f"-DB200FED_ODE_NP={self.n_params}",
+             "-DB200FED_ODE_ENTRY=b200_launch_ode_custom"],
+            f"libb200fed_ode_{self.digest()}", "ODE right-hand side")
         self._lib = C.CDLL(str(so))
         return self._lib
 
@@ -134,7 +130,14 @@ class OdeShards(ShardModel):
         for y0, yo, t in zip(self.y0s, self.y_obs, self.ts):
             if y0.shape[0] != self.n_states or yo.shape[1] != self.n_states or yo.shape[0] != t.numel() or yo.shape[2] != y0.shape[1]:
                 raise ValueError("expected y0 [n_states, n_series] and y_obs [n_t, n_states, n_series]")
-        self.sigmas = [float(s) for s in sigmas]
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError("every time point must be finite")
+        self.sigmas = [float(np.float32(s)) for s in sigmas]    # what the kernels see, and so the oracle too
+        if len(self.sigmas) != len(self.ts) or not all(math.isfinite(s) and s > 0 for s in self.sigmas):
+            raise ValueError(f"sigmas needs one finite sigma > 0 per shard, got {sigmas!r}")
+        # substeps = 0 would give h = inf and no RK4 step at all: the likelihood of y0 at every time point
+        if isinstance(substeps, bool) or not isinstance(substeps, numbers.Integral) or substeps < 1:
+            raise ValueError(f"substeps must be an integer >= 1, got {substeps!r}")
         self.substeps = int(substeps)
         self.device = self.ts[0].device
         if self.node_ids is not None and (len(self.node_ids) != len(self.ts) or not all(0 <= i < self.n_nodes for i in self.node_ids)):

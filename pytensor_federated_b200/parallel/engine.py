@@ -368,6 +368,11 @@ class FederatedEngine:
     def kernel_launches(self) -> int:
         return int(self._lib.b200_engine_launches(self._handle)) if self._handle else 0
 
+    @property
+    def grid(self) -> int:
+        """CTAs per launch of the model kernel (fused backend; negative values select single-CTA modes)."""
+        return int(self._lib.b200_engine_grid(self._handle)) if self._handle else 0
+
     def trace(self, epoch: int) -> Tuple[int, int, int]:
         buf = (C.c_ulonglong * 4)()
         self._lib.b200_engine_trace(self._handle, epoch, buf)

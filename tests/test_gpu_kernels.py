@@ -500,7 +500,7 @@ def test_glm_fp8_keeps_per_node_output_blocks(dev):
     np.testing.assert_allclose(summed[0], want[:, 0, 0].sum(), rtol=2e-5)
 
 
-@pytest.mark.parametrize("which", ["glm-tc", "glm-fp8", "glm-simt", "linreg-1cta", "linreg-multi"])
+@pytest.mark.parametrize("which", ["glm-tc", "glm-fp8", "glm-simt", "linreg-1cta", "linreg-multi", "ode", "ode-system"])
 def test_speculative_root_launches_give_the_same_results(dev, which):
     """`set_speculative`: the next evaluation's kernel is enqueued before theta exists and picks it up as tagged
     words from host memory.  Same bits as one launch per evaluation; kernels that wait in vain give up (idle
@@ -518,6 +518,12 @@ def test_speculative_root_launches_give_the_same_results(dev, which):
         else:
             model = GlmShards(Xs, ys, groups=[0, 1], n_groups=2, kernel=which.split("-")[1])
         thetas = [[rng.normal(size=2) * 0.1, (rng.normal(size=256) * 0.03).astype(np.float32)] for _ in range(12)]
+    elif which.startswith("ode"):
+        from pytensor_federated_b200.models import LOTKA_VOLTERRA
+
+        shards = [synth_lv_shard(n, 8, seed=s, device=dev) for s, n in enumerate([300, 129])]
+        model = OdeShards(*[[s[i] for s in shards] for i in range(4)], system=LOTKA_VOLTERRA if which == "ode-system" else None)
+        thetas = [[np.array([1.0, 0.4, 0.8, 0.2]) * (1 + 0.05 * rng.normal(size=4))] for _ in range(12)]
     else:
         sizes = [10] if which == "linreg-1cta" else [10, 70001, 333]
         xs = [rng.normal(size=n) for n in sizes]

@@ -21,7 +21,7 @@ Environment variables (all optional):
                             PEM files that switch the gRPC path to TLS (see :class:`TlsConfig`)
 ``B200FED_ALLOW_PICKLE``    set to decode object-dtype arrays (unpickles peer data: trusted federations only)
 ``B200FED_NO_LL``           set to force the fence + flag protocol for small results (default: flag-in-data words)
-``B200FED_LL_MAX_VALS`` / ``B200FED_LL_MAX_THETA``   size thresholds of the flag-in-data protocol (128 / 256)
+``B200FED_LL_MAX_VALS`` / ``B200FED_LL_MAX_THETA``   size thresholds of the flag-in-data protocol (2048 values / 4096 words)
 """
 from __future__ import annotations
 

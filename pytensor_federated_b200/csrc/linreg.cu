@@ -109,9 +109,18 @@ __global__ void __launch_bounds__(256) fed_linreg_kernel(FedComm comm, const Lin
 
 extern "C" int b200_launch_linreg(const FedComm* comm, const LinregShard* shards_dev, int n_shards, int dtype_is_f64,
                                   int grid, cudaStream_t stream) {
+    // theta (16 bytes per shard of the federation) lives in dynamic shared memory: from 3056 shards on, it and the
+    // kernel's static variables (< 256 bytes) need more than the default 48 KB, which a launch gets only after
+    // opting in, up to 227 KB (LinregShards.MAX_SHARDS_TOTAL).  Smaller models skip the call and launch as before.
     const size_t smem = ((comm->n_theta * 4 + 15) & ~15) + 32 * sizeof(double);
     const int small_mode = grid < 0 ? 1 : 0;  // negative grid = "one CTA, warp per shard"
     if (grid < 0) grid = 1;
+    if (smem > 48 * 1024 - 256) {
+        const cudaError_t err =
+            dtype_is_f64 ? cudaFuncSetAttribute(fed_linreg_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                         : cudaFuncSetAttribute(fed_linreg_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (err != cudaSuccess) return (int)err;
+    }
     if (dtype_is_f64)
         fed_linreg_kernel<double><<<grid, 256, smem, stream>>>(*comm, shards_dev, n_shards, small_mode);
     else

@@ -60,6 +60,10 @@ enum ModelKind { MODEL_NONE = 0, MODEL_LINREG = 1, MODEL_GLM_SIMT = 2, MODEL_GLM
 
 thread_local std::string g_last_error;
 
+// return code of every entry point whose kernel launch failed (b200_last_error names the CUDA error);
+// FederatedEngine._raise knows it
+constexpr int B200FED_RC_LAUNCH_FAILED = -10;
+
 int fail(const char* what, cudaError_t err) {
     g_last_error = std::string(what) + ": " + cudaGetErrorString(err);
     return (int)err ? (int)err : -1;
@@ -250,8 +254,10 @@ int launch_model(Engine* e, const FedComm* c) {
             return -2;
     }
     if (rc != 0) {
+        // a positive rc is the launch's cudaError_t; it must not reach callers that read positive codes as the
+        // completion flag's status bits (1 would read as "theta never arrived")
         g_last_error = std::string("kernel launch failed: ") + (rc > 0 ? cudaGetErrorString((cudaError_t)rc) : "unsupported shape");
-        return rc;
+        return B200FED_RC_LAUNCH_FAILED;
     }
     e->launches++;
     return 0;
@@ -740,8 +746,12 @@ int b200_engine_launch(void* h) {
     fill_comm(e, &c, true);
     c.epoch = ++e->epoch;
     const int rc = launch_model(e, &c);
-    if (rc == 0 && e->spec_enabled) e->spec_launched++;
-    return rc;
+    if (rc != 0) {
+        e->epoch--;   // nothing runs this epoch: the next launch takes it, and device-side epoch counts stay in step
+        return rc;
+    }
+    if (e->spec_enabled) e->spec_launched++;
+    return 0;
 }
 
 // One launch that takes its theta from the tagged host words and its epoch from the device counter.
@@ -765,7 +775,8 @@ int b200_engine_set_device_theta(void* h, const float* theta_host, int n, int en
 }
 
 // Wait (host spin on the mapped completion flag) for epoch `epoch`; copies the result.
-// Returns 0, or 1 = theta timeout, 2 = peer timeout (bit-or), -5 = host-side timeout.
+// Returns 0, or 1 = theta timeout, 2 = peer timeout (bit-or), -5 = host-side timeout,
+// B200FED_RC_LAUNCH_FAILED = a speculative launch failed.
 int b200_engine_wait(void* h, unsigned long long epoch, double* out, double timeout_s) {
     Engine* e = static_cast<Engine*>(h);
     volatile unsigned long long* flag = e->h_flag();
@@ -787,7 +798,7 @@ int b200_engine_wait(void* h, unsigned long long epoch, double* out, double time
             v = *flag;
             if ((v & B200FED_EPOCH_MASK) >= epoch && (v >> B200FED_STATUS_SHIFT) != 0) return (int)(v >> B200FED_STATUS_SHIFT);
             if ((++spins & 0xFFF) == 0) {
-                if (e->spec_enabled && !e->theta_from_device && e->spec_in_flight() == 0 && spec_launch(e) != 0) return -8;
+                if (e->spec_enabled && !e->theta_from_device && e->spec_in_flight() == 0 && spec_launch(e) != 0) return B200FED_RC_LAUNCH_FAILED;
                 const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
                 if (dt > timeout_s) {
                     cudaError_t err = cudaStreamQuery(e->stream);
@@ -810,7 +821,7 @@ int b200_engine_wait(void* h, unsigned long long epoch, double* out, double time
         v = *flag;
         if ((v & B200FED_EPOCH_MASK) >= epoch) break;
         if ((++spins & 0xFFF) == 0) {
-            if (e->spec_enabled && !e->theta_from_device && e->spec_in_flight() == 0 && spec_launch(e) != 0) return -8;
+            if (e->spec_enabled && !e->theta_from_device && e->spec_in_flight() == 0 && spec_launch(e) != 0) return B200FED_RC_LAUNCH_FAILED;
             const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
             if (dt > timeout_s) {
                 cudaError_t err = cudaStreamQuery(e->stream);

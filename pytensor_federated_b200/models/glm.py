@@ -24,6 +24,10 @@ FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gauss
             "ordinal": 6, "weibull": 7, "lognormal": 8}
 
 
+#: dynamic shared memory one CTA may opt in to on the H100 (227 KB), less 256 bytes for a kernel's static variables
+CTA_SMEM_LIMIT = 227 * 1024 - 256
+
+
 def _family_code(family) -> int:
     return family.code_id if hasattr(family, "code_id") else FAMILIES[family]
 
@@ -325,7 +329,35 @@ class GlmShards(ShardModel):
     # -- native ----------------------------------------------------------------------------
     def use_tensor_cores(self):
         """Kernel selector passed to the runtime: 0 = SIMT, 1 = tensor cores (bf16), 2 = block-scaled fp8,
-        3 / 4 = general-shape fallback (bf16 / fp32 design matrix)."""
+        3 / 4 = general-shape fallback (bf16 / fp32 design matrix).  Raises ValueError for a CUDA-core model whose
+        shared memory would exceed what one CTA can have."""
+        code = self._select_kernel()
+        if code in (0, 3, 4) and self.cuda_core_smem_bytes(code) > CTA_SMEM_LIMIT:
+            fits, too_many = 0, self.n_groups   # the most groups that fit (bytes grow with the group count)
+            while too_many - fits > 1:
+                mid = (fits + too_many) // 2
+                fits, too_many = (mid, too_many) if self.cuda_core_smem_bytes(code, mid) <= CTA_SMEM_LIMIT else (fits, mid)
+            raise ValueError(
+                f"the CUDA-core GLM kernels keep theta and one accumulator per group in shared memory: {self.n_groups} "
+                f"groups with {self.n_features} features need {self.cuda_core_smem_bytes(code)} bytes, more than the "
+                f"{CTA_SMEM_LIMIT} a CTA can have; at most {fits} groups fit")
+        return code
+
+    def cuda_core_smem_bytes(self, code: int, n_groups: Optional[int] = None) -> int:
+        """Dynamic shared memory of one CTA of the SIMT (``code`` 0) or general-shape (3, 4) kernel, by the
+        formulas of ``b200_glm_simt_smem`` (csrc/glm_simt.cu) and ``launch_generic`` (csrc/glm_generic.cu),
+        for this model or for the same model with ``n_groups`` groups."""
+        G = self.n_groups if n_groups is None else int(n_groups)
+        n_theta = self.n_theta_words + (G - self.n_groups) * self.kernel_chains
+        P = self.n_features
+        if code == 0:
+            per_warp = ((P + 255) // 256) * 256
+        else:
+            j = (P + 31) // 32
+            per_warp = (8 if j <= 8 else 16 if j <= 16 else 32) * 32
+        return ((n_theta + 3) & ~3) * 4 + 8 * per_warp * 4 + ((G + 1) & ~1) * 8 + 32 * 8
+
+    def _select_kernel(self) -> int:
         import torch
 
         X0 = self.Xs[0]

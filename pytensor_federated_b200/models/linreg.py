@@ -29,6 +29,10 @@ def make_demo_data(seed: int = 123, n: int = 10, sigma: float = 0.4):
 class LinregShards(ShardModel):
     """Shards ``local_ids`` (global shard indices) of an ``n_shards_total`` federation."""
 
+    #: largest federation the kernel takes: theta (16 bytes per shard) and a 256-byte reduction buffer share the
+    #: 227 KB of shared memory one CTA can have on the H100, less 256 bytes for the kernel's static variables
+    MAX_SHARDS_TOTAL = (227 * 1024 - 256 - 256) // 16
+
     def __init__(
         self,
         xs: Sequence,
@@ -48,6 +52,18 @@ class LinregShards(ShardModel):
         self.n_shards_total = int(n_shards_total if n_shards_total is not None else len(xs))
         if len(xs) != len(ys) or len(xs) != len(sigmas) or len(xs) != len(self.local_ids):
             raise ValueError("xs, ys, sigmas and local_ids must have the same length")
+        if self.n_shards_total > self.MAX_SHARDS_TOTAL:
+            raise ValueError(f"{self.n_shards_total} shards in total: the kernel keeps theta in shared memory, which "
+                             f"holds at most {self.MAX_SHARDS_TOTAL}")
+        if not all(0 <= s < self.n_shards_total for s in self.local_ids) or len(set(self.local_ids)) != len(self.local_ids):
+            raise ValueError(f"local_ids must be distinct shard indices in [0, {self.n_shards_total})")
+        for s, (x, y, sigma) in enumerate(zip(xs, ys, sigmas)):
+            # the kernel reads n = len(x) rows of both arrays
+            if np.ndim(x) != 1 or np.ndim(y) != 1 or np.shape(x) != np.shape(y):
+                raise ValueError(f"x and y of shard {s} must be 1-D with the same length, got shapes "
+                                 f"{tuple(np.shape(x))} and {tuple(np.shape(y))}")
+            if not (np.isfinite(float(sigma)) and float(sigma) > 0.0):
+                raise ValueError(f"sigma of shard {s} must be finite and > 0, got {sigma}")
         self.xs = [torch.as_tensor(np.asarray(x), dtype=self.dtype).to(self.device).contiguous() for x in xs]
         self.ys = [torch.as_tensor(np.asarray(y), dtype=self.dtype).to(self.device).contiguous() for y in ys]
         self.sigmas = [float(s) for s in sigmas]

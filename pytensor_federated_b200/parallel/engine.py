@@ -32,6 +32,8 @@ from ..models.base import ShardModel
 _log = logging.getLogger(__name__)
 
 _STOP = -1.0
+#: return code of the native runtime when a kernel launch failed (csrc/runtime.cu: B200FED_RC_LAUNCH_FAILED)
+RC_LAUNCH_FAILED = -10
 
 
 class FederationError(RuntimeError):
@@ -326,15 +328,21 @@ class FederatedEngine:
             )
         if rc == -5:
             raise FederationTimeout(native.last_error())
+        if rc == RC_LAUNCH_FAILED:
+            raise FederationError(
+                f"the model kernel could not be launched ({native.last_error()}); nothing was evaluated"
+            )
         raise FederationError(f"native evaluation failed (rc={rc}): {native.last_error()}")
 
     # device-timed benchmarking hooks (root, fused)
     def launch(self) -> int:
         """Enqueues one evaluation with the current theta (``set_device_theta`` or the last ``evaluate``)
         and returns its epoch without waiting.  Results live in ONE host-mapped buffer: with several
-        epochs in flight ``wait`` returns the newest completed result, and models small enough for the
-        flag-in-data protocol (``n_vals <= 128``) must ``wait`` for each epoch before launching the next —
-        their result words are tagged with the exact epoch."""
+        epochs in flight ``wait`` returns the newest completed result.  Models whose results travel as
+        tagged words (the flag-in-data protocol of docs/PROTOCOL.md: ``n_vals <= 2048`` by default,
+        ``B200FED_LL_MAX_VALS``) must ``wait`` for each epoch before launching the next: waiting for an
+        older epoch while newer ones are in flight is not supported, since the copy can then mix the
+        words of two epochs."""
         rc = self._lib.b200_engine_launch(self._handle)
         if rc != 0:
             self._raise(rc)
@@ -346,6 +354,17 @@ class FederatedEngine:
         if rc != 0:
             self._raise(rc)
         return self._out
+
+    def reset(self) -> None:
+        """Single-node fused engine: waits for the launches in its stream, then clears its epoch count,
+        completion flags, tagged-word mailboxes and reduction tickets, as a new engine would start.  The
+        next evaluation is epoch 1 again."""
+        from ..ops import native
+
+        if self.backend != "fused" or self.world != 1:
+            raise FederationError("reset() is for single-node engines on the fused backend")
+        with self._lock:
+            native.check(self._lib.b200_engine_reset(self._handle), "engine reset")
 
     def set_device_theta(self, inputs: Sequence[np.ndarray], enable: bool = True) -> None:
         """Parks theta in device memory so back-to-back launches need no host traffic."""

@@ -103,7 +103,12 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 // row holds intercept - c_j (packed by the host), so MMA #1 gives z_j = eta - c_j, and the columns of one row are
 // coupled only through tc::ordinal_loglik; SURV (with DISP) = the right-censored survival families (codes 7 and 8,
 // tc::weibull_loglik / tc::lognormal_loglik), which share DISP's layout and take each row's event from the sign of
-// its y (+t event, -t censored; log |y| is computed once per row).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
+// its y (+t event, -t censored; log |y| is computed once per row); HVP = Hessian-vector products of families 0 to 2
+// (GlmParams::family carries kGlmHvp, masked off for the family branch): pair p runs as column 2p (theta_p, the scalar
+// epilogue unchanged) and column 2p + 1 (a direction v_p: the host packs theta row 2p + 1 = (v_intercept, v_beta),
+// so the intercept table's odd rows are v_intercept), whose epilogue writes ll = 0 and r = w h(eta_2p) u with u its
+// own eta without the offset; its output block is then [0, (H v)_intercept[G], (H v)_beta[P]].  Both columns of a pair
+// sit in one thread (e = 0 and e = 1).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
 // 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
 template <int KC>
 struct Cfg {
@@ -131,7 +136,7 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD, bool SURV>
+template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD, bool SURV, bool HVP>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
@@ -477,7 +482,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                                        od_ll, od_r);
                         }
 #pragma unroll
-                        for (int jc = 0; jc < NJ; ++jc)
+                        for (int jc = 0; jc < NJ; ++jc) {
+                            float hv_h = 0.f;   // HVP: h = d2ll / deta2 of the pair's theta column (e = 0), for e = 1
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int k = 8 * jc + 2 * q + e;
@@ -518,6 +524,25 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                             ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
                                             r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
                                         }
+                                    } else if constexpr (HVP) {
+                                        // column 2p (e = 0): theta_p, exactly as the scalar families below, plus h at
+                                        // its eta; column 2p + 1 (e = 1): the direction v_p, u = x'v_beta + v_intercept
+                                        // (no offset: u is linear in v), ll = 0 and r = s = w h u, so that MMA #2 and
+                                        // the intercept sums give (H v)_beta and (H v)_intercept
+                                        const int fam = prm.family & ~kGlmHvp;
+                                        if (e == 0) {
+                                            float et = eta + icpt[k];
+                                            if constexpr (ROWS) et = __fadd_rn(et, o);
+                                            link_loglik(fam, y, et, ll, r);
+                                            hv_h = link_curvature(fam, et);
+                                            if constexpr (ROWS) {
+                                                ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
+                                                r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                            }
+                                        } else {
+                                            r = __fmul_rn(hv_h, eta + icpt[k]);
+                                            if constexpr (ROWS) r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                        }
                                     } else if constexpr (ROWS) {
                                         // offset after the intercept, weight after the likelihood, both rounded on their
                                         // own (no FMA contraction): w = 1, o = 0 gives the bits of the plain model; a
@@ -540,6 +565,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                     *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k + 1) % 8) * 16) = lo;
                                 }
                             }
+                        }
                     }
                     fence_proxy_async();
                     named_sync(1, 32 * kConsumerWarps);   // R of all 128 rows written
@@ -740,12 +766,12 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
     const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD, SURV)                                                                    \
+#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP)                                                                    \
     do {                                                                                                           \
         const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
                                                  DISP ? tc::kDispWords : 0, KC, tc::row_arrays(ROWS, prm->row_data)); \
         if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
+        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
         cudaLaunchConfig_t cfg{};                                                                                  \
         cfg.gridDim = dim3(grid);                                                                                  \
         cfg.blockDim = dim3(tc::kThreads);                                                                         \
@@ -756,41 +782,47 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
         attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
         cfg.attrs = attr;                                                                                          \
         cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV>, *comm, segs_dev, *prm, maps,       \
+        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP>, *comm, segs_dev, *prm, maps,       \
                            reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
     } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
-    if (prm->family == 3) {                 // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
+    if (prm->family & kGlmHvp) {            // Hessian-vector products: K (theta, v) pairs as columns 2k, 2k + 1
+        if (kc == 1 || prm->n_chains % 2 != 0 || (prm->family & ~kGlmHvp) > 2) return -3;
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false, true); else LAUNCH_TC(4, false, false, false, false, false, true); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false, true); else LAUNCH_TC(8, false, false, false, false, false, true); }
+        else { if (rows) LAUNCH_TC(16, true, false, false, false, false, true); else LAUNCH_TC(16, false, false, false, false, false, true); }
+    }
+    else if (prm->family == 3) {                // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
         if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false, false); else LAUNCH_TC(4, false, true, false, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false, false); else LAUNCH_TC(8, false, true, false, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, true, false, false, false); else LAUNCH_TC(16, false, true, false, false, false); }
+        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false, false, false); else LAUNCH_TC(4, false, true, false, false, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false, false, false); else LAUNCH_TC(8, false, true, false, false, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, true, false, false, false, false); else LAUNCH_TC(16, false, true, false, false, false, false); }
     }
     else if (prm->family == 6) {            // ordinal: K (C - 1) cutpoint columns; C = 2, K = 1 runs the KC = 1 bucket
         if (prm->n_classes < 2 || prm->n_chains % (prm->n_classes - 1) != 0) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true, false); else LAUNCH_TC(1, false, false, false, true, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true, false); else LAUNCH_TC(4, false, false, false, true, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true, false); else LAUNCH_TC(8, false, false, false, true, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, false, true, false); else LAUNCH_TC(16, false, false, false, true, false); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true, false, false); else LAUNCH_TC(1, false, false, false, true, false, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true, false, false); else LAUNCH_TC(4, false, false, false, true, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true, false, false); else LAUNCH_TC(8, false, false, false, true, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, false, true, false, false); else LAUNCH_TC(16, false, false, false, true, false, false); }
     }
     else if (prm->family == 7 || prm->family == 8) {   // right-censored survival: the dispersion layout, SURV epilogue
         if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, true); else LAUNCH_TC(1, false, false, true, false, true); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, true); else LAUNCH_TC(4, false, false, true, false, true); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, true); else LAUNCH_TC(8, false, false, true, false, true); }
-        else { if (rows) LAUNCH_TC(16, true, false, true, false, true); else LAUNCH_TC(16, false, false, true, false, true); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, true, false); else LAUNCH_TC(1, false, false, true, false, true, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, true, false); else LAUNCH_TC(4, false, false, true, false, true, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, true, false); else LAUNCH_TC(8, false, false, true, false, true, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, true, false, true, false); else LAUNCH_TC(16, false, false, true, false, true, false); }
     }
     else if (prm->family == 4 || prm->family == 5) {   // learned dispersion: theta rows [G + P + 1]
         if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, false); else LAUNCH_TC(1, false, false, true, false, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, false); else LAUNCH_TC(4, false, false, true, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, false); else LAUNCH_TC(8, false, false, true, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, true, false, false); else LAUNCH_TC(16, false, false, true, false, false); }
+        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, false, false); else LAUNCH_TC(1, false, false, true, false, false, false); }
+        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, false, false); else LAUNCH_TC(4, false, false, true, false, false, false); }
+        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, false, false); else LAUNCH_TC(8, false, false, true, false, false, false); }
+        else { if (rows) LAUNCH_TC(16, true, false, true, false, false, false); else LAUNCH_TC(16, false, false, true, false, false, false); }
     }
-    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false, false); else LAUNCH_TC(1, false, false, false, false, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false); else LAUNCH_TC(4, false, false, false, false, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false); else LAUNCH_TC(8, false, false, false, false, false); }
-    else { if (rows) LAUNCH_TC(16, true, false, false, false, false); else LAUNCH_TC(16, false, false, false, false, false); }
+    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false, false, false); else LAUNCH_TC(1, false, false, false, false, false, false); }
+    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false, false); else LAUNCH_TC(4, false, false, false, false, false, false); }
+    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false, false); else LAUNCH_TC(8, false, false, false, false, false, false); }
+    else { if (rows) LAUNCH_TC(16, true, false, false, false, false, false); else LAUNCH_TC(16, false, false, false, false, false, false); }
 #undef LAUNCH_TC
     return (int)cudaGetLastError();
 }

@@ -37,7 +37,8 @@ struct GlmParams {
                           // block per chain [LL, gi[G], g[P], dLL/dlog_dispersion], 6 = ordinal (cumulative logit,
                           // n_classes = C categories, C - 1 cutpoint columns per chain; tensor-core bf16 kernel only),
                           // 7 = Weibull, 8 = log-normal right-censored survival (AFT, log_dispersion = log sigma;
-                          // y = +t for an event, -t for a censored row; the layout and kernel of 4 and 5)
+                          // y = +t for an event, -t for a censored row; the layout and kernel of 4 and 5);
+                          // kGlmHvp | (0, 1 or 2): Hessian-vector products of that family (tensor-core bf16 kernel only)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)
@@ -50,6 +51,11 @@ struct GlmParams {
 
 constexpr int kGlmRowOffsets = 1;
 constexpr int kGlmRowWeights = 2;
+// Flag bit on GlmParams::family: the launch evaluates pairs of columns, column 2k the parameters theta_k and column
+// 2k + 1 a direction v_k, whose output block is [0, (H v)_intercept[G], (H v)_beta[P]] with H the Hessian of LL at
+// theta_k.  Only the bf16 tensor-core kernel takes it (families 0 to 2, an even n_chains); the runtime refuses it
+// for every other kernel.
+constexpr int kGlmHvp = 16;
 
 // Unit of work of the dynamically scheduled tensor-core GLM kernel: n_tiles consecutive 128-row tiles of one
 // segment starting at tile first_tile (n_tiles is even; the last one may lie past the segment's rows).

@@ -559,9 +559,27 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
                         const float** offsets, const float** weights, int n_classes) {
     Engine* e = static_cast<Engine*>(h);
     CK(cudaSetDevice(e->device));
-    // family 3 (multinomial) exists in the bf16 tensor-core kernel only; the CUDA-core kernels would take an
-    // unknown family code for the Gaussian one, so it must never reach them
-    if (family == 3) {
+    // Hessian-vector products (kGlmHvp on family 0, 1 or 2): K (theta, v) pairs as columns 2k and 2k + 1 of a 2K-chain
+    // launch of the bf16 tensor-core kernel; every other kernel would read the flagged code as an unknown family
+    if (family & kGlmHvp) {
+        const int base = family & ~kGlmHvp;
+        if (use_tensor_cores != 1) {
+            g_last_error = "Hessian-vector products run on the bf16 tensor-core kernel only";
+            return -34;
+        }
+        if (base < 0 || base > 2) {
+            g_last_error = "Hessian-vector products exist for the logistic, Poisson and Gaussian families only";
+            return -40;
+        }
+        if (n_classes != 1) {
+            g_last_error = "n_classes must be 1 for Hessian-vector products";
+            return -38;
+        }
+        if (n_chains < 2 || n_chains > 16 || n_chains % 2 != 0) {
+            g_last_error = "Hessian-vector products need an even n_chains in [2, 16] (one theta and one direction column per pair)";
+            return -36;
+        }
+    } else if (family == 3) {
         if (use_tensor_cores != 1) {
             g_last_error = "the multinomial family runs on the bf16 tensor-core kernel only";
             return -34;

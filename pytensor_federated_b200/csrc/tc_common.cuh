@@ -228,6 +228,18 @@ __device__ __forceinline__ void link_loglik(int family, float y, float eta, floa
     }
 }
 
+// h = d2ll / deta2 of families 0 to 2 at eta (the Hessian-vector product's per-row weight): logistic -mu (1 - mu) =
+// -e / (1 + e)^2 with e = exp(-|eta|), from an accurate expf so that h keeps its relative accuracy in both tails;
+// Poisson -mu, the very __expf(eta) that link_loglik's residual uses; Gaussian -1.
+__device__ __forceinline__ float link_curvature(int family, float eta) {
+    if (family == 0) {
+        const float e = expf(-fabsf(eta));
+        const float d = 1.f + e;
+        return -e / (d * d);
+    }
+    return family == 1 ? -__expf(eta) : -1.f;
+}
+
 // Multinomial (softmax) likelihood of one row, family 3.  The row's columns are spread over the four lanes of a
 // quad (the lanes sharing lane >> 2); this lane holds NS of them: eta[s] is column s of this lane, chain[s] the
 // chain it belongs to (-1: no chain, i.e. a column past K*C) and cls[s] its class.  Per chain, the row maximum m

@@ -129,8 +129,16 @@ class NodeFederation:
     def evaluate_node(self, node: int, *inputs) -> Tuple[np.ndarray, List[np.ndarray]]:
         return self.evaluate_nodes({node: inputs})[node]
 
+    def _gradients_only(self, what: str) -> None:
+        """Refuses ``what`` for a model whose outputs after logp are not all gradients (``GlmShards(..., hvp=True)``:
+        its last two outputs are Hessian-vector products, which an Op would hand to the graph as gradients)."""
+        if getattr(self.engine.model, "hvp", False):
+            raise ValueError(f"{what} presents every output after logp as a gradient, but this model's last two outputs "
+                             "are Hessian-vector products: use evaluate_nodes, evaluate_node or compute_func")
+
     def logp_grad_func(self, node: int) -> Callable:
         """The node as a plain ``LogpGradFunc`` (usable with the generic ``LogpGradOp``)."""
+        self._gradients_only("logp_grad_func")
         return lambda *inputs: self.evaluate_node(node, *inputs)
 
     def compute_func(self, node: int) -> Callable:
@@ -155,6 +163,7 @@ class NodeFederation:
 
         With :meth:`all_nodes_op` the model graph has ONE federated node instead of one per data holder, so the
         Python cost of a model evaluation no longer grows with the size of the federation."""
+        self._gradients_only("all_nodes_func")
         kind, eng = self._kind, self.engine
         if kind == "linreg":
             def func(intercepts, slopes):
@@ -187,12 +196,14 @@ class NodeFederation:
     def node_ops(self):
         from .wrapper_ops import FederatedLogpGradOp
 
+        self._gradients_only("node_ops")
         return [FederatedLogpGradOp(self, i) for i in range(self.n_nodes)]
 
     def all_nodes_op(self):
         """One ``LogpGradOp`` over :meth:`all_nodes_func` (vector parameters in, summed logp and vector gradients out)."""
         from .wrapper_ops import LogpGradOp
 
+        self._gradients_only("all_nodes_op")
         return LogpGradOp(self.all_nodes_func())
 
     # -- reference client API ------------------------------------------------------------------

@@ -166,6 +166,24 @@ class GlmShards(ShardModel):
         these families, with the shape limits of the multinomial one; ``n_classes`` is rejected.
     events
         Per-row event indicators of the survival families (see ``family``).
+    hvp
+        Hessian-vector products of the ``"logistic"``, ``"poisson"`` and ``"gaussian"`` families.  The inputs per
+        call are ``(intercept, beta, v_intercept, v_beta)``: the parameters and a direction ``v``, shapes ``[G]``,
+        ``[P]``, ``[G]`` and ``[P]`` (a scalar intercept when G = 1), batched with a leading ``K = n_chains`` (at most
+        8).  ``evaluate`` returns ``[LL, d_intercept, d_beta, Hv_intercept, Hv_beta]``: the last two are NOT gradients
+        with respect to ``v`` but the product ``H v`` of the Hessian of LL (negative semidefinite for these families)
+        at ``(intercept, beta)`` with ``v``.  With ``h = ll''(eta)`` (logistic ``-mu (1 - mu)``, Poisson ``-mu``,
+        Gaussian ``-1``) and ``u_i = v_intercept[group] + x_i' v_beta`` (no offset: u is linear in v),
+
+            (H v)_intercept[g] = sum_{i in g} w_i h_i u_i,     (H v)_beta = sum_i w_i h_i u_i x_i.
+
+        Pair k runs as the kernel columns 2k (the parameters) and 2k + 1 (the direction) of a 2K-column launch, so
+        X is read once for K products.  Offsets and weights work as for every family (a row of weight 0 gives exactly
+        0).  Only the bf16 tensor-core kernel evaluates products: any other family, ``kernel`` other than ``"auto"``
+        or ``"tc"``, :class:`Fp8GlmShards`, shapes outside that kernel's limits, ``n_chains > 8`` and a shape whose
+        2K-column launch gets fewer than two pipeline stages (checked when an engine attaches the model) raise a
+        ValueError.  :func:`~pytensor_federated_b200.sampling.glm_hessian` assembles the full Hessian from
+        ``ceil((G + P) / K)`` launches.
     """
 
     def __init__(
@@ -185,6 +203,7 @@ class GlmShards(ShardModel):
         weights: Optional[Sequence] = None,
         n_classes: Optional[int] = None,
         events: Optional[Sequence] = None,
+        hvp: bool = False,
     ) -> None:
         import torch
 
@@ -222,7 +241,9 @@ class GlmShards(ShardModel):
         self.n_nodes = int(n_nodes) if n_nodes is not None else 1
         if self.node_ids is not None and (len(self.node_ids) != len(self.Xs) or not all(0 <= i < self.n_nodes for i in self.node_ids)):
             raise ValueError("node_ids needs one node index in [0, n_nodes) per segment")
-        layout = _LAYOUTS.get(family, _Scalar) if isinstance(family, str) else _Scalar
+        #: Hessian-vector products: every call also takes a direction per chain (see ``hvp``)
+        self.hvp = bool(hvp)
+        layout = _Hvp if self.hvp else (_LAYOUTS.get(family, _Scalar) if isinstance(family, str) else _Scalar)
         if events is not None and not layout.takes_events:
             raise ValueError(f"events= is for family='weibull' or 'lognormal' only, not {family!r}")
         #: per-row event indicators of the survival families (one float32 tensor or None per segment)
@@ -411,6 +432,14 @@ class GlmShards(ShardModel):
         rows = (C.c_longlong * n)(*[X.shape[0] for X in self.Xs])
         grp = (C.c_int * n)(*self.groups)
         code = int(self.use_tensor_cores())
+        if self.hvp:
+            # the 2K-column launch must get two TMA stages; refused here, before the engine's model changes
+            row_data = (1 if any(o is not None for o in self.offsets) else 0) | (2 if any(w is not None for w in self.weights) else 0)
+            fam = _family_code(self.family) | HVP_FLAG
+            if int(lib.b200_glm_tc_stages(self.n_features, self.kernel_chains, self.n_groups, fam, row_data)) < 2:
+                raise ValueError(f"hvp=True with {self.n_chains} pairs at P = {self.n_features}: the tensor-core kernel's "
+                                 f"{self.kernel_chains}-column launch gets fewer than two pipeline stages in shared memory; "
+                                 f"use fewer pairs per launch")
         #: which fused kernel serves this model ("tc" / "fp8" = wgmma tensor cores, else CUDA cores)
         self.selected_kernel = {0: "simt", 1: "tc", 2: "fp8", 3: "generic-bf16", 4: "generic-fp32"}[code]
         if self.kernel == "auto" and code not in (1, 2) and not hasattr(self.family, "code_id"):
@@ -428,7 +457,7 @@ class GlmShards(ShardModel):
         native.check(
             lib.b200_engine_set_glm(
                 handle, n, Xp, yp, sp, rows, grp, self.n_features, self.ld, self.n_groups,
-                self.kernel_chains, _family_code(self.family), code, out_grp, self.n_nodes, op, wp,
+                self.kernel_chains, _family_code(self.family) | (HVP_FLAG if self.hvp else 0), code, out_grp, self.n_nodes, op, wp,
                 self.n_classes,
             ),
             "set_glm",
@@ -485,7 +514,8 @@ class GlmShards(ShardModel):
                     eta = Xf @ B
                 eta = eta + icpt[g]
                 if self.offsets[si] is not None:
-                    eta = eta + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
+                    cols = lay.offset_columns
+                    eta[:, cols] = eta[:, cols] + self.offsets[si][r0:r1].to(dtype).unsqueeze(1)
                 # ll, r (and the dispersion families' q = dll/dlog_dispersion), [n, K] or [n, K, columns]
                 ll, r, *q = self._weigh(si, r0, r1, *terms(y[r0:r1], None if w is None else w[r0:r1], eta))
                 out[:, 0] += ll.double().sum(0).reshape(-1)
@@ -585,6 +615,7 @@ class _Layout:
     columns = 1
     n_classes = 1
     tc_only = True   # no kernel but the bf16 tensor-core one evaluates the family
+    offset_columns = slice(None)   # the columns of eta that take the per-row offset (all of them)
     takes_events = False   # the survival families' per-row event indicators
 
     def __init__(self, m) -> None:
@@ -608,7 +639,7 @@ class _Layout:
         views = self._views
         if views is None or views[0] is not out:
             # float32 windows into the staging buffer, built once per buffer (this runs on every evaluation)
-            th = out.view(np.float32).reshape(self.K, self.words)
+            th = out.view(np.float32).reshape(self.K, -1)
             views = self._views = (out, _split(th, [(n,) for n in (int(np.prod(s)) for s in self.shapes)]))
         xs = [x if type(x) is np.ndarray else np.asarray(x) for x in inputs]
         for view, x in zip(views[1], xs):
@@ -688,6 +719,54 @@ class _Scalar(_Layout):
             out[:, 1 + g] += r.sum(0).double()
             out[:, 1 + self.G :] += (r.T.to(torch.bfloat16) @ X).double()
         return out.reshape(-1).cpu().numpy()
+
+
+class _Hvp(_Scalar):
+    """Hessian-vector products (``GlmShards(..., hvp=True)``): inputs ``(intercept[G], beta[P], v_intercept[G],
+    v_beta[P])``; pair k runs as kernel columns 2k, with the theta row ``(intercept, beta)`` and the output block
+    ``[LL, d intercept[G], d beta[P]]``, and 2k + 1, with the theta row ``(v_intercept, v_beta)`` and the output block
+    ``[0, (H v)_intercept[G], (H v)_beta[P]]``.  Only the parameter columns take the offset."""
+
+    columns = 2
+    tc_only = True
+    offset_columns = slice(0, None, 2)
+
+    def __init__(self, m, n_classes) -> None:
+        if m.family not in ("logistic", "poisson", "gaussian"):
+            raise ValueError(f"hvp=True is for family='logistic', 'poisson' or 'gaussian', not {m.family!r}")
+        _tc_kernel_only(m)
+        if not 1 <= m.n_chains <= 8:
+            raise ValueError(f"hvp=True takes n_chains in [1, 8] (each pair of parameters and direction is two of the "
+                             f"tensor-core kernel's 16 columns per launch), got {m.n_chains}")
+        super().__init__(m, n_classes)
+        self.shapes = self.shapes * 2
+
+    def fold(self, raw: np.ndarray, ctx) -> np.ndarray:
+        n = raw.shape[0]
+        raw = raw.reshape(n, self.K, 2, 1 + self.words)
+        return np.concatenate([raw[:, :, 0], raw[:, :, 1, 1:]], axis=2)
+
+    def oracle(self, inputs, device, dtype):
+        import torch
+
+        ic, bt = self._matrices(inputs[:2])
+        vic, vbt = self._matrices(inputs[2:])
+        pairs = lambda a, b: torch.stack([a, b], dim=2).reshape(a.shape[0], -1)   # column 2k: theta, 2k + 1: v
+
+        def terms(y, w, eta):
+            et, u = eta[:, 0::2], eta[:, 1::2]
+            ll, r = self._terms(y, w, et)
+            if self.family == "logistic":
+                h = -torch.sigmoid(et) * torch.sigmoid(-et)
+            elif self.family == "poisson":
+                h = -torch.exp(et)
+            else:
+                h = -torch.ones_like(et)
+            return torch.stack([ll, torch.zeros_like(ll)], dim=2), torch.stack([r, h * u], dim=2)
+
+        return pairs(ic, vic), pairs(bt, vbt), terms
+
+    baseline = _Layout.baseline
 
 
 class _Dispersion(_Layout):
@@ -877,6 +956,8 @@ _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_bi
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
+#: flag bit on the family code of a Hessian-vector-product launch (csrc/models.h: kGlmHvp)
+HVP_FLAG = 16
 
 
 def _gaussian_scale_terms(y, eta, s):
@@ -1033,7 +1114,10 @@ class Fp8GlmShards(GlmShards):
     """
 
     def __init__(self, Xqs, scales, ys, *, groups=None, n_groups: int = 1, n_chains: int = 1,
-                 family: str = "logistic", node_ids=None, n_nodes=None, offsets=None, weights=None) -> None:
+                 family: str = "logistic", node_ids=None, n_nodes=None, offsets=None, weights=None,
+                 hvp: bool = False) -> None:
+        if hvp:
+            raise ValueError("hvp=True runs on the bf16 tensor-core kernel only, not on the block-scaled fp8 kernel")
         if not 1 <= n_chains <= 3:
             raise ValueError("the fp8 kernel batches at most 3 chains per launch")
         super().__init__(Xqs, ys, groups=groups, n_groups=n_groups, family=family, n_chains=n_chains, kernel="fp8",

@@ -9,9 +9,10 @@ callable, plus a minimal model builder over the graph IR.  With PyMC installed t
 """
 from .batched import BatchedResult, glm_batch_fn, hmc_sample_batched
 from .diagnostics import effective_sample_size, split_rhat, summarize
+from .laplace import glm_hessian, glm_hvp_fn, laplace
 from .mcmc import SamplerResult, find_map, hmc_sample, metropolis_sample, nuts_sample
 from .model import Model
 from .parallel import sample_parallel
 
 __all__ = ["Model", "SamplerResult", "find_map", "hmc_sample", "nuts_sample", "metropolis_sample", "BatchedResult", "hmc_sample_batched", "glm_batch_fn",
-           "split_rhat", "effective_sample_size", "summarize", "sample_parallel"]
+           "glm_hvp_fn", "glm_hessian", "laplace", "split_rhat", "effective_sample_size", "summarize", "sample_parallel"]

@@ -556,23 +556,6 @@ fed_glm_fp8_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParam
 
 }  // namespace fp8
 
-namespace {
-typedef CUresult (*EncodeTiledFn8)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn8 get_encode8() {
-    static EncodeTiledFn8 fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn8>(p);
-    }
-    return fn;
-}
-}  // namespace
-
 extern "C" int b200_glm_fp8_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count,
                                     void** tmaps_dev, void** chunks_dev, int* n_chunks) {
     if (prm->n_features != 128 && prm->n_features != 256) return -21;   // <= 8 scale blocks per tile row
@@ -580,7 +563,7 @@ extern "C" int b200_glm_fp8_prepare(const GlmSegment* segs_host, int n_segments,
         if (segs_host[s].n_rows + fp8::kTile * fp8::kChunkMultiple >= (1ll << 31)) return -22;   // row coordinates are 32-bit
     if (prm->n_chains < 1 || prm->n_chains > 3 || prm->family < 0 || prm->family > 2) return -23;
     if (prm->ld % 16 != 0) return -24;
-    EncodeTiledFn8 encode = get_encode8();
+    const PFN_cuTensorMapEncodeTiled encode = tc::encode_tiled();
     if (!encode) return -25;
     CUtensorMap* host = new CUtensorMap[n_segments];
     for (int s = 0; s < n_segments; ++s) {
@@ -617,40 +600,16 @@ extern "C" int b200_launch_glm_fp8(const FedComm* comm, const GlmSegment* segs_d
                                    cudaStream_t stream) {
     const fp8::SmemLayoutF L = fp8::smem_layout(prm->n_features, comm->n_theta, prm->n_groups);
     if (L.stages < 2) return -2;
-    const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define B200FED_FP8_LAUNCH(KF, DYN, ROWS)                                                                                 \
-    do {                                                                                                                 \
-        cudaFuncSetAttribute(fp8::fed_glm_fp8_kernel<KF, DYN, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
-                             (int)L.total);                                                                              \
-        cudaLaunchConfig_t cfg{};                                                                                        \
-        cfg.gridDim = dim3(grid);                                                                                        \
-        cfg.blockDim = dim3(fp8::kThreadsF);                                                                             \
-        cfg.dynamicSmemBytes = L.total;                                                                                  \
-        cfg.stream = stream;                                                                                             \
-        cudaLaunchAttribute attr[1];                                                                                     \
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                 \
-        attr[0].val.programmaticStreamSerializationAllowed = 1;                                                          \
-        cfg.attrs = attr;                                                                                                \
-        cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                            \
-        cudaLaunchKernelEx(&cfg, fp8::fed_glm_fp8_kernel<KF, DYN, ROWS>, *comm, segs_dev, *prm, maps,                    \
-                           reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                       \
-    } while (0)
     // unbounded residuals (Poisson, Gaussian, or any weighted model): per-row-group scales for the R operand
     const bool dyn = prm->family != 0 || (prm->row_data & kGlmRowWeights);
     const bool rows = prm->row_data != 0;
-    if (prm->n_chains == 1) {
-        if (rows) {
-            if (dyn) B200FED_FP8_LAUNCH(1, true, true); else B200FED_FP8_LAUNCH(1, false, true);
-        } else {
-            if (dyn) B200FED_FP8_LAUNCH(1, true, false); else B200FED_FP8_LAUNCH(1, false, false);
-        }
-    } else {
-        if (rows) {
-            if (dyn) B200FED_FP8_LAUNCH(3, true, true); else B200FED_FP8_LAUNCH(3, false, true);
-        } else {
-            if (dyn) B200FED_FP8_LAUNCH(3, true, false); else B200FED_FP8_LAUNCH(3, false, false);
-        }
-    }
-#undef B200FED_FP8_LAUNCH
-    return (int)cudaGetLastError();
+    using fp8::fed_glm_fp8_kernel;
+    const auto kernel = prm->n_chains == 1
+        ? (rows ? (dyn ? fed_glm_fp8_kernel<1, true, true> : fed_glm_fp8_kernel<1, false, true>)
+                : (dyn ? fed_glm_fp8_kernel<1, true, false> : fed_glm_fp8_kernel<1, false, false>))
+        : (rows ? (dyn ? fed_glm_fp8_kernel<3, true, true> : fed_glm_fp8_kernel<3, false, true>)
+                : (dyn ? fed_glm_fp8_kernel<3, true, false> : fed_glm_fp8_kernel<3, false, false>));
+    return tc::launch_pdl(kernel, grid, fp8::kThreadsF, L.total, stream, *comm, segs_dev, *prm,
+                          reinterpret_cast<const CUtensorMap*>(tmaps), reinterpret_cast<const GlmChunk*>(chunks_dev),
+                          n_chunks, work_counter);
 }

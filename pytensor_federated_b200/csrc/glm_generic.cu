@@ -8,6 +8,7 @@
 // fallback explicit, not silent"); arbitrary Python compute functions use the gRPC / local-node path.
 #include <cuda_bf16.h>
 #include "fed_comm.cuh"
+#include "glm_link.cuh"
 #include "models.h"
 #ifdef B200FED_SNIPPET_HEADER
 #include B200FED_SNIPPET_HEADER   // defines B200FED_CUSTOM_LINK (models/custom.py, build.py)
@@ -29,22 +30,7 @@ __device__ __forceinline__ void link_loglik_g(int family, float y, float eta, fl
 }
 #else
 __device__ __forceinline__ void link_loglik_g(int family, float y, float eta, float& ll, float& r) {
-    if (family == 0) {
-        const float e = __expf(-fabsf(eta));
-        const float sp = fmaxf(eta, 0.f) + __logf(1.f + e);
-        const float inv = __fdividef(1.f, 1.f + e);
-        const float p = eta >= 0.f ? inv : e * inv;
-        ll = y * eta - sp;
-        r = y - p;
-    } else if (family == 1) {
-        const float mu = __expf(eta);
-        ll = y * eta - mu;
-        r = y - mu;
-    } else {
-        const float d = y - eta;
-        ll = -0.5f * d * d - 0.918938533204672742f;
-        r = d;
-    }
+    link_loglik(family, y, eta, ll, r);
 }
 #endif
 #ifndef B200FED_GENERIC_ENTRY
@@ -141,8 +127,8 @@ fed_glm_generic_kernel(FedComm comm, const GlmSegment* __restrict__ segs, GlmPar
                 link_loglik_g(prm.family, __ldg(seg.y + row), eta, ll, r);
                 if (seg.weight) {
                     const float wt = __ldg(seg.weight + row);
-                    ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                    r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                    apply_weight(wt, ll);
+                    apply_weight(wt, r);
                 }
 #pragma unroll
                 for (int j = 0; j < J; ++j) g[j] = fmaf(r, x[j], g[j]);

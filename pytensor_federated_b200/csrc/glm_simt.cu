@@ -15,6 +15,7 @@
 // BASELINE.json ("federated logistic GLM, 10M rows x 256 features per shard").
 #include <cuda_bf16.h>
 #include "fed_comm.cuh"
+#include "glm_link.cuh"
 #include "models.h"
 
 namespace {
@@ -36,25 +37,6 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
-}
-
-__device__ __forceinline__ void link_loglik(int family, float y, float eta, float& ll, float& r) {
-    if (family == 0) {  // Bernoulli / logit
-        const float e = __expf(-fabsf(eta));
-        const float sp = fmaxf(eta, 0.f) + __logf(1.f + e);       // softplus(eta)
-        const float inv = __fdividef(1.f, 1.f + e);
-        const float p = eta >= 0.f ? inv : e * inv;               // sigmoid(eta)
-        ll = y * eta - sp;
-        r = y - p;
-    } else if (family == 1) {  // Poisson / log (constant -lgamma(y+1) omitted)
-        const float mu = __expf(eta);
-        ll = y * eta - mu;
-        r = y - mu;
-    } else {  // Gaussian / identity, unit variance
-        const float d = y - eta;
-        ll = -0.5f * d * d - 0.918938533204672742f;
-        r = d;
-    }
 }
 
 template <int NCH>
@@ -198,8 +180,8 @@ fed_glm_simt_kernel(FedComm comm, const GlmSegment* __restrict__ segs, GlmParams
                 link_loglik(prm.family, y, eta, ll, r);
                 if (seg.weight) {
                     const float wt = __ldg(seg.weight + myrow);
-                    ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                    r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                    apply_weight(wt, ll);
+                    apply_weight(wt, r);
                 }
             }
             ll_acc += ll;

@@ -91,31 +91,60 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
     return 1 + (rows && (row_data & kGlmRowOffsets) ? 1 : 0) + (rows && (row_data & kGlmRowWeights) ? 1 : 0);
 }
 
-// KC = chains per launch; ROWS = some segment has per-row offsets or weights (GlmSegment::offset / weight), so
-// models without them run an instantiation with no trace of the extra loads; SOFTMAX = the multinomial family
-// (code 3), whose C classes ride along N as "virtual chains": column v = k C + c is class c of chain k, and the
-// columns of one row are coupled only through the log-sum-exp of the epilogue (tc::softmax_loglik); DISP = a family
-// with a learned dispersion parameter (codes 4 and 5, tc::gaussian_scale_loglik / tc::negbin_loglik): theta rows
-// have stride G + P + 1, the intercept table is followed by kDispWords per-chain constants, the epilogue produces a
-// third per-row value q = dll/dlog_dispersion next to ll and r, and each chain's output block is
-// [LL, gi[G], g[P], dlog_dispersion]; ORD = the ordinal (cumulative-logit) family (code 6), whose C - 1 cutpoints
-// ride along N like the multinomial classes: column v = k (C - 1) + j is cutpoint j of chain k, its intercept table
-// row holds intercept - c_j (packed by the host), so MMA #1 gives z_j = eta - c_j, and the columns of one row are
-// coupled only through tc::ordinal_loglik; SURV (with DISP) = the right-censored survival families (codes 7 and 8,
-// tc::weibull_loglik / tc::lognormal_loglik), which share DISP's layout and take each row's event from the sign of
-// its y (+t event, -t censored; log |y| is computed once per row); HVP = Hessian-vector products of families 0 to 2
-// (GlmParams::family carries kGlmHvp, masked off for the family branch): pair p runs as column 2p (theta_p, the scalar
-// epilogue unchanged) and column 2p + 1 (a direction v_p: the host packs theta row 2p + 1 = (v_intercept, v_beta),
-// so the intercept table's odd rows are v_intercept), whose epilogue writes ll = 0 and r = w h(eta_2p) u with u its
-// own eta without the offset; its output block is then [0, (H v)_intercept[G], (H v)_beta[P]].  Both columns of a pair
-// sit in one thread (e = 0 and e = 1).  Column layouts follow the wgmma accumulator fragment (thread lane owns columns
-// 8j + 2 (lane % 4) + {0, 1}), so that one thread holds every term of the chains it works on.
-template <int KC>
+// The kernel's template parameters: KC = columns per launch (the K bucket 1, 4, 8 or 16); ROWS = some segment has
+// per-row offsets or weights (GlmSegment::offset / weight), so models without them run an instantiation with no trace
+// of the extra loads; E = the epilogue, which turns a row's eta into its ll and r (epilogue() maps each family code):
+//   Scalar      families 0 to 2 (link_loglik), one column per chain.
+//   Softmax     the multinomial family: its C classes ride along N as "virtual chains", column v = k C + c is class c
+//               of chain k, and the columns of one row are coupled only through the log-sum-exp of
+//               tc::softmax_loglik.  At least two columns, so no KC = 1 instance.
+//   Dispersion  a learned dispersion parameter (tc::gaussian_scale_loglik / tc::negbin_loglik): theta rows have stride
+//               G + P + 1, the intercept table is followed by kDispWords per-chain constants, the epilogue produces a
+//               third per-row value q = dll/dlog_dispersion next to ll and r, and each chain's output block is
+//               [LL, gi[G], g[P], dlog_dispersion].
+//   Ordinal     the cumulative-logit family: its C - 1 cutpoints ride along N like the multinomial classes, column
+//               v = k (C - 1) + j is cutpoint j of chain k, its intercept table row holds intercept - c_j (packed by
+//               the host), so MMA #1 gives z_j = eta - c_j, and the columns of one row are coupled only through
+//               tc::ordinal_loglik.
+//   Survival    the right-censored survival families (tc::weibull_loglik / tc::lognormal_loglik): Dispersion's layout,
+//               each row's event taken from the sign of its y (+t event, -t censored; log |y| computed once per row).
+//   Hvp         Hessian-vector products of families 0 to 2 (GlmParams::family carries kGlmHvp, masked off for the
+//               family branch): pair p runs as column 2p (theta_p, the Scalar epilogue unchanged) and column 2p + 1 (a
+//               direction v_p: the host packs theta row 2p + 1 = (v_intercept, v_beta), so the intercept table's odd
+//               rows are v_intercept), whose epilogue writes ll = 0 and r = w h(eta_2p) u with u its own eta without
+//               the offset; its output block is then [0, (H v)_intercept[G], (H v)_beta[P]].  Both columns of a pair
+//               sit in one thread (e = 0 and e = 1).  No KC = 1 instance.
+// Column layouts follow the wgmma accumulator fragment (thread lane owns columns 8j + 2 (lane % 4) + {0, 1}), so
+// that one thread holds every term of the chains it works on.
+enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp };
+
+__host__ __device__ constexpr bool has_dispersion(Epi e) { return e == Epi::Dispersion || e == Epi::Survival; }
+
+constexpr Epi epilogue(int family) {
+    if (family & kGlmHvp) return Epi::Hvp;
+    switch (family) {
+        case kGlmMultinomial: return Epi::Softmax;
+        case kGlmGaussianScale: case kGlmNegBinomial: return Epi::Dispersion;
+        case kGlmOrdinal: return Epi::Ordinal;
+        case kGlmWeibull: case kGlmLogNormal: return Epi::Survival;
+        default: return Epi::Scalar;
+    }
+}
+static_assert([] {
+    for (int code = 0; code <= kGlmLogNormal; ++code)
+        if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
+    return true;
+}(), "the epilogue's theta and output layout must match the family's");
+
+// Column layout of the K bucket kc
 struct Cfg {
-    static constexpr int C8 = KC <= 8 ? 8 : 16;           // chain columns per theta term
-    static constexpr int N1 = 3 * C8;                     // eta: term t of chain k in column t * C8 + k
-    static constexpr int N2 = ((2 * KC + 7) / 8) * 8;     // residual: (hi, lo) of chain k in columns 2k, 2k + 1
+    int C8;   // chain columns per theta term
+    int N1;   // eta: term t of chain k in column t * C8 + k
+    int N2;   // residual: (hi, lo) of chain k in columns 2k, 2k + 1
 };
+__host__ __device__ constexpr Cfg cfg(int kc) {
+    return {kc <= 8 ? 8 : 16, 3 * (kc <= 8 ? 8 : 16), ((2 * kc + 7) / 8) * 8};
+}
 
 // doubles per CTA row of the partial array: (hi, lo) pairs of the n_vals outputs, then the per-warp slots of
 // the values that a whole warp contributes to — [kLLRows][n_out][KC][1 + G + disp]: log-likelihood, the G
@@ -136,13 +165,15 @@ __host__ __device__ constexpr size_t partial_row_doubles(int n_vals, int kc, int
 // a statically assigned straggler.  Everything a chunk contributes (fp32 register accumulation over its tiles,
 // per-thread fp32 sums) depends on the chunk alone, and chunk results are combined as double-double pairs
 // (fed::dd_add), so the evaluation stays reproducible although the assignment is not.
-template <int KC, bool ROWS, bool SOFTMAX, bool DISP, bool ORD, bool SURV, bool HVP>
+template <int KC, bool ROWS, Epi E>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
-    constexpr int C8 = Cfg<KC>::C8;
-    constexpr int N1 = Cfg<KC>::N1;
-    constexpr int N2 = Cfg<KC>::N2;
+    constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
+                   SURV = E == Epi::Survival, HVP = E == Epi::Hvp;
+    constexpr int C8 = cfg(KC).C8;
+    constexpr int N1 = cfg(KC).N1;
+    constexpr int N2 = cfg(KC).N2;
     extern __shared__ unsigned char smem_dyn[];
     // 1 KB alignment (128B-swizzled TMA tiles) by offsetting INSIDE the shared array: the pointer keeps its
     // shared address space, so the compiler emits LDS / STS instead of generic LD / ST for everything below
@@ -504,25 +535,25 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                             else negbin_loglik(y, et, dt, ll, r, dq);
                                         }
                                         if constexpr (ROWS) {
-                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
-                                            dq = wt == 0.f ? 0.f : __fmul_rn(wt, dq);
+                                            apply_weight(wt, ll);
+                                            apply_weight(wt, r);
+                                            apply_weight(wt, dq);
                                         }
                                     } else if constexpr (ORD) {
                                         // offset already in z; weight as in ROWS
                                         ll = od_ll[2 * jc + e];
                                         r = od_r[2 * jc + e];
                                         if constexpr (ROWS) {
-                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                            apply_weight(wt, ll);
+                                            apply_weight(wt, r);
                                         }
                                     } else if constexpr (SOFTMAX) {
                                         // weight as in ROWS (offsets are rejected for this family)
                                         ll = sm_ll[2 * jc + e];
                                         r = sm_r[2 * jc + e];
                                         if constexpr (ROWS) {
-                                            ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                                            r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                            apply_weight(wt, ll);
+                                            apply_weight(wt, r);
                                         }
                                     } else if constexpr (HVP) {
                                         // column 2p (e = 0): theta_p, exactly as the scalar families below, plus h at
@@ -536,20 +567,20 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                             link_loglik(fam, y, et, ll, r);
                                             hv_h = link_curvature(fam, et);
                                             if constexpr (ROWS) {
-                                                ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                                                r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                                apply_weight(wt, ll);
+                                                apply_weight(wt, r);
                                             }
                                         } else {
                                             r = __fmul_rn(hv_h, eta + icpt[k]);
-                                            if constexpr (ROWS) r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                            if constexpr (ROWS) apply_weight(wt, r);
                                         }
                                     } else if constexpr (ROWS) {
                                         // offset after the intercept, weight after the likelihood, both rounded on their
                                         // own (no FMA contraction): w = 1, o = 0 gives the bits of the plain model; a
                                         // zero weight selects 0, so a masked row's non-finite y or o never reaches a sum
                                         link_loglik(prm.family, y, __fadd_rn(eta + icpt[k], o), ll, r);
-                                        ll = wt == 0.f ? 0.f : __fmul_rn(wt, ll);
-                                        r = wt == 0.f ? 0.f : __fmul_rn(wt, r);
+                                        apply_weight(wt, ll);
+                                        apply_weight(wt, r);
                                     } else {
                                         link_loglik(prm.family, y, eta + icpt[k], ll, r);
                                     }
@@ -661,21 +692,52 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 
 // ------------------------------------------------------------------ host side
 namespace {
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
 int chains_bucket(int k) { return k <= 1 ? 1 : (k <= 4 ? 4 : (k <= 8 ? 8 : (k <= 16 ? 16 : 0))); }
+
+// The shared-memory layout of a launch in bucket kc with epilogue e (the kernel derives the same one)
+tc::SmemLayout launch_layout(int n_features, int kc, tc::Epi e, int n_theta, bool rows, int row_data) {
+    return tc::smem_layout((n_features + 127) & ~127, tc::cfg(kc).N1, tc::cfg(kc).N2, n_theta,
+                           tc::has_dispersion(e) ? tc::kDispWords : 0, kc, tc::row_arrays(rows, row_data));
+}
+
+using LaunchFn = int (*)(const FedComm*, const GlmSegment*, const GlmParams*, const void*, const void*, int, unsigned int*,
+                         int, cudaStream_t);
+
+template <int KC, bool ROWS, tc::Epi E>
+int launch(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps, const void* chunks_dev,
+           int n_chunks, unsigned int* work_counter, int grid, cudaStream_t stream) {
+    const tc::SmemLayout L = launch_layout(prm->n_features, KC, E, comm->n_theta, ROWS, prm->row_data);
+    if (L.stages < 2) return -2;
+    return tc::launch_pdl(tc::fed_glm_tc_kernel<KC, ROWS, E>, grid, tc::kThreads, L.total, stream, *comm, segs_dev, *prm,
+                          reinterpret_cast<const CUtensorMap*>(tmaps), reinterpret_cast<const GlmChunk*>(chunks_dev),
+                          n_chunks, work_counter);
+}
+
+// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax and Hvp (two columns at least) in
+// KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are instantiated, which is the order
+// of the cases here.
+template <tc::Epi E>
+LaunchFn pick(int kc, bool rows) {
+    switch (kc) {
+        case 1:
+            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp) return nullptr;
+            else return rows ? launch<1, true, E> : launch<1, false, E>;
+        case 4: return rows ? launch<4, true, E> : launch<4, false, E>;
+        case 8: return rows ? launch<8, true, E> : launch<8, false, E>;
+        default: return rows ? launch<16, true, E> : launch<16, false, E>;
+    }
+}
+LaunchFn pick(tc::Epi e, int kc, bool rows) {
+    using tc::Epi;
+    switch (e) {
+        case Epi::Hvp: return pick<Epi::Hvp>(kc, rows);
+        case Epi::Softmax: return pick<Epi::Softmax>(kc, rows);
+        case Epi::Ordinal: return pick<Epi::Ordinal>(kc, rows);
+        case Epi::Survival: return pick<Epi::Survival>(kc, rows);
+        case Epi::Dispersion: return pick<Epi::Dispersion>(kc, rows);
+        default: return pick<Epi::Scalar>(kc, rows);
+    }
+}
 }  // namespace
 
 // Builds the TMA descriptors of every segment, [n_segments][4]: X ([n_rows, P] bf16, box = 64 features x 128 rows,
@@ -686,7 +748,7 @@ extern "C" int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, 
     if (prm->n_features % 8 != 0 || prm->n_features > 384 || prm->n_features < 8) return -11;   // padded to 128s by TMA
     if (chains_bucket(prm->n_chains) == 0) return -13;
     if ((prm->ld * 2) % 16 != 0) return -14;
-    EncodeTiledFn encode = get_encode();
+    const PFN_cuTensorMapEncodeTiled encode = tc::encode_tiled();
     if (!encode) return -15;
     for (int s = 0; s < n_segments; ++s) {
         const GlmSegment& g = segs_host[s];
@@ -744,9 +806,9 @@ extern "C" int b200_glm_tc_chunk_table(const long long* n_rows, int n_segments, 
 }
 
 // doubles in the partial array of the tensor-core kernel: one row of (hi, lo) pairs + per-warp LL slots per CTA
-// (dispersion = 1: families 4, 5, 7 and 8, whose slots also hold dlog_dispersion)
-extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int dispersion) {
-    return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups, dispersion ? 1 : 0);
+extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int family) {
+    return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups,
+                                   tc::has_dispersion(tc::epilogue(family)) ? 1 : 0);
 }
 
 // Stages of the TMA ring the launch of this shape gets (host only; tests/test_glm_row_stream.py).  The launch
@@ -754,10 +816,7 @@ extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int 
 extern "C" int b200_glm_tc_stages(int n_features, int n_chains, int n_groups, int family, int row_data) {
     const int kc = chains_bucket(n_chains);
     if (kc == 0) return 0;
-    const int n1 = kc <= 8 ? 24 : 48, n2 = ((2 * kc + 7) / 8) * 8;   // Cfg<kc>
-    const bool disp = family == 4 || family == 5 || family == 7 || family == 8;
-    return (int)tc::smem_layout((n_features + 127) & ~127, n1, n2, 0, disp ? tc::kDispWords : 0, kc,
-                                tc::row_arrays(row_data != 0, row_data)).stages;
+    return (int)launch_layout(n_features, kc, tc::epilogue(family), 0, row_data != 0, row_data).stages;
 }
 
 extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps,
@@ -765,64 +824,8 @@ extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_de
                                   cudaStream_t stream) {
     const int kc = chains_bucket(prm->n_chains);
     if (kc == 0) return -1;
-    const CUtensorMap* maps = reinterpret_cast<const CUtensorMap*>(tmaps);
-#define LAUNCH_TC(KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP)                                                                    \
-    do {                                                                                                           \
-        const tc::SmemLayout L = tc::smem_layout((prm->n_features + 127) & ~127, tc::Cfg<KC>::N1, tc::Cfg<KC>::N2, comm->n_theta,  \
-                                                 DISP ? tc::kDispWords : 0, KC, tc::row_arrays(ROWS, prm->row_data)); \
-        if (L.stages < 2) return -2;                                                                               \
-        cudaFuncSetAttribute(tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total); \
-        cudaLaunchConfig_t cfg{};                                                                                  \
-        cfg.gridDim = dim3(grid);                                                                                  \
-        cfg.blockDim = dim3(tc::kThreads);                                                                         \
-        cfg.dynamicSmemBytes = L.total;                                                                            \
-        cfg.stream = stream;                                                                                       \
-        cudaLaunchAttribute attr[1];                                                                               \
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                           \
-        attr[0].val.programmaticStreamSerializationAllowed = 1;                                                    \
-        cfg.attrs = attr;                                                                                          \
-        cfg.numAttrs = tc::use_pdl() ? 1 : 0;                                                                      \
-        cudaLaunchKernelEx(&cfg, tc::fed_glm_tc_kernel<KC, ROWS, SOFTMAX, DISP, ORD, SURV, HVP>, *comm, segs_dev, *prm, maps,       \
-                           reinterpret_cast<const GlmChunk*>(chunks_dev), n_chunks, work_counter);                 \
-    } while (0)
     const bool rows = prm->row_data != 0;   // per-row offsets / weights somewhere: the instantiation that reads them
-    if (prm->family & kGlmHvp) {            // Hessian-vector products: K (theta, v) pairs as columns 2k, 2k + 1
-        if (kc == 1 || prm->n_chains % 2 != 0 || (prm->family & ~kGlmHvp) > 2) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false, true); else LAUNCH_TC(4, false, false, false, false, false, true); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false, true); else LAUNCH_TC(8, false, false, false, false, false, true); }
-        else { if (rows) LAUNCH_TC(16, true, false, false, false, false, true); else LAUNCH_TC(16, false, false, false, false, false, true); }
-    }
-    else if (prm->family == 3) {                // multinomial: K C >= 2 virtual chains, so never the KC = 1 bucket
-        if (kc == 1 || prm->n_classes < 2 || prm->n_chains % prm->n_classes != 0) return -3;
-        if (kc == 4) { if (rows) LAUNCH_TC(4, true, true, false, false, false, false); else LAUNCH_TC(4, false, true, false, false, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, true, false, false, false, false); else LAUNCH_TC(8, false, true, false, false, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, true, false, false, false, false); else LAUNCH_TC(16, false, true, false, false, false, false); }
-    }
-    else if (prm->family == 6) {            // ordinal: K (C - 1) cutpoint columns; C = 2, K = 1 runs the KC = 1 bucket
-        if (prm->n_classes < 2 || prm->n_chains % (prm->n_classes - 1) != 0) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, true, false, false); else LAUNCH_TC(1, false, false, false, true, false, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, true, false, false); else LAUNCH_TC(4, false, false, false, true, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, true, false, false); else LAUNCH_TC(8, false, false, false, true, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, false, true, false, false); else LAUNCH_TC(16, false, false, false, true, false, false); }
-    }
-    else if (prm->family == 7 || prm->family == 8) {   // right-censored survival: the dispersion layout, SURV epilogue
-        if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, true, false); else LAUNCH_TC(1, false, false, true, false, true, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, true, false); else LAUNCH_TC(4, false, false, true, false, true, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, true, false); else LAUNCH_TC(8, false, false, true, false, true, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, true, false, true, false); else LAUNCH_TC(16, false, false, true, false, true, false); }
-    }
-    else if (prm->family == 4 || prm->family == 5) {   // learned dispersion: theta rows [G + P + 1]
-        if (prm->n_classes != 1) return -3;
-        if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, true, false, false, false); else LAUNCH_TC(1, false, false, true, false, false, false); }
-        else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, true, false, false, false); else LAUNCH_TC(4, false, false, true, false, false, false); }
-        else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, true, false, false, false); else LAUNCH_TC(8, false, false, true, false, false, false); }
-        else { if (rows) LAUNCH_TC(16, true, false, true, false, false, false); else LAUNCH_TC(16, false, false, true, false, false, false); }
-    }
-    else if (kc == 1) { if (rows) LAUNCH_TC(1, true, false, false, false, false, false); else LAUNCH_TC(1, false, false, false, false, false, false); }
-    else if (kc == 4) { if (rows) LAUNCH_TC(4, true, false, false, false, false, false); else LAUNCH_TC(4, false, false, false, false, false, false); }
-    else if (kc == 8) { if (rows) LAUNCH_TC(8, true, false, false, false, false, false); else LAUNCH_TC(8, false, false, false, false, false, false); }
-    else { if (rows) LAUNCH_TC(16, true, false, false, false, false, false); else LAUNCH_TC(16, false, false, false, false, false, false); }
-#undef LAUNCH_TC
-    return (int)cudaGetLastError();
+    const LaunchFn fn = pick(tc::epilogue(prm->family), kc, rows);
+    if (!fn) return -3;
+    return fn(comm, segs_dev, prm, tmaps, chunks_dev, n_chunks, work_counter, grid, stream);
 }

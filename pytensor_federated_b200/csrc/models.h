@@ -30,23 +30,13 @@ struct GlmParams {
     int ld;               // row stride of X in elements
     int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8: [.., log_dispersion])
     int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8: [K][G+P+1])
-    int family;           // 0 = logistic (Bernoulli), 1 = Poisson (log link), 2 = Gaussian (identity, unit variance),
-                          // 3 = multinomial (softmax over n_classes columns; tensor-core bf16 kernel only),
-                          // 4 = Gaussian with unknown scale (log_dispersion = log sigma), 5 = negative binomial (NB2,
-                          // log link, log_dispersion = log alpha); 4 and 5: tensor-core bf16 kernel only, output
-                          // block per chain [LL, gi[G], g[P], dLL/dlog_dispersion], 6 = ordinal (cumulative logit,
-                          // n_classes = C categories, C - 1 cutpoint columns per chain; tensor-core bf16 kernel only),
-                          // 7 = Weibull, 8 = log-normal right-censored survival (AFT, log_dispersion = log sigma;
-                          // y = +t for an event, -t for a censored row; the layout and kernel of 4 and 5);
-                          // kGlmHvp | (0, 1 or 2): Hessian-vector products of that family (tensor-core bf16 kernel only)
+    int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
     int early_loads;      // tensor-core kernels: claim + load the first tiles before theta arrives (B200FED_NO_EARLY_LOADS=1: off)
     int row_data;         // kGlmRowOffsets | kGlmRowWeights when any segment has them: selects the kernel instantiation
-    int n_classes;        // multinomial: C classes per chain, n_chains = K C "virtual chains" (column k C + c is class
-                          // c of chain k; theta row k C + c = (intercept[:, c], beta[:, c]) of chain k); ordinal: C
-                          // categories, n_chains = K (C - 1) (column k (C - 1) + j is cutpoint j of chain k; theta row
-                          // k (C - 1) + j = (intercept - c_j, beta) of chain k); else 1
+    int n_classes;        // C: multinomial classes or ordinal categories (GlmFamily::columns), else 1.  Theta row v holds
+                          // column v: (intercept[:, c], beta[:, c]) of class c, (intercept - c_j, beta) of cutpoint j
 };
 
 constexpr int kGlmRowOffsets = 1;
@@ -56,6 +46,44 @@ constexpr int kGlmRowWeights = 2;
 // theta_k.  Only the bf16 tensor-core kernel takes it (families 0 to 2, an even n_chains); the runtime refuses it
 // for every other kernel.
 constexpr int kGlmHvp = 16;
+
+// GlmParams::family (models/glm.py FAMILIES holds the same codes)
+enum GlmFamilyCode : int {
+    kGlmLogistic = 0,        // Bernoulli, logit link
+    kGlmPoisson = 1,         // log link
+    kGlmGaussian = 2,        // identity link, unit variance
+    kGlmMultinomial = 3,     // softmax over n_classes columns
+    kGlmGaussianScale = 4,   // Gaussian with unknown scale, log_dispersion = log sigma
+    kGlmNegBinomial = 5,     // NB2, log link, log_dispersion = log alpha
+    kGlmOrdinal = 6,         // cumulative logit over n_classes categories, one column per cutpoint
+    kGlmWeibull = 7,         // right-censored survival (AFT), log_dispersion = log sigma,
+    kGlmLogNormal = 8,       //   y = +t for an event, -t for a censored row
+};
+
+// How a family's columns make up n_chains: one per chain, one per chain and class (column k C + c is class c of chain
+// k), or one per chain and cutpoint (column k (C - 1) + j is cutpoint j of chain k), for C = n_classes
+enum class GlmColumns { kOne, kPerClass, kPerCutpoint };
+
+// What the runtime and the bf16 tensor-core kernel need to know about a family code.
+struct GlmFamily {
+    const char* name;        // as in models/glm.py
+    bool tc_only;            // runs on the bf16 tensor-core kernel only
+    bool dispersion;         // theta rows and output blocks end in a log_dispersion word: [LL, gi[G], g[P], dLL/dlog_dispersion]
+    GlmColumns columns;
+    int min_classes, max_classes;
+    bool offsets;            // takes per-row offsets
+};
+constexpr GlmFamily glm_family(int code) {
+    switch (code) {
+        case kGlmMultinomial: return {"multinomial", true, false, GlmColumns::kPerClass, 2, 16, false};
+        case kGlmGaussianScale: return {"gaussian_scale", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmNegBinomial: return {"negative_binomial", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmOrdinal: return {"ordinal", true, false, GlmColumns::kPerCutpoint, 2, 17, true};
+        case kGlmWeibull: return {"weibull", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmLogNormal: return {"lognormal", true, true, GlmColumns::kOne, 1, 1, true};
+        default: return {"", false, false, GlmColumns::kOne, 1, 1, true};   // 0 to 2: every GLM kernel
+    }
+}
 
 // Unit of work of the dynamically scheduled tensor-core GLM kernel: n_tiles consecutive 128-row tiles of one
 // segment starting at tile first_tile (n_tiles is even; the last one may lie past the segment's rows).

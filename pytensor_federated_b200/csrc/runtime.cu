@@ -44,7 +44,7 @@ int b200_launch_glm_tc(const FedComm*, const GlmSegment*, const GlmParams*, cons
                        int n_chunks, unsigned int* work_counter, int grid, cudaStream_t);
 int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count, void** tmaps_dev,
                         void** chunks_dev, int* n_chunks);
-size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int dispersion);
+size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int family);
 int b200_launch_ode(const FedComm*, const OdeShard*, int, int, cudaStream_t);
 int b200_launch_glm_fp8(const FedComm*, const GlmSegment*, const GlmParams*, const void* tmaps, const void* chunks,
                         int n_chunks, unsigned int* work_counter, int grid, cudaStream_t stream);
@@ -226,25 +226,19 @@ int launch_model(Engine* e, const FedComm* c) {
         case MODEL_GLM_SIMT:
             rc = b200_launch_glm_simt(c, e->glm_segs_dev, &e->glm, e->grid, e->stream);
             break;
-        case MODEL_GLM_TC: {
-            FedComm ct = *c;   // double-double rows + group partials of the dynamically scheduled kernel
+        case MODEL_GLM_TC:
+        case MODEL_GLM_FP8: {
+            FedComm ct = *c;   // double-double rows + group partials of the dynamically scheduled tensor-core kernels
             ct.cta_partials = e->tc_partials;
             ct.group_partials = e->tc_partials + (size_t)e->sm_count * e->tc_row_doubles;
-            rc = b200_launch_glm_tc(&ct, e->glm_segs_dev, &e->glm, e->glm_tmaps_dev, e->glm_chunks_dev, e->glm_n_chunks,
-                                    e->work_counter, e->grid, e->stream);
+            rc = (e->kind == MODEL_GLM_TC ? b200_launch_glm_tc : b200_launch_glm_fp8)(
+                &ct, e->glm_segs_dev, &e->glm, e->glm_tmaps_dev, e->glm_chunks_dev, e->glm_n_chunks, e->work_counter,
+                e->grid, e->stream);
             break;
         }
         case MODEL_ODE:
             rc = (e->ode_launcher ? e->ode_launcher : b200_launch_ode)(c, e->ode_dev, (int)e->ode.size(), e->grid, e->stream);
             break;
-        case MODEL_GLM_FP8: {
-            FedComm ct = *c;   // same partial layout as the bf16 tensor-core kernel
-            ct.cta_partials = e->tc_partials;
-            ct.group_partials = e->tc_partials + (size_t)e->sm_count * e->tc_row_doubles;
-            rc = b200_launch_glm_fp8(&ct, e->glm_segs_dev, &e->glm, e->glm_tmaps_dev, e->glm_chunks_dev, e->glm_n_chunks,
-                                     e->work_counter, e->grid, e->stream);
-            break;
-        }
         case MODEL_GLM_GENERIC:
             rc = (e->custom_launcher ? e->custom_launcher : b200_launch_glm_generic)(c, e->glm_segs_dev, &e->glm,
                                                                                       e->glm_elem_bytes, e->grid, e->stream);
@@ -559,6 +553,9 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
                         const float** offsets, const float** weights, int n_classes) {
     Engine* e = static_cast<Engine*>(h);
     CK(cudaSetDevice(e->device));
+    // The family's checks come before any engine state changes, so a refused call leaves the engine's model as it was.
+    const int n_blocks = n_out > 0 ? n_out : 1;
+    const GlmFamily f = glm_family(family);   // a kGlmHvp code: the description of families 0 to 2
     // Hessian-vector products (kGlmHvp on family 0, 1 or 2): K (theta, v) pairs as columns 2k and 2k + 1 of a 2K-chain
     // launch of the bf16 tensor-core kernel; every other kernel would read the flagged code as an unknown family
     if (family & kGlmHvp) {
@@ -579,59 +576,39 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
             g_last_error = "Hessian-vector products need an even n_chains in [2, 16] (one theta and one direction column per pair)";
             return -36;
         }
-    } else if (family == 3) {
-        if (use_tensor_cores != 1) {
-            g_last_error = "the multinomial family runs on the bf16 tensor-core kernel only";
-            return -34;
+    } else {
+        if (f.tc_only && use_tensor_cores != 1) {
+            g_last_error = std::string("the ") + f.name + " family runs on the bf16 tensor-core kernel only";
+            return f.dispersion ? -39 : -34;
         }
-        if (n_classes < 2 || n_classes > 16) {
-            g_last_error = "the multinomial family needs 2 <= n_classes <= 16";
+        if (n_classes < f.min_classes || n_classes > f.max_classes) {
+            if (f.max_classes == 1) {
+                g_last_error = "n_classes must be 1 for every family but the multinomial and ordinal ones";
+                return -38;
+            }
+            g_last_error = std::string("the ") + f.name + " family needs " + std::to_string(f.min_classes) +
+                           " <= n_classes <= " + std::to_string(f.max_classes);
             return -35;
         }
-        if (n_chains % n_classes != 0) {
-            g_last_error = "the multinomial family needs n_chains = K x n_classes (one column per chain and class)";
+        if (f.columns == GlmColumns::kPerClass && n_chains % n_classes != 0) {
+            g_last_error = std::string("the ") + f.name +
+                           " family needs n_chains = K x n_classes (one column per chain and class)";
             return -36;
         }
-        for (int s = 0; s < n_segments && offsets; ++s)
+        if (f.columns == GlmColumns::kPerCutpoint && n_chains % (n_classes - 1) != 0) {
+            g_last_error = std::string("the ") + f.name +
+                           " family needs n_chains = K x (n_classes - 1) (one column per chain and cutpoint)";
+            return -36;
+        }
+        for (int s = 0; s < n_segments && offsets && !f.offsets; ++s)
             if (offsets[s]) {
-                g_last_error = "the multinomial family takes no offsets (one common to all classes cancels)";
+                g_last_error = std::string("the ") + f.name + " family takes no offsets (one common to all classes cancels)";
                 return -37;
             }
-    } else if (family == 6) {
-        // family 6 (ordinal): the C - 1 cutpoints of each chain are columns of a K (C - 1)-chain launch, so like
-        // family 3 it exists in the bf16 tensor-core kernel only; checked before any engine state changes
-        if (use_tensor_cores != 1) {
-            g_last_error = "the ordinal family runs on the bf16 tensor-core kernel only";
-            return -34;
-        }
-        if (n_classes < 2 || n_classes > 17) {
-            g_last_error = "the ordinal family needs 2 <= n_classes <= 17";
-            return -35;
-        }
-        if (n_chains % (n_classes - 1) != 0) {
-            g_last_error = "the ordinal family needs n_chains = K x (n_classes - 1) (one column per chain and cutpoint)";
-            return -36;
-        }
-        if ((long long)(n_out > 0 ? n_out : 1) * n_chains * (1 + n_groups + n_features) != e->n_vals) {
-            g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
-            return -33;
-        }
-    } else if (n_classes != 1) {
-        g_last_error = "n_classes must be 1 for every family but the multinomial and ordinal ones";
-        return -38;
     }
-    // families 4 and 5 (Gaussian with unknown scale, negative binomial) and 7 and 8 (right-censored Weibull and
-    // log-normal survival, with s = log sigma) carry a log-dispersion parameter after beta; like family 3 they exist
-    // in the bf16 tensor-core kernel only
-    const bool dispersion = family == 4 || family == 5 || family == 7 || family == 8;
-    if (dispersion && use_tensor_cores != 1) {
-        static const char* const names[] = {"gaussian_scale", "negative_binomial", "", "weibull", "lognormal"};
-        g_last_error = std::string("the ") + names[family - 4] + " family runs on the bf16 tensor-core kernel only";
-        return -39;
-    }
-    // checked before any engine state changes, so a refused call leaves the engine's model as it was
-    if (dispersion && (long long)(n_out > 0 ? n_out : 1) * n_chains * (2 + n_groups + n_features) != e->n_vals) {
-        g_last_error = "n_vals does not match n_out x n_chains x (2 + n_groups + n_features)";
+    if ((long long)n_blocks * n_chains * (1 + n_groups + n_features + (f.dispersion ? 1 : 0)) != e->n_vals) {
+        g_last_error = f.dispersion ? "n_vals does not match n_out x n_chains x (2 + n_groups + n_features)"
+                                    : "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
         return -33;
     }
     const int tile_rows = (use_tensor_cores == 1 || use_tensor_cores == 2) ? 128 : 8;
@@ -651,19 +628,15 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         g.first_tile = tiles;
         g.group = groups[s];
         g.out_group = out_groups ? out_groups[s] : 0;
-        if (g.out_group < 0 || g.out_group >= (n_out > 0 ? n_out : 1)) {
+        if (g.out_group < 0 || g.out_group >= n_blocks) {
             g_last_error = "segment output block out of range";
             return -31;
         }
         segs[s] = g;
         tiles += (n_rows[s] + tile_rows - 1) / tile_rows;
     }
-    const GlmParams glm{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_out > 0 ? n_out : 1,
+    const GlmParams glm{n_segments, n_features, ld, n_groups, n_chains, family, tiles, n_blocks,
                         early_loads_enabled() ? 1 : 0, row_data, n_classes};
-    if (!dispersion && (long long)glm.n_out * n_chains * (1 + n_groups + n_features) != e->n_vals) {
-        g_last_error = "n_vals does not match n_out x n_chains x (1 + n_groups + n_features)";
-        return -33;
-    }
     // the bf16 tensor-core kernel checks the shape and the alignment of every array it reads through TMA before
     // anything is committed, so a refused model leaves the engine evaluating the one it had
     if (use_tensor_cores == 1) {
@@ -684,28 +657,23 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         e->glm_elem_bytes = use_tensor_cores == 3 ? 2 : 4;
         e->kind = MODEL_GLM_GENERIC;
         e->grid = e->sm_count * 2;
-    } else if (use_tensor_cores == 2) {  // block-scaled fp8
-        int rc = b200_glm_fp8_prepare(e->glm_segs.data(), n_segments, &e->glm, e->sm_count, &e->glm_tmaps_dev,
-                                      &e->glm_chunks_dev, &e->glm_n_chunks);
-        if (rc != 0) {
-            g_last_error = "fp8 GLM path rejected this shape (rc=" + std::to_string(rc) + ")";
-            return rc;
+    } else if (use_tensor_cores) {   // the tensor-core kernels: block-scaled fp8 (2) or bf16 (prepared above)
+        const bool fp8 = use_tensor_cores == 2;
+        if (fp8) {
+            int rc = b200_glm_fp8_prepare(e->glm_segs.data(), n_segments, &e->glm, e->sm_count, &e->glm_tmaps_dev,
+                                          &e->glm_chunks_dev, &e->glm_n_chunks);
+            if (rc != 0) {
+                g_last_error = "fp8 GLM path rejected this shape (rc=" + std::to_string(rc) + ")";
+                return rc;
+            }
         }
-        e->tc_row_doubles = b200_glm_fp8_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups);
+        e->tc_row_doubles = fp8 ? b200_glm_fp8_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups)
+                                : b200_glm_tc_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups, family);
         if (e->tc_partials) cudaFree(e->tc_partials);
-        const size_t fp8_doubles = (size_t)e->sm_count * e->tc_row_doubles + ((size_t)e->sm_count / 16 + 2) * e->n_vals * 2;
-        CK(cudaMalloc((void**)&e->tc_partials, fp8_doubles * 8));
-        CK(cudaMemset(e->tc_partials, 0, fp8_doubles * 8));
-        e->kind = MODEL_GLM_FP8;
-        e->grid = e->sm_count;
-        if (e->glm_n_chunks > 0 && e->grid > e->glm_n_chunks) e->grid = e->glm_n_chunks;
-    } else if (use_tensor_cores) {   // prepared above
-        e->tc_row_doubles = b200_glm_tc_partial_row_doubles(e->n_vals, n_chains, e->glm.n_out, n_groups, dispersion ? 1 : 0);
-        if (e->tc_partials) cudaFree(e->tc_partials);
-        const size_t tc_doubles = (size_t)e->sm_count * e->tc_row_doubles + ((size_t)e->sm_count / 16 + 2) * e->n_vals * 2;
-        CK(cudaMalloc((void**)&e->tc_partials, tc_doubles * 8));
-        CK(cudaMemset(e->tc_partials, 0, tc_doubles * 8));
-        e->kind = MODEL_GLM_TC;
+        const size_t doubles = (size_t)e->sm_count * e->tc_row_doubles + ((size_t)e->sm_count / 16 + 2) * e->n_vals * 2;
+        CK(cudaMalloc((void**)&e->tc_partials, doubles * 8));
+        CK(cudaMemset(e->tc_partials, 0, doubles * 8));
+        e->kind = fp8 ? MODEL_GLM_FP8 : MODEL_GLM_TC;
         e->grid = e->sm_count;
         if (e->glm_n_chunks > 0 && e->grid > e->glm_n_chunks) e->grid = e->glm_n_chunks;
     } else {

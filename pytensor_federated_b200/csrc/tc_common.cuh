@@ -6,8 +6,10 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
+#include <cudaTypedefs.h>
 
 #include "fed_comm.cuh"
+#include "glm_link.cuh"
 
 namespace tc {
 
@@ -189,6 +191,39 @@ inline bool use_pdl() {
     return on;
 }
 
+// Launches `kernel` with `smem` bytes of dynamic shared memory, with programmatic stream serialization when use_pdl()
+// (the kernel's theta-independent setup then overlaps the tail of the previous evaluation).  Returns the launch's
+// cudaError_t.
+template <typename... Params, typename... Args>
+int launch_pdl(void (*kernel)(Params...), int grid, int threads, uint32_t smem, cudaStream_t stream, Args... args) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = use_pdl() ? 1 : 0;
+    cudaLaunchKernelEx(&cfg, kernel, args...);
+    return (int)cudaGetLastError();
+}
+
+// The driver's cuTensorMapEncodeTiled, or null when the driver does not have it.
+inline PFN_cuTensorMapEncodeTiled encode_tiled() {
+    static PFN_cuTensorMapEncodeTiled fn = nullptr;
+    if (!fn) {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+            q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(p);
+    }
+    return fn;
+}
+
 // Index + phase bit of an n-deep circular buffer, advanced without division (the single-thread
 // TMA / MMA issue loops are latency chains: a 64-bit `it % n`, `it / n` pair costs ~100 instructions).
 struct Ring {
@@ -207,37 +242,6 @@ __device__ __forceinline__ void dd_accumulate(double* slot, double x) {
     double2 cur = *reinterpret_cast<double2*>(slot);
     fed::dd_add(cur.x, cur.y, x, 0.0);
     *reinterpret_cast<double2*>(slot) = cur;
-}
-
-__device__ __forceinline__ void link_loglik(int family, float y, float eta, float& ll, float& r) {
-    if (family == 0) {
-        const float e = __expf(-fabsf(eta));
-        const float sp = fmaxf(eta, 0.f) + __logf(1.f + e);
-        const float inv = __fdividef(1.f, 1.f + e);
-        const float p = eta >= 0.f ? inv : e * inv;
-        ll = y * eta - sp;
-        r = y - p;
-    } else if (family == 1) {
-        const float mu = __expf(eta);
-        ll = y * eta - mu;
-        r = y - mu;
-    } else {
-        const float d = y - eta;
-        ll = -0.5f * d * d - 0.918938533204672742f;
-        r = d;
-    }
-}
-
-// h = d2ll / deta2 of families 0 to 2 at eta (the Hessian-vector product's per-row weight): logistic -mu (1 - mu) =
-// -e / (1 + e)^2 with e = exp(-|eta|), from an accurate expf so that h keeps its relative accuracy in both tails;
-// Poisson -mu, the very __expf(eta) that link_loglik's residual uses; Gaussian -1.
-__device__ __forceinline__ float link_curvature(int family, float eta) {
-    if (family == 0) {
-        const float e = expf(-fabsf(eta));
-        const float d = 1.f + e;
-        return -e / (d * d);
-    }
-    return family == 1 ? -__expf(eta) : -1.f;
 }
 
 // Multinomial (softmax) likelihood of one row, family 3.  The row's columns are spread over the four lanes of a

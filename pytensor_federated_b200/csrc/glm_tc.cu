@@ -21,6 +21,7 @@
 // The federation prologue/epilogue (theta broadcast, NVLink reduce) is fed_comm.cuh.
 //
 // Workload: BASELINE.json "federated logistic GLM, 10M rows x 256 features per shard, bf16".
+#include <cstring>
 #include <vector>
 
 #include <cuda.h>
@@ -44,15 +45,76 @@ constexpr int kMinChunk = 4;
 constexpr int kRing = 16;            // published chunks the consumers may lag behind (needs only ~3)
 constexpr int kLLRows = 16;          // per-warp log-likelihood slot rows (>= kConsumerWarps)
 
+// Packed X (GlmParams::packed_x).  A bf16 value is [sign | exponent 8 | mantissa 7]; its high byte (sign and the upper
+// 7 exponent bits) takes few values on real data, its low byte is close to random.  Each (128-row tile, 64-feature
+// panel) is one kXBlock block: the 8192 low bytes in row-major order, then 8192 4-bit codes (two per byte, the even
+// feature in the low nibble), code c < 15 standing for the high byte in entry c of the segment's table (entry 0 is
+// 0x00, which padding uses) and 15 for an exception.  A tile's kXFoot-byte footer holds the exception count and up
+// to kXMaxExceptions words (position in the tile << 8 | high byte), position = panel * 8192 + row * 64 + feature.
+// The producer (warp 0) streams the blocks into a ring of kXSlots slots with cp.async.bulk; warps 1 to 3 decode
+// each panel into the 128B-swizzled image TMA would have written, so the consumers see the same stage bytes.
+constexpr int kXBlock = kTileM * kPanel * 3 / 2;   // 12 KB
+constexpr int kXFoot = 256;
+constexpr int kXMaxExceptions = kXFoot / 4 - 1;
+constexpr int kXSlots = 6;                           // compressed panel slots at most
+constexpr int kDecThreads = 96;                      // warps 1 to 3
+
+// prmt.b32 (byte permute; selector nibble bit 3 replicates the sign of the selected byte)
+__host__ __device__ __forceinline__ uint32_t x12_prmt(uint32_t a, uint32_t b, uint32_t s) {
+#ifdef __CUDA_ARCH__
+    uint32_t r;
+    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(s));
+    return r;
+#else
+    const uint64_t v = (uint64_t)b << 32 | a;
+    uint32_t r = 0;
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t sel = (s >> (4 * k)) & 0xFu;
+        uint32_t byte = (uint32_t)(v >> (8 * (sel & 7u))) & 0xFFu;
+        if (sel & 8u) byte = (byte & 0x80u) ? 0xFFu : 0u;
+        r |= byte << (8 * k);
+    }
+    return r;
+#endif
+}
+// Eight consecutive values of a row: low bytes lo (values 0-3 in .x, 4-7 in .y), codes c (nibble k: value k), table t
+// (entry 4 q + b in byte b of t[q]) -> the 8 bf16 values as one 16-byte chunk.  Codes index entries 0-7 (t[0], t[1])
+// or 8-15 (t[2], t[3]) with their low 3 bits; the per-byte select on bit 3 comes from a sign-replicating prmt of the
+// code word's bytes (c << 4 holds bit 3 of the even nibbles in its byte MSBs, c that of the odd ones).
+__host__ __device__ __forceinline__ uint4 x12_decode8(uint2 lo, uint32_t c, const uint32_t (&t)[4]) {
+    const uint32_t w = c << 4;
+    const uint32_t s0 = c & 0x7777u, s1 = (c >> 16) & 0x7777u;
+    const uint32_t m0 = x12_prmt(w, c, 0xD9C8u), m1 = x12_prmt(w, c, 0xFBEAu);
+    const uint32_t h0 = (x12_prmt(t[0], t[1], s0) & ~m0) | (x12_prmt(t[2], t[3], s0) & m0);
+    const uint32_t h1 = (x12_prmt(t[0], t[1], s1) & ~m1) | (x12_prmt(t[2], t[3], s1) & m1);
+    uint4 r;
+    r.x = x12_prmt(lo.x, h0, 0x5140u);
+    r.y = x12_prmt(lo.x, h0, 0x7362u);
+    r.z = x12_prmt(lo.y, h1, 0x5140u);
+    r.w = x12_prmt(lo.y, h1, 0x7362u);
+    return r;
+}
+// Byte offset in the decoded (128B-swizzled) tile of chunk i = row * 8 + j of a panel
+__host__ __device__ __forceinline__ uint32_t x12_chunk_offset(int i) { return (i >> 3) * 128 + (((i & 7) ^ ((i >> 3) & 7)) << 4); }
+// Byte offset of the high byte of the value at an exception position (panel * 8192 + row * 64 + feature)
+__host__ __device__ __forceinline__ uint32_t x12_high_byte_offset(uint32_t pos) {
+    const uint32_t pnl = pos >> 13, row = (pos >> 6) & 127, f = pos & 63;
+    return pnl * kPanelBytes + row * 128 + ((((f >> 3) ^ (row & 7)) << 4) | ((f & 7) << 1)) + 1;
+}
+
 struct SmemLayout {
     uint32_t stages, stage_bytes, off_theta_b, theta_b_bytes, off_r, r_bytes, off_rows, row_bytes, off_theta_f,
-        off_disp, off_ring, off_bars, total, preload;
+        off_disp, off_ring, off_bars, total, preload, xslots, xslot_bytes, off_x, off_xfoot;
 };
 // chain_words: per-chain fp32 constants kept in shared memory next to the chunk's intercept column (kDispWords for
 // the dispersion families, else 0);
 // row_arrays: fp32 per-row arrays a tile carries (y, and the offsets / weights the launch has: 1 to 3)
+// packed: X comes packed (kXBlock blocks): two bf16 stages, then as many compressed panel slots as fit (xslots, at most
+// kXSlots; fewer than 2 means the shape cannot run packed), each a block plus the footer and row data of its tile.
+// theta (fp32) is staged in the two bf16 stages as in the unpacked layout, so a theta larger than both (many groups
+// and chains) gets no slots: such a shape reads X itself, with its 3 or 4 stages
 __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_theta, int chain_words, int chains,
-                                                  int row_arrays) {
+                                                  int row_arrays, bool packed = false) {
     SmemLayout L;
     const uint32_t panels = P / kPanel;
     L.stage_bytes = panels * kPanelBytes;
@@ -63,24 +125,38 @@ __host__ __device__ inline SmemLayout smem_layout(int P, int n1, int n2, int n_t
     L.row_bytes = (uint32_t)row_arrays * kTileM * 4;
     // theta (fp32) is staged inside the TMA stage ring and is dead once the bf16 B operand and the intercept
     // table are built, so it costs no shared memory of its own.
-    const uint32_t fixed = L.theta_b_bytes + 2 * L.r_bytes + ((chains * (1 + chain_words) * 4 + 15) & ~15) + kRing * 24 + 192 +
-                           1024 /*alignment slack*/;
+    const uint32_t bars_bytes = packed ? 256 : 192;
+    const uint32_t fixed = L.theta_b_bytes + 2 * L.r_bytes + ((chains * (1 + chain_words) * 4 + 15) & ~15) + kRing * 24 +
+                           bars_bytes + (packed ? 2 * kXFoot : 0) + 1024 /*alignment slack*/;
     uint32_t stages = (227u * 1024u - fixed) / (L.stage_bytes + L.row_bytes);
     if (stages > 4) stages = 4;
+    L.xslots = 0;
+    L.xslot_bytes = kXBlock + kXFoot + L.row_bytes;
+    if (packed) {
+        const uint32_t two = fixed + 2 * (L.stage_bytes + L.row_bytes);
+        stages = 2;
+        if (two <= 227u * 1024u && (uint32_t)n_theta * 4u <= 2u * L.stage_bytes) {
+            const uint32_t fit = (227u * 1024u - two) / L.xslot_bytes;
+            L.xslots = fit < (uint32_t)kXSlots ? fit : (uint32_t)kXSlots;
+        }
+    }
     L.stages = stages;
     uint32_t o = stages * L.stage_bytes;
     L.off_theta_b = o; o += L.theta_b_bytes;
     L.off_r = o; o += 2 * L.r_bytes;
     L.off_rows = o; o += stages * L.row_bytes;   // 512-byte multiples: 16-byte aligned like every TMA destination
+    L.off_x = o; o += L.xslots * L.xslot_bytes;   // 256-byte multiples
+    L.off_xfoot = o; o += packed ? 2 * kXFoot : 0;
     // theta (fp32) sits in the LAST stage when it fits into one: the TMA warp fills the first stages - 1 stages
     // with this CTA's first tiles BEFORE theta has arrived (`preload`), the last stage is free once the B
     // operand is built.  (larger theta: stage 0 onwards, needs n_theta * 4 <= stages * stage_bytes, no preload)
     const bool theta_in_last = (uint32_t)n_theta * 4u <= L.stage_bytes && stages >= 2;
     L.off_theta_f = theta_in_last ? (stages - 1) * L.stage_bytes : 0;
     L.preload = theta_in_last ? stages - 1 : 0;
+    if (packed) L.preload = L.xslots;   // compressed slots never hold theta: all of them may fill early (panel loads)
     L.off_disp = o; o += (chains * (1 + chain_words) * 4 + 15) & ~15;   // intercept column, then the constants
     L.off_ring = o; o += kRing * 24;   // published chunks + one mbarrier per ring slot
-    L.off_bars = o; o += 192;
+    L.off_bars = o; o += bars_bytes;
     L.total = o + 1024;
     return L;
 }
@@ -186,7 +262,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     const int panels = PP / kPanel;
     // row slot of a stage: y, then the offsets and the weights when some segment of the launch has them
     const int o_slot = 1, w_slot = ROWS && (prm.row_data & kGlmRowOffsets) ? 2 : 1;
-    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, DISP ? kDispWords : 0, KC, row_arrays(ROWS, prm.row_data));
+    const bool PK = prm.packed_x != 0;   // X packed: warp 0 loads compressed panels, warps 1 to 3 decode them
+    const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, DISP ? kDispWords : 0, KC, row_arrays(ROWS, prm.row_data), PK);
     const int S = (int)L.stages;
     const int nch = prm.n_chains < KC ? prm.n_chains : KC;  // chains actually present in theta
     const int NV1 = 1 + G + P + DISP; // outputs per chain: [LL, gi[G], g[P]] (DISP: and dlog_dispersion)
@@ -201,6 +278,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bars);
     uint64_t* bar_full = bars;            // [4] X stage landed
     uint64_t* bar_empty = bars + 4;       // [4] X stage consumed by both consumer warpgroups (bars + 128 B: chunk decision)
+    uint64_t* bar_xfull = bars + 20;      // PK: [kXSlots] compressed panel landed (bars + 144 B: the decoders' chunk decision)
+    uint64_t* bar_xempty = bars + 20 + kXSlots;   // PK: [kXSlots] compressed panel decoded
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -210,7 +289,10 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     if (threadIdx.x == 0) {
         *pipeline_fault() = 0;
         for (int i = 0; i < kRing; ++i) mbar_init(&bar_ring[i], 1);
-        for (int i = 0; i < 4; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 32 * kConsumerWarps); }
+        // PK: a stage is full once every decoder thread has arrived (its decoded stores fenced for the async proxy)
+        for (int i = 0; i < 4; ++i) { mbar_init(&bar_full[i], PK ? kDecThreads : 1); mbar_init(&bar_empty[i], 32 * kConsumerWarps); }
+        if (PK)
+            for (int i = 0; i < kXSlots; ++i) { mbar_init(&bar_xfull[i], 1); mbar_init(&bar_xempty[i], kDecThreads); }
         fence_barrier_init();
     }
     // tmaps[4 s + a]: X, y, offset, weight of segment s (the last two only where the segment has them)
@@ -234,6 +316,23 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         if (rows & 1) tma_load_1d(slot + o_slot * kTileM, m + 2, row0, &bar_full[st]);
         if (rows & 2) tma_load_1d(slot + w_slot * kTileM, m + 3, row0, &bar_full[st]);
     };
+    // PK: panel pnl of tile `tile` of segment seg into compressed slot xs, issued by one lane; with panel 0 come the
+    // tile's exception footer and row data (laid out as in a stage's row slot), all counted on xfull[xs]
+    auto load_xpanel = [&](int xs, int seg, int tile, int pnl, int rows) {
+        unsigned char* dst = smem + L.off_x + (size_t)xs * L.xslot_bytes;
+        const GlmSegment& g = segs_g[seg];
+        const uint32_t extra = pnl == 0 ? kXFoot + kTileM * 4 * (1 + (rows & 1) + (rows >> 1)) : 0;
+        mbar_expect_tx(&bar_xfull[xs], kXBlock + extra);
+        bulk_load(dst, static_cast<const unsigned char*>(g.xpack) + ((size_t)tile * panels + pnl) * kXBlock, kXBlock, &bar_xfull[xs]);
+        if (pnl == 0) {
+            const CUtensorMap* m = tmaps + 4 * seg;
+            float* slot = reinterpret_cast<float*>(dst + kXBlock + kXFoot);
+            bulk_load(dst + kXBlock, static_cast<const unsigned char*>(g.xfoot) + (size_t)tile * kXFoot, kXFoot, &bar_xfull[xs]);
+            tma_load_1d(slot, m + 1, tile * kTileM, &bar_xfull[xs]);
+            if (rows & 1) tma_load_1d(slot + o_slot * kTileM, m + 2, tile * kTileM, &bar_xfull[xs]);
+            if (rows & 2) tma_load_1d(slot + w_slot * kTileM, m + 3, tile * kTileM, &bar_xfull[xs]);
+        }
+    };
     // the row arrays of segment seg that the producer loads (bit 0: offset, bit 1: weight)
     auto seg_row_mask = [&](int seg) -> int {
         if constexpr (!ROWS) return 0;
@@ -252,11 +351,15 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         claim0 = __shfl_sync(0xffffffffu, claim0, 0);
         if (claim0 < (unsigned int)n_chunks) {
             const GlmChunk ch = chunks[claim0];
-            preloaded = ch.n_tiles < (int)L.preload ? ch.n_tiles : (int)L.preload;
+            const int units = PK ? ch.n_tiles * panels : ch.n_tiles;   // PK: compressed panels, else tiles
+            preloaded = units < (int)L.preload ? units : (int)L.preload;
             if (!prm.early_loads) preloaded = 0;
             const int rows = seg_row_mask(ch.seg);
             if (elect_one())
-                for (int t = 0; t < preloaded; ++t) load_tile(t, ch.seg, (ch.first_tile + t) * kTileM, rows);
+                for (int t = 0; t < preloaded; ++t) {
+                    if (PK) load_xpanel(t, ch.seg, ch.first_tile + t / panels, t % panels, rows);
+                    else load_tile(t, ch.seg, (ch.first_tile + t) * kTileM, rows);
+                }
             __syncwarp();
         }
     }
@@ -341,7 +444,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             // ================= TMA producer + chunk scheduler ==================================
             // The role loops are warp-uniform (all 32 lanes wait and count); only the issue is predicated on
             // elect.sync, so the compiler keeps addresses / descriptors in uniform registers.
-            Ring stage;
+            Ring stage, xs;
             unsigned int claim = claim0, ahead = 0;   // the first chunk was claimed before theta arrived
             for (int j = 0;; ++j) {
                 const bool have = claim < (unsigned int)n_chunks;
@@ -356,7 +459,18 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 __syncwarp();
                 if (!have) break;
                 const int rows = seg_row_mask(ch.seg);
-                for (int t = 0; t < ch.n_tiles; ++t) {
+                for (int t = 0; t < ch.n_tiles && PK; ++t)
+                    for (int pnl = 0; pnl < panels; ++pnl) {
+                        const int k = t * panels + pnl;
+                        if (!(j == 0 && k < preloaded)) {   // else already in flight (early loads)
+                            mbar_wait(&bar_xempty[xs.idx], xs.phase ^ 1);
+                            if (j == 0 && k == preloaded && lane == 0) fed::stamp(comm, 3);
+                            if (elect_one()) load_xpanel(xs.idx, ch.seg, ch.first_tile + t, pnl, rows);
+                            __syncwarp();
+                        }
+                        xs.advance((int)L.xslots);
+                    }
+                for (int t = 0; t < ch.n_tiles && !PK; ++t) {
                     const int st = stage.idx;
                     if (j == 0 && t < preloaded) {   // already in flight (early loads)
                         stage.advance(S);
@@ -371,7 +485,78 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 claim = __shfl_sync(0xffffffffu, ahead, 0);
             }
             if (lane == 0) fed::stamp(comm, 4);
-        } else if (warp >= 4) {
+        } else if (warp < 4) {
+            // ================= PK: decoders (warps 1 to 3) ==========================================
+            // Per tile: wait for a free stage, decode its panels in order as their compressed slots land (the slot is
+            // released right after), copy the footer (double-buffered by tile parity: the barrier below orders every
+            // read of buffer b before its next write, two tiles later) and the row data, then patch the exceptions
+            // once all 96 threads' stores are in, and arrive on full[stage] after a proxy fence.
+            if (PK) {
+                const int td = threadIdx.x - 32;
+                int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
+                Ring stage, xs;
+                uint32_t fb = 0;
+                for (int j = 0;; ++j) {
+                    // decide each chunk together, as the consumers do: a decoder warp leaving on a stalled pipeline
+                    // while the others wait at the barrier below would hang
+                    mbar_wait(&bar_ring[j & (kRing - 1)], (uint32_t)((j / kRing) & 1));
+                    named_sync(2, kDecThreads);
+                    if (td == 0) *decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[j & (kRing - 1)];
+                    named_sync(2, kDecThreads);
+                    const int4 ch = *decided;
+                    if (ch.x < 0) break;
+                    const uint32_t tab[4] = {segs_g[ch.x].xtab[0], segs_g[ch.x].xtab[1], segs_g[ch.x].xtab[2],
+                                             segs_g[ch.x].xtab[3]};
+                    for (int t = 0; t < ch.z; ++t) {
+                        mbar_wait(&bar_empty[stage.idx], stage.phase ^ 1);
+                        unsigned char* dst = smem + (size_t)stage.idx * L.stage_bytes;
+                        int* foot = reinterpret_cast<int*>(smem + L.off_xfoot + fb * kXFoot);
+                        for (int pnl = 0; pnl < panels; ++pnl) {
+                            mbar_wait(&bar_xfull[xs.idx], xs.phase);
+                            const unsigned char* src = smem + L.off_x + (size_t)xs.idx * L.xslot_bytes;
+                            if (pnl == 0) {
+                                if (td < kXFoot / 4) foot[td] = reinterpret_cast<const int*>(src + kXBlock)[td];
+                                const float* rsrc = reinterpret_cast<const float*>(src + kXBlock + kXFoot);
+                                float* rdst = reinterpret_cast<float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
+                                for (int i = td; i < (int)L.row_bytes / 4; i += kDecThreads) rdst[i] = rsrc[i];
+                            }
+                            // all of this thread's loads of the panel first, then the decodes and stores: one warp
+                            // per scheduler runs this, so the shared-memory latency is hidden by ILP, not by warps
+                            unsigned char* pd = dst + pnl * kPanelBytes;
+                            constexpr int kPer = (kTileM * 8 + kDecThreads - 1) / kDecThreads;
+                            uint2 lo[kPer];
+                            uint32_t cw[kPer];
+#pragma unroll
+                            for (int k = 0; k < kPer; ++k) {
+                                const int i = td + k * kDecThreads;
+                                if (k < kPer - 1 || i < kTileM * 8) {
+                                    lo[k] = reinterpret_cast<const uint2*>(src)[i];
+                                    cw[k] = reinterpret_cast<const uint32_t*>(src + kTileM * kPanel)[i];
+                                }
+                            }
+#pragma unroll
+                            for (int k = 0; k < kPer; ++k) {
+                                const int i = td + k * kDecThreads;
+                                if (k < kPer - 1 || i < kTileM * 8)
+                                    *reinterpret_cast<uint4*>(pd + x12_chunk_offset(i)) = x12_decode8(lo[k], cw[k], tab);
+                            }
+                            mbar_arrive(&bar_xempty[xs.idx]);
+                            xs.advance((int)L.xslots);
+                        }
+                        named_sync(2, kDecThreads);   // the tile's decoded chunks and its footer are in
+                        const int n_ex = min(foot[0], kXMaxExceptions);
+                        for (int e = td; e < n_ex; e += kDecThreads) {
+                            const uint32_t v = (uint32_t)foot[1 + e];
+                            if ((v >> 8) < (uint32_t)panels * kTileM * kPanel) dst[x12_high_byte_offset(v >> 8)] = (unsigned char)(v & 0xFFu);
+                        }
+                        fence_proxy_async();
+                        mbar_arrive(&bar_full[stage.idx]);
+                        stage.advance(S);
+                        fb ^= 1u;
+                    }
+                }
+            }
+        } else {
             // ================= consumer warpgroups ===============================================
             const int c = (warp >> 2) - 1;          // rows 64c .. 64c + 63 of every tile, gradient features c PP/2 ..
             const int w = warp & 3;                 // warp within the group: accumulator rows 16w .. 16w + 15
@@ -680,7 +865,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         if (threadIdx.x == 0) fed::stamp(comm, 6);
     } else if (warp == 0) {
         // nothing will be computed (stop / idle): the early loads still have to land before the CTA may exit
-        for (int t = 0; t < preloaded; ++t) mbar_wait(&bar_full[t], 0u);
+        for (int t = 0; t < preloaded; ++t) mbar_wait(PK ? &bar_xfull[t] : &bar_full[t], 0u);
     }
     __syncthreads();
     const unsigned long long status = *pipeline_fault() ? B200FED_ERR_PIPELINE : 0ull;
@@ -695,9 +880,9 @@ namespace {
 int chains_bucket(int k) { return k <= 1 ? 1 : (k <= 4 ? 4 : (k <= 8 ? 8 : (k <= 16 ? 16 : 0))); }
 
 // The shared-memory layout of a launch in bucket kc with epilogue e (the kernel derives the same one)
-tc::SmemLayout launch_layout(int n_features, int kc, tc::Epi e, int n_theta, bool rows, int row_data) {
+tc::SmemLayout launch_layout(int n_features, int kc, tc::Epi e, int n_theta, bool rows, int row_data, bool packed = false) {
     return tc::smem_layout((n_features + 127) & ~127, tc::cfg(kc).N1, tc::cfg(kc).N2, n_theta,
-                           tc::has_dispersion(e) ? tc::kDispWords : 0, kc, tc::row_arrays(rows, row_data));
+                           tc::has_dispersion(e) ? tc::kDispWords : 0, kc, tc::row_arrays(rows, row_data), packed);
 }
 
 using LaunchFn = int (*)(const FedComm*, const GlmSegment*, const GlmParams*, const void*, const void*, int, unsigned int*,
@@ -706,8 +891,9 @@ using LaunchFn = int (*)(const FedComm*, const GlmSegment*, const GlmParams*, co
 template <int KC, bool ROWS, tc::Epi E>
 int launch(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps, const void* chunks_dev,
            int n_chunks, unsigned int* work_counter, int grid, cudaStream_t stream) {
-    const tc::SmemLayout L = launch_layout(prm->n_features, KC, E, comm->n_theta, ROWS, prm->row_data);
+    const tc::SmemLayout L = launch_layout(prm->n_features, KC, E, comm->n_theta, ROWS, prm->row_data, prm->packed_x != 0);
     if (L.stages < 2) return -2;
+    if (prm->packed_x && L.xslots < 2) return -4;
     return tc::launch_pdl(tc::fed_glm_tc_kernel<KC, ROWS, E>, grid, tc::kThreads, L.total, stream, *comm, segs_dev, *prm,
                           reinterpret_cast<const CUtensorMap*>(tmaps), reinterpret_cast<const GlmChunk*>(chunks_dev),
                           n_chunks, work_counter);
@@ -817,6 +1003,40 @@ extern "C" int b200_glm_tc_stages(int n_features, int n_chains, int n_groups, in
     const int kc = chains_bucket(n_chains);
     if (kc == 0) return 0;
     return (int)launch_layout(n_features, kc, tc::epilogue(family), 0, row_data != 0, row_data).stages;
+}
+
+// Compressed panel slots of the packed-X layout of this shape with n_theta theta words (host only): the shape can run
+// packed when >= 2.
+extern "C" int b200_glm_tc_packed_slots(int n_features, int n_chains, int n_groups, int family, int row_data, int n_theta) {
+    const int kc = chains_bucket(n_chains);
+    if (kc == 0) return 0;
+    return (int)launch_layout(n_features, kc, tc::epilogue(family), n_theta, row_data != 0, row_data, true).xslots;
+}
+
+// The decoder of the packed X on the host (tests/test_glm_packed.py): one tile of `panels` kXBlock blocks, its
+// footer (kXFoot bytes) and the segment's table (4 words) -> the tile's 128B-swizzled bf16 image (panels x 16 KB),
+// in the order the kernel's decoders use.  Returns the exception count, or -1 for a footer that holds too many.
+extern "C" int b200_glm_x12_decode_tile(const unsigned char* blocks, const int* footer, const unsigned int* tab, int panels,
+                                        unsigned char* out) {
+    const uint32_t t[4] = {tab[0], tab[1], tab[2], tab[3]};
+    for (int pnl = 0; pnl < panels; ++pnl) {
+        const unsigned char* src = blocks + (size_t)pnl * tc::kXBlock;
+        for (int i = 0; i < tc::kTileM * 8; ++i) {
+            uint2 lo;
+            uint32_t c;
+            std::memcpy(&lo, src + 8 * i, 8);
+            std::memcpy(&c, src + tc::kTileM * tc::kPanel + 4 * i, 4);
+            const uint4 v = tc::x12_decode8(lo, c, t);
+            std::memcpy(out + (size_t)pnl * tc::kPanelBytes + tc::x12_chunk_offset(i), &v, 16);
+        }
+    }
+    if (footer[0] < 0 || footer[0] > tc::kXMaxExceptions) return -1;
+    for (int e = 0; e < footer[0]; ++e) {
+        const uint32_t v = (uint32_t)footer[1 + e];
+        if ((v >> 8) >= (uint32_t)panels * tc::kTileM * tc::kPanel) return -1;
+        out[tc::x12_high_byte_offset(v >> 8)] = (unsigned char)(v & 0xFFu);
+    }
+    return footer[0];
 }
 
 extern "C" int b200_launch_glm_tc(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm, const void* tmaps,

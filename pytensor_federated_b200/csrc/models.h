@@ -22,6 +22,12 @@ struct GlmSegment {
     long long first_tile; // prefix sum over segments of ceil(n_rows / tile_rows)
     int group;            // which intercept this segment uses
     int out_group;        // which output block this segment's [LL, grads] go to (0 unless per-node outputs are kept)
+    // bf16 tensor-core kernel, GlmParams::packed_x: X as a lossless 12-bit code (tc::x12_decode8), one 12 KB block per
+    // (128-row tile, 64-feature panel) in tile-major order, a 256-byte exception footer per tile, and the segment's
+    // 16-entry table of high bytes (entry 4 q + b in byte b of xtab[q])
+    const void* xpack;
+    const void* xfoot;
+    unsigned int xtab[4];
 };
 
 struct GlmParams {
@@ -37,6 +43,7 @@ struct GlmParams {
     int row_data;         // kGlmRowOffsets | kGlmRowWeights when any segment has them: selects the kernel instantiation
     int n_classes;        // C: multinomial classes or ordinal categories (GlmFamily::columns), else 1.  Theta row v holds
                           // column v: (intercept[:, c], beta[:, c]) of class c, (intercept - c_j, beta) of cutpoint j
+    int packed_x;         // bf16 tensor-core kernel: X is read from GlmSegment::xpack / xfoot (B200FED_NO_PACKED_X=1: never)
 };
 
 constexpr int kGlmRowOffsets = 1;

@@ -45,6 +45,7 @@ int b200_launch_glm_tc(const FedComm*, const GlmSegment*, const GlmParams*, cons
 int b200_glm_tc_prepare(const GlmSegment* segs_host, int n_segments, const GlmParams* prm, int sm_count, void** tmaps_dev,
                         void** chunks_dev, int* n_chunks);
 size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int family);
+int b200_glm_tc_packed_slots(int n_features, int n_chains, int n_groups, int family, int row_data, int n_theta);
 int b200_launch_ode(const FedComm*, const OdeShard*, int, int, cudaStream_t);
 int b200_launch_glm_fp8(const FedComm*, const GlmSegment*, const GlmParams*, const void* tmaps, const void* chunks,
                         int n_chunks, unsigned int* work_counter, int grid, cudaStream_t stream);
@@ -681,6 +682,38 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         e->grid = e->sm_count * 2;
     }
     if ((long long)e->grid > tiles && tiles > 0) e->grid = (int)tiles;
+    return 0;
+}
+
+// Switches the bf16 tensor-core model set by b200_engine_set_glm to the packed design matrix (GlmSegment::xpack,
+// xfoot, xtab; tabs: 4 words per segment), or back to X itself when xpack is null.  Refused (and nothing changes)
+// when the model is not on that kernel, an array is not 16-byte aligned or the shape's packed layout (with the engine's
+// theta, which is staged in the two bf16 stages) does not fit.
+int b200_engine_set_glm_packed(void* h, int n_segments, const void** xpack, const void** xfoot, const unsigned int* tabs) {
+    Engine* e = static_cast<Engine*>(h);
+    CK(cudaSetDevice(e->device));
+    if (e->kind != MODEL_GLM_TC || n_segments != (int)e->glm_segs.size()) {
+        g_last_error = "packed X needs the bf16 tensor-core GLM model it was made for";
+        return -41;
+    }
+    std::vector<GlmSegment> segs = e->glm_segs;
+    for (int s = 0; s < n_segments; ++s) {
+        segs[s].xpack = xpack ? xpack[s] : nullptr;
+        segs[s].xfoot = xpack ? xfoot[s] : nullptr;
+        for (int q = 0; q < 4; ++q) segs[s].xtab[q] = xpack ? tabs[4 * s + q] : 0u;
+        if (xpack && (!segs[s].xpack || !segs[s].xfoot || (((uintptr_t)segs[s].xpack | (uintptr_t)segs[s].xfoot) & 15) != 0)) {
+            g_last_error = "packed X: every segment needs 16-byte aligned blocks and footers";
+            return -42;
+        }
+    }
+    if (xpack && b200_glm_tc_packed_slots(e->glm.n_features, e->glm.n_chains, e->glm.n_groups, e->glm.family,
+                                          e->glm.row_data, e->n_theta) < 2) {
+        g_last_error = "packed X: this shape's packed layout does not fit in shared memory";
+        return -43;
+    }
+    CK(cudaMemcpy(e->glm_segs_dev, segs.data(), sizeof(GlmSegment) * n_segments, cudaMemcpyHostToDevice));
+    e->glm_segs = segs;
+    e->glm.packed_x = xpack ? 1 : 0;
     return 0;
 }
 

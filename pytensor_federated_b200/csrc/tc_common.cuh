@@ -90,6 +90,13 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const CUtensorMap* m
         "l"(map), "r"(c0), "r"(smem_u32(bar))
         : "memory");
 }
+// Plain (non-tensor) bulk copy of `bytes` (a multiple of 16, 16-byte aligned at both ends) into shared memory
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar))
+        : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }

@@ -14,6 +14,7 @@ oracle's per-row terms) is decided by one layout object per family (``_Scalar``,
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -464,6 +465,60 @@ class GlmShards(ShardModel):
         )
         if hasattr(self.family, "code_id"):
             lib.b200_engine_set_custom_launcher(handle, C.c_void_p(self.family.launcher_address()))
+        #: whether the tensor-core kernel reads X in its packed 12-bit form (see :func:`pack_x12`)
+        self.packed_x = False
+        if code == 1 and os.environ.get("B200FED_NO_PACKED_X", "0") in ("", "0"):
+            row_data = (1 if any(o is not None for o in self.offsets) else 0) | (2 if any(w is not None for w in self.weights) else 0)
+            fam = _family_code(self.family) | (HVP_FLAG if self.hvp else 0)
+            slots = int(lib.b200_glm_tc_packed_slots(self.n_features, self.kernel_chains, self.n_groups, fam, row_data,
+                                                     self.n_theta_words))
+            if slots >= 2 and self._packing_pays(row_data):
+                packs = self._packed()
+                if packs is not None:
+                    tabs = (C.c_uint * (4 * n))(*[w for _, _, t in packs for w in t])
+                    native.check(lib.b200_engine_set_glm_packed(
+                        handle, n, native.void_p_array([p.data_ptr() for p, _, _ in packs]),
+                        native.void_p_array([f.data_ptr() for _, f, _ in packs]), tabs), "set_glm_packed")
+                    self.packed_x = True
+
+    _packs = None            # the packed X, once made
+    _packs_refused = False   # some tile of X has more exceptions than its footer holds: X never packs
+
+    def _packing_pays(self, row_data: int) -> bool:
+        """Whether packed X is faster for this launch shape, as measured (docs/KERNELS.md, "Packed X"): launches of up to
+        4 kernel columns with the tile padded to 256 features (129 <= P <= 256).  At 16 columns the consumer chain binds
+        and at P <= 128 the bf16 layout has 4 stages to the packed one's 2: both were measured slower packed, and 8
+        columns were not measured, so those launches read X as bf16."""
+        return (self.n_features + 127) // 128 == 2 and self.kernel_chains <= X12_MAX_COLUMNS
+
+    def _packed(self):
+        """The packed form of every segment's X (made once, kept with the model), or None where some segment's X does
+        not pack (a tile with more exceptions than its footer holds: remembered, X does not change) or the device
+        lacks the memory for it now (tried again at the next attach); the kernel then reads X itself."""
+        import logging
+
+        import torch
+
+        if self._packs is not None or self._packs_refused:
+            return self._packs
+        log = logging.getLogger(__name__)
+        need = sum(x12_packed_bytes(X.shape[0], self.n_features) for X in self.Xs)
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need + (2 << 30) > free:   # headroom for the packing's temporaries
+            log.warning("not packing X: it needs %.1f GB and %.1f GB are free; the kernel reads the bf16 matrix",
+                        need / 1e9, free / 1e9)
+            return None
+        packs = []
+        for si, X in enumerate(self.Xs):
+            p = pack_x12(X[:, : self.n_features])
+            if p is None:
+                log.warning("not packing X: a tile of segment %d has more than %d values outside its table", si,
+                            X12_MAX_EXCEPTIONS)
+                self._packs_refused = True
+                return None
+            packs.append(p)
+        self._packs = packs
+        return packs
 
     # -- eager oracle (also the compute step of the NCCL baseline) ---------------------------
     def reference_partial(self, inputs, *, dtype=None, chunk_rows: int = 1 << 20) -> np.ndarray:
@@ -554,10 +609,92 @@ class GlmShards(ShardModel):
         return int(sum(4 * v.shape[0] for v in self.offsets + self.weights if v is not None))
 
     def bytes_per_eval(self) -> int:
+        """Bytes the kernel reads per evaluation: X (or its packed form, blocks and footers of every tile the kernel
+        visits), y and the row data."""
+        if getattr(self, "packed_x", False):
+            xb = sum(x12_packed_bytes(X.shape[0], self.n_features) for X in self.Xs)
+            return int(xb + sum(4 * X.shape[0] for X in self.Xs)) + self._row_data_bytes()
         return int(sum(X.shape[0] * (self.n_features * X.element_size() + 4) for X in self.Xs)) + self._row_data_bytes()
 
     def flops_per_eval(self) -> int:
         return int(4 * self.n_rows * self.n_features * self.kernel_chains)
+
+
+# -- packed X: a lossless 12-bit form of a bf16 design matrix (csrc/glm_tc.cu, "Packed X") ----------------------
+X12_BLOCK = 128 * 64 * 3 // 2   # bytes per (128-row tile, 64-feature panel): 8192 low bytes + 8192 4-bit codes
+X12_FOOT = 256                  # bytes of a tile's exception footer: count, then (position << 8 | high byte) words
+X12_MAX_EXCEPTIONS = X12_FOOT // 4 - 1
+X12_MAX_COLUMNS = 4             # kernel columns up to which a launch reads X packed (GlmShards._packing_pays)
+
+
+def x12_tiles(n_rows: int) -> int:
+    """Tiles the packed form of an n-row segment holds: the tensor-core kernel's chunks visit an even number."""
+    t = (n_rows + 127) // 128
+    return t + (t & 1)
+
+
+def x12_packed_bytes(n_rows: int, n_features: int) -> int:
+    return x12_tiles(n_rows) * (((n_features + 127) // 128 * 2) * X12_BLOCK + X12_FOOT)
+
+
+def pack_x12(X, chunk_rows: int = 1 << 17):
+    """The packed form of one segment's bf16 matrix ``X[n, P]``, on its device: ``(blocks, footers, table)``.
+
+    The 16-entry table of high bytes (sign and upper 7 exponent bits) holds 0x00 in entry 0 (padding: rows past n
+    and features past P are +0), the 14 most frequent other high bytes of X in entries 1-14, and code 15 marks an
+    exception.  ``blocks`` is uint8 ``[tiles, panels, 12288]``: per 128-row tile and 64-feature panel the low bytes
+    in row-major order, then the codes two per byte (the even feature in the low nibble).  ``footers`` is int32
+    ``[tiles, 64]``: the tile's exception count, then ``position << 8 | high byte`` with position = panel * 8192 +
+    row * 64 + feature, in increasing order.  ``table`` is the 4 little-endian words of the table.  Returns None
+    when a tile has more than 63 exceptions.  Works through ``chunk_rows`` rows (a multiple of 128) at a time."""
+    import torch
+
+    n, P = X.shape
+    PP = (P + 127) // 128 * 128
+    panels = PP // 64
+    tiles = x12_tiles(n)
+    dev = X.device
+    hist = torch.zeros(256, dtype=torch.long, device=dev)
+    for r0 in range(0, n, chunk_rows):
+        hb = (X[r0 : r0 + chunk_rows].contiguous().view(torch.int16) >> 8) & 0xFF
+        hist += torch.bincount(hb.reshape(-1).long(), minlength=256)
+    hist[0] = -1   # entry 0 is 0x00 whatever its count
+    order = torch.argsort(hist, descending=True, stable=True)[:14].tolist()
+    counts = hist.tolist()
+    entries = [0] + [b for b in order if counts[b] > 0]
+    entries += [0] * (16 - len(entries))
+    lut = torch.full((256,), 15, dtype=torch.uint8, device=dev)
+    for code in range(15 - 1, -1, -1):   # entries past the used ones repeat 0x00, which keeps code 0
+        lut[entries[code]] = code
+    table = [int.from_bytes(bytes(entries[4 * q : 4 * q + 4]), "little") for q in range(4)]
+
+    blocks = torch.empty(tiles, panels, X12_BLOCK, dtype=torch.uint8, device=dev)
+    foot = torch.zeros(tiles, X12_FOOT // 4, dtype=torch.int32, device=dev)
+    for r0 in range(0, tiles * 128, chunk_rows):
+        rows = min(chunk_rows, tiles * 128 - r0)
+        nt = rows // 128
+        t0 = r0 // 128
+        v = torch.zeros(rows, PP, dtype=torch.int16, device=dev)
+        valid = max(0, min(n, r0 + rows) - r0)
+        if valid:
+            v[:valid, :P] = X[r0 : r0 + valid].view(torch.int16)
+        v = v.view(nt, 128, panels, 64).permute(0, 2, 1, 3)                    # [tile, panel, row, feature]
+        hb = ((v >> 8) & 0xFF).to(torch.uint8)
+        code = lut[hb.long()]
+        blocks[t0 : t0 + nt, :, : 8192] = (v & 0xFF).to(torch.uint8).reshape(nt, panels, 8192)
+        blocks[t0 : t0 + nt, :, 8192 :] = (code[..., 0::2] | (code[..., 1::2] << 4)).reshape(nt, panels, 4096)
+        ex = (code == 15).reshape(nt, panels * 8192)
+        cnt = ex.sum(1)
+        if int(cnt.max()) > X12_MAX_EXCEPTIONS:
+            return None
+        foot[t0 : t0 + nt, 0] = cnt.to(torch.int32)
+        tile, pos = ex.nonzero(as_tuple=True)                                   # row-major: by tile, then position
+        if tile.numel():
+            start = torch.cumsum(cnt, 0) - cnt
+            rank = torch.arange(tile.numel(), device=dev) - start[tile]
+            word = (pos << 8) | hb.reshape(nt, panels * 8192)[tile, pos].long()
+            foot[t0 + tile, 1 + rank] = word.to(torch.int32)
+    return blocks, foot, table
 
 
 # -- family layouts ------------------------------------------------------------------------------

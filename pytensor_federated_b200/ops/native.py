@@ -85,6 +85,9 @@ def _declare(lib: C.CDLL) -> None:
     sig("b200_engine_trace", C.c_int, C.c_void_p, C.c_ulonglong, C.POINTER(C.c_ulonglong))
     sig("b200_glm_tc_chunk_table", C.c_int, c_ll_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_int_p, C.c_int)
     sig("b200_glm_tc_stages", C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)
+    sig("b200_glm_tc_packed_slots", C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)
+    sig("b200_glm_x12_decode_tile", C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p)
+    sig("b200_engine_set_glm_packed", C.c_int, C.c_void_p, C.c_int, c_void_pp, c_void_pp, C.POINTER(C.c_uint))
     sig("b200_engine_enable_cta_trace", None, C.c_void_p, C.c_int)
     sig("b200_engine_cta_trace", C.c_int, C.c_void_p, C.POINTER(C.c_ulonglong), C.c_int)
     sig("b200_engine_destroy", None, C.c_void_p)

@@ -190,11 +190,22 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 //               rows are v_intercept), whose epilogue writes ll = 0 and r = w h(eta_2p) u with u its own eta without
 //               the offset; its output block is then [0, (H v)_intercept[G], (H v)_beta[P]].  Both columns of a pair
 //               sit in one thread (e = 0 and e = 1).  No KC = 1 instance.
+//   ZeroInflated      the zero-inflated Poisson family (tc::zero_inflated_loglik over link_loglik): pair p runs as
+//                     column 2p (the count predictor eta: theta row (intercept, beta), the only one that takes the
+//                     offset) and column 2p + 1 (the zero logit zeta: theta row (zi_intercept, zi_beta)), in one thread
+//                     as in Hvp.  Both predictors are formed before either column's values: column 2p gets the pair's
+//                     ll and r = dll/deta, column 2p + 1 ll = 0 and r = dll/dzeta, so the intercept sums, the (hi, lo)
+//                     split and MMA #2 give both predictors' gradients.  No KC = 1 instance.
+//   ZeroInflatedDisp  the zero-inflated negative binomial: ZeroInflated over negbin_loglik, with Dispersion's theta and
+//                     output layout (both theta rows of a pair end in log alpha; the table of column 2p is used, q
+//                     comes from column 2p and column 2p + 1 writes q = 0).
 // Column layouts follow the wgmma accumulator fragment (thread lane owns columns 8j + 2 (lane % 4) + {0, 1}), so
 // that one thread holds every term of the chains it works on.
-enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp };
+enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp };
 
-__host__ __device__ constexpr bool has_dispersion(Epi e) { return e == Epi::Dispersion || e == Epi::Survival; }
+__host__ __device__ constexpr bool has_dispersion(Epi e) {
+    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp;
+}
 
 constexpr Epi epilogue(int family) {
     if (family & kGlmHvp) return Epi::Hvp;
@@ -203,11 +214,13 @@ constexpr Epi epilogue(int family) {
         case kGlmGaussianScale: case kGlmNegBinomial: return Epi::Dispersion;
         case kGlmOrdinal: return Epi::Ordinal;
         case kGlmWeibull: case kGlmLogNormal: return Epi::Survival;
+        case kGlmZeroInflatedPoisson: return Epi::ZeroInflated;
+        case kGlmZeroInflatedNegBinomial: return Epi::ZeroInflatedDisp;
         default: return Epi::Scalar;
     }
 }
 static_assert([] {
-    for (int code = 0; code <= kGlmLogNormal; ++code)
+    for (int code = 0; code <= kGlmZeroInflatedNegBinomial; ++code)
         if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
     return true;
 }(), "the epilogue's theta and output layout must match the family's");
@@ -246,7 +259,8 @@ __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
     constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
-                   SURV = E == Epi::Survival, HVP = E == Epi::Hvp;
+                   SURV = E == Epi::Survival, HVP = E == Epi::Hvp,
+                   ZI = E == Epi::ZeroInflated || E == Epi::ZeroInflatedDisp, ZNB = E == Epi::ZeroInflatedDisp;
     constexpr int C8 = cfg(KC).C8;
     constexpr int N1 = cfg(KC).N1;
     constexpr int N2 = cfg(KC).N2;
@@ -384,7 +398,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         if constexpr (SURV)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 survival_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
-        else if constexpr (DISP)
+        else if constexpr (DISP)   // families 4 and 5, and 10, whose table is family 5's (any code but 4)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = term * C8 + chain
@@ -700,6 +714,27 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc) {
                             float hv_h = 0.f;   // HVP: h = d2ll / deta2 of the pair's theta column (e = 0), for e = 1
+                            // ZI: the pair's values (columns k0 = 8 jc + 2 q and k0 + 1), from both predictors, before
+                            // the column loop; offset and weight as in ROWS (the offset to eta only).  n_chains is even,
+                            // so k0 < nch covers both columns.
+                            float zi_ll = 0.f, zi_rc = 0.f, zi_rz = 0.f, zi_q = 0.f;
+                            if constexpr (ZI) {
+                                const int k0 = 8 * jc + 2 * q;
+                                if (valid && k0 < nch) {
+                                    float et = ((eacc[4 * jc + 2 * h] + eacc[4 * (NJ + jc) + 2 * h]) +
+                                                eacc[4 * (2 * NJ + jc) + 2 * h]) + icpt[k0];
+                                    if constexpr (ROWS) et = __fadd_rn(et, o);
+                                    const float zt = ((eacc[4 * jc + 2 * h + 1] + eacc[4 * (NJ + jc) + 2 * h + 1]) +
+                                                      eacc[4 * (2 * NJ + jc) + 2 * h + 1]) + icpt[k0 + 1];
+                                    zero_inflated_loglik<ZNB>(y, et, zt, disp + k0 * kDispWords, zi_ll, zi_rc, zi_rz, zi_q);
+                                    if constexpr (ROWS) {
+                                        apply_weight(wt, zi_ll);
+                                        apply_weight(wt, zi_rc);
+                                        apply_weight(wt, zi_rz);
+                                        apply_weight(wt, zi_q);
+                                    }
+                                }
+                            }
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int k = 8 * jc + 2 * q + e;
@@ -707,7 +742,12 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
                                 float ll = 0.f, r = 0.f, dq = 0.f;
                                 if (valid && k < nch) {
-                                    if constexpr (DISP) {
+                                    if constexpr (ZI) {
+                                        // column 2p: the pair's ll, dll/deta (and dll/dlog_alpha); 2p + 1: dll/dzeta
+                                        ll = e == 0 ? zi_ll : 0.f;
+                                        r = e == 0 ? zi_rc : zi_rz;
+                                        dq = e == 0 ? zi_q : 0.f;
+                                    } else if constexpr (DISP) {
                                         // offset and weight as in ROWS, the weight applied to all three values
                                         float et = eta + icpt[k];
                                         if constexpr (ROWS) et = __fadd_rn(et, o);
@@ -899,14 +939,16 @@ int launch(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm
                           n_chunks, work_counter);
 }
 
-// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax and Hvp (two columns at least) in
-// KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are instantiated, which is the order
-// of the cases here.
+// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax, Hvp and the zero-inflated ones (two
+// columns at least) in KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are
+// instantiated, which is the order of the cases here: later epilogues go after the default.
 template <tc::Epi E>
 LaunchFn pick(int kc, bool rows) {
     switch (kc) {
         case 1:
-            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp) return nullptr;
+            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp || E == tc::Epi::ZeroInflated ||
+                          E == tc::Epi::ZeroInflatedDisp)
+                return nullptr;
             else return rows ? launch<1, true, E> : launch<1, false, E>;
         case 4: return rows ? launch<4, true, E> : launch<4, false, E>;
         case 8: return rows ? launch<8, true, E> : launch<8, false, E>;
@@ -922,6 +964,8 @@ LaunchFn pick(tc::Epi e, int kc, bool rows) {
         case Epi::Survival: return pick<Epi::Survival>(kc, rows);
         case Epi::Dispersion: return pick<Epi::Dispersion>(kc, rows);
         default: return pick<Epi::Scalar>(kc, rows);
+        case Epi::ZeroInflated: return pick<Epi::ZeroInflated>(kc, rows);
+        case Epi::ZeroInflatedDisp: return pick<Epi::ZeroInflatedDisp>(kc, rows);
     }
 }
 }  // namespace

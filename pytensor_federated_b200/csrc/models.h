@@ -34,8 +34,8 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10: [.., log_dispersion])
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10: [K][G+P+1])
     int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
@@ -65,11 +65,14 @@ enum GlmFamilyCode : int {
     kGlmOrdinal = 6,         // cumulative logit over n_classes categories, one column per cutpoint
     kGlmWeibull = 7,         // right-censored survival (AFT), log_dispersion = log sigma,
     kGlmLogNormal = 8,       //   y = +t for an event, -t for a censored row
+    kGlmZeroInflatedPoisson = 9,       // zero-inflated counts: pair p is column 2p (count eta) and 2p + 1 (zero logit
+    kGlmZeroInflatedNegBinomial = 10,  //   zeta); family 10 adds NB2's log_dispersion = log alpha
 };
 
 // How a family's columns make up n_chains: one per chain, one per chain and class (column k C + c is class c of chain
-// k), or one per chain and cutpoint (column k (C - 1) + j is cutpoint j of chain k), for C = n_classes
-enum class GlmColumns { kOne, kPerClass, kPerCutpoint };
+// k), one per chain and cutpoint (column k (C - 1) + j is cutpoint j of chain k), for C = n_classes, or two per chain
+// (column 2k and 2k + 1: the zero-inflated families' count and zero predictors)
+enum class GlmColumns { kOne, kPerClass, kPerCutpoint, kPair };
 
 // What the runtime and the bf16 tensor-core kernel need to know about a family code.
 struct GlmFamily {
@@ -88,6 +91,9 @@ constexpr GlmFamily glm_family(int code) {
         case kGlmOrdinal: return {"ordinal", true, false, GlmColumns::kPerCutpoint, 2, 17, true};
         case kGlmWeibull: return {"weibull", true, true, GlmColumns::kOne, 1, 1, true};
         case kGlmLogNormal: return {"lognormal", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmZeroInflatedPoisson: return {"zero_inflated_poisson", true, false, GlmColumns::kPair, 1, 1, true};
+        case kGlmZeroInflatedNegBinomial:
+            return {"zero_inflated_negative_binomial", true, true, GlmColumns::kPair, 1, 1, true};
         default: return {"", false, false, GlmColumns::kOne, 1, 1, true};   // 0 to 2: every GLM kernel
     }
 }

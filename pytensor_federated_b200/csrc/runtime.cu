@@ -601,6 +601,11 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
                            " family needs n_chains = K x (n_classes - 1) (one column per chain and cutpoint)";
             return -36;
         }
+        if (f.columns == GlmColumns::kPair && (n_chains < 2 || n_chains > 16 || n_chains % 2 != 0)) {
+            g_last_error = std::string("the ") + f.name +
+                           " family needs an even n_chains in [2, 16] (a count and a zero-inflation column per chain)";
+            return -44;
+        }
         for (int s = 0; s < n_segments && offsets && !f.offsets; ++s)
             if (offsets[s]) {
                 g_last_error = std::string("the ") + f.name + " family takes no offsets (one common to all classes cancels)";

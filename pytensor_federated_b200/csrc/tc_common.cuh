@@ -490,6 +490,44 @@ __device__ __forceinline__ void negbin_loglik(float y, float eta, const float* t
     q = alpha * (dpsi - sp) - r;
 }
 
+// Zero-inflated counts (families 9 and 10), one row of a pair: count predictor eta (offset included), zero logit zeta,
+// pi = sigmoid(zeta).  (l, r, q) = the base family's values at eta exactly as the plain family computes them (Poisson:
+// link_loglik, NB: negbin_loglik with the chain's table t; both omit -lgamma(y + 1), which is 0 at y = 0, so l is
+// log f(0) there), then mixed:
+//   y > 0:  ll = l - softplus(zeta),  rc = r,  rz = -sigmoid(zeta),  q unchanged
+//   y = 0:  ll = log(e^zeta + e^L0) - softplus(zeta) with L0 = l, d = zeta - L0,  w0 = sigmoid(-d),
+//           rc = w0 r,  rz = sigmoid(d) - sigmoid(zeta) = -sigmoid(d) sigmoid(-zeta) expm1(L0),  q = w0 q
+// rc = dll/deta, rz = dll/dzeta, q = dll/dlog_alpha.  The product form of rz keeps its relative accuracy as mu -> 0
+// (-expm1(L0) ~ mu).  The mixing comes after the base values and in this order, so that at zeta = -120 with
+// L0 >= -15 (exp(-|d|) and exp(zeta) underflow to 0, sigmoid(-d) is exactly 1) ll, rc and q are the base family's
+// bits and rz is 0.  A NaN y (a masked row) takes the y = 0 branch and is dropped by its weight.
+template <bool NB>
+__device__ __forceinline__ void zero_inflated_loglik(float y, float eta, float zeta, const float* t, float& ll, float& rc,
+                                                     float& rz, float& q) {
+    float l, r;
+    q = 0.f;
+    if constexpr (NB) negbin_loglik(y, eta, t, l, r, q);
+    else link_loglik(1, y, eta, l, r);
+    const float ez = expf(-fabsf(zeta));
+    const float spz = fmaxf(zeta, 0.f) + log1pf(ez);   // softplus(zeta)
+    const float iz = __frcp_rn(1.f + ez);
+    if (y > 0.f) {
+        ll = l - spz;
+        rc = r;
+        rz = -(zeta >= 0.f ? iz : ez * iz);
+    } else {
+        const float d = zeta - l;
+        const float ed = expf(-fabsf(d));
+        ll = (fmaxf(zeta, l) + log1pf(ed)) - spz;
+        const float id = __frcp_rn(1.f + ed);
+        const float sd = d >= 0.f ? id : ed * id;    // sigmoid(d)
+        const float w0 = d >= 0.f ? ed * id : id;    // sigmoid(-d)
+        rc = w0 * r;
+        q = w0 * q;
+        rz = -(sd * (zeta >= 0.f ? ez * iz : iz)) * expm1f(l);
+    }
+}
+
 // Right-censored survival, accelerated failure time: log T = eta + sigma eps, s = log sigma, z = (log t - eta) / sigma,
 // delta = 1 for an event and 0 for a censored row.  Family 7 (Weibull, eps standard minimum-Gumbel, shape 1 / sigma)
 // and family 8 (log-normal, eps ~ N(0, 1)) use the Gaussian's table words kDwSinv and kDwS.  The host stores each

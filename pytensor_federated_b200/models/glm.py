@@ -9,7 +9,7 @@ Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
 
 How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
 oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
-``_Ordinal``, ``_Survival`` below); :class:`GlmShards` and its callers are generic over it.
+``_Ordinal``, ``_Survival``, ``_Hvp``, ``_ZeroInflated`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ import numpy as np
 from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
-            "ordinal": 6, "weibull": 7, "lognormal": 8}
+            "ordinal": 6, "weibull": 7, "lognormal": 8, "zero_inflated_poisson": 9, "zero_inflated_negative_binomial": 10}
 
 
 #: dynamic shared memory one CTA may opt in to on the H100 (227 KB), less 256 bytes for a kernel's static variables
@@ -165,6 +165,30 @@ class GlmShards(ShardModel):
         for every other family.  The model keeps a float32 copy of the times with censored rows negated, which is
         what the kernel reads (the tensors passed in are not modified).  Only the bf16 tensor-core kernel evaluates
         these families, with the shape limits of the multinomial one; ``n_classes`` is rejected.
+
+        ``"zero_inflated_poisson"`` and ``"zero_inflated_negative_binomial"`` are count models with excess zeros
+        (brms' ``zero_inflated_poisson`` / ``zero_inflated_negbinomial``, PyMC's ``ZeroInflatedPoisson`` /
+        ``ZeroInflatedNegativeBinomial``, R's ``pscl::zeroinfl``): insurance claims, species counts, visits, defects.
+        Two linear predictors share the covariates: the count predictor ``eta = intercept[group] + x' beta + o`` (the
+        offset goes into eta only, as in brms and pscl) and the zero-inflation logit ``zeta = zi_intercept[group] + x'
+        zi_beta``.  ``pi = sigmoid(zeta)`` is the probability of a structural zero (brms' ``zi``; PyMC's ``psi`` is
+        ``1 - pi``), and with f the Poisson(``mu = e^eta``) or NB2(``mu``, ``alpha = e^a``) pmf of the plain families:
+
+            P(y = 0) = pi + (1 - pi) f(0),     P(y > 0) = (1 - pi) f(y).
+
+        LL omits ``-lgamma(y + 1)`` on the rows with y > 0, as ``"poisson"`` and ``"negative_binomial"`` do; that
+        constant is 0 at y = 0, so the plain families' per-row LL at y = 0 is exactly ``log f(0)`` and the mixture
+        is exact.  The inputs per call are ``(intercept, beta, zi_intercept, zi_beta)``, shapes ``[G]``, ``[P]``,
+        ``[G]`` and ``[P]`` (a scalar intercept when G = 1), and for the negative binomial a trailing scalar
+        ``log_dispersion = log alpha``; batched with a leading K (at most 8).  Gradients come back in the shapes of
+        the inputs.  Chain k runs as the kernel columns 2k (eta) and 2k + 1 (zeta) of a 2K-column launch, so X is
+        read once for both predictors.  An intercept-only zero part (brms' ``zi ~ 1``) is ``zi_beta = 0``, held
+        fixed (its gradient ignored); it costs the same launch.  Both parts are identified by the data only through
+        the zeros: with few zeros or a zeta far below 0 the zero part is weakly identified, so give it a prior.
+        Counts must be integers in ``[0, 2^24]`` on every row of non-zero weight; offsets and weights work as for
+        every family.  Only the bf16 tensor-core kernel evaluates these families, with the shape limits of the
+        multinomial one; ``n_classes``, ``events`` and ``hvp`` are rejected, and so is a shape whose 2K-column
+        launch gets fewer than two pipeline stages (checked when an engine attaches the model).
     events
         Per-row event indicators of the survival families (see ``family``).
     hvp
@@ -433,12 +457,13 @@ class GlmShards(ShardModel):
         rows = (C.c_longlong * n)(*[X.shape[0] for X in self.Xs])
         grp = (C.c_int * n)(*self.groups)
         code = int(self.use_tensor_cores())
-        if self.hvp:
+        if self._layout.pairs:
             # the 2K-column launch must get two TMA stages; refused here, before the engine's model changes
             row_data = (1 if any(o is not None for o in self.offsets) else 0) | (2 if any(w is not None for w in self.weights) else 0)
-            fam = _family_code(self.family) | HVP_FLAG
+            fam = _family_code(self.family) | (HVP_FLAG if self.hvp else 0)
             if int(lib.b200_glm_tc_stages(self.n_features, self.kernel_chains, self.n_groups, fam, row_data)) < 2:
-                raise ValueError(f"hvp=True with {self.n_chains} pairs at P = {self.n_features}: the tensor-core kernel's "
+                what = "hvp=True" if self.hvp else f"family={self.family!r}"
+                raise ValueError(f"{what} with {self.n_chains} pairs at P = {self.n_features}: the tensor-core kernel's "
                                  f"{self.kernel_chains}-column launch gets fewer than two pipeline stages in shared memory; "
                                  f"use fewer pairs per launch")
         #: which fused kernel serves this model ("tc" / "fp8" = wgmma tensor cores, else CUDA cores)
@@ -582,7 +607,7 @@ class GlmShards(ShardModel):
                 else:
                     out[::step, 1 + G : 1 + G + P] += (r.sum(2).T.to(torch.bfloat16) @ Xf).double()
                 for t in q:
-                    out[:, 1 + G + P] += t.double().sum(0)
+                    out[:, 1 + G + P] += t.double().sum(0).reshape(-1)
         return full.reshape(-1).cpu().numpy()
 
     def _weigh(self, seg: int, r0: int, r1: int, *terms):
@@ -754,6 +779,7 @@ class _Layout:
     tc_only = True   # no kernel but the bf16 tensor-core one evaluates the family
     offset_columns = slice(None)   # the columns of eta that take the per-row offset (all of them)
     takes_events = False   # the survival families' per-row event indicators
+    pairs = False   # two kernel columns per chain (2k, 2k + 1), at most 8 chains, checked for two stages at attach
 
     def __init__(self, m) -> None:
         self.family, self.K, self.G, self.P = m.family, m.n_chains, m.n_groups, m.n_features
@@ -867,6 +893,7 @@ class _Hvp(_Scalar):
     columns = 2
     tc_only = True
     offset_columns = slice(0, None, 2)
+    pairs = True
 
     def __init__(self, m, n_classes) -> None:
         if m.family not in ("logistic", "poisson", "gaussian"):
@@ -1088,8 +1115,69 @@ class _Ordinal(_Layout):
         return (*self._matrices(inputs), terms)
 
 
+class _ZeroInflated(_Layout):
+    """``zero_inflated_poisson`` and ``zero_inflated_negative_binomial``: inputs ``(intercept[G], beta[P],
+    zi_intercept[G], zi_beta[P])`` and, for the negative binomial, a trailing ``log_dispersion``.  Chain k runs as
+    kernel columns 2k, with the theta row ``(intercept, beta[, log_dispersion])`` and the output block ``[LL,
+    d intercept[G], d beta[P](, d log_dispersion)]``, and 2k + 1, with the theta row ``(zi_intercept, zi_beta[,
+    log_dispersion])`` and the output block ``[0, d zi_intercept[G], d zi_beta[P](, 0)]``.  Only the count columns
+    take the offset."""
+
+    columns = 2
+    offset_columns = slice(0, None, 2)
+    pairs = True
+
+    def __init__(self, m, n_classes) -> None:
+        self._no_classes(n_classes)
+        _tc_kernel_only(m)
+        if not 1 <= m.n_chains <= 8:
+            raise ValueError(f"the {m.family} family takes n_chains in [1, 8] (each chain's count and zero-inflation "
+                             f"predictors are two of the tensor-core kernel's 16 columns per launch), got {m.n_chains}")
+        _check_integers(m, "counts", "[0, 2^24]", lambda y: y <= 2.0 ** 24)
+        super().__init__(m)
+        self.nb = m.family == "zero_inflated_negative_binomial"
+        self.shapes = self.shapes * 2 + ([()] if self.nb else [])
+        self.words += int(self.nb)
+
+    def pack(self, inputs, out: np.ndarray):
+        G, P = self.G, self.P
+        xs = [np.asarray(x) for x in inputs]
+        th = out.view(np.float32).reshape(self.K, 2, self.words)
+        th[:, 0, :G] = xs[0].reshape(self.K, G)
+        th[:, 0, G : G + P] = xs[1].reshape(self.K, P)
+        th[:, 1, :G] = xs[2].reshape(self.K, G)
+        th[:, 1, G : G + P] = xs[3].reshape(self.K, P)
+        if self.nb:
+            th[:, :, G + P] = xs[4].reshape(self.K, 1)   # both rows: every column's table is built from its own row
+        return self.call_context(xs)
+
+    def _theta_rows(self, words: np.ndarray) -> np.ndarray:
+        th = words.view(np.float32).reshape(self.K, 2, self.words)
+        GP = self.G + self.P
+        return np.concatenate([th[:, 0, :GP], th[:, 1, :GP], th[:, 0, GP:]], axis=1)
+
+    def fold(self, raw: np.ndarray, ctx) -> np.ndarray:
+        n, GP = raw.shape[0], self.G + self.P
+        raw = raw.reshape(n, self.K, 2, 1 + self.words)
+        return np.concatenate([raw[:, :, 0, : 1 + GP], raw[:, :, 1, 1 : 1 + GP], raw[:, :, 0, 1 + GP :]], axis=2)
+
+    def oracle(self, inputs, device, dtype):
+        import torch
+
+        ic, bt = self._matrices(inputs[:2])
+        zic, zbt = self._matrices(inputs[2:4])
+        pairs = lambda a, b: torch.stack([a, b], dim=2).reshape(a.shape[0], -1)   # column 2k: eta, 2k + 1: zeta
+        ld = _f64(inputs[4]).reshape(self.K).to(device, dtype) if self.nb else None
+
+        def terms(y, w, eta):
+            return _zero_inflated_terms(y.to(eta.dtype).unsqueeze(1), eta[:, 0::2], eta[:, 1::2], ld)
+
+        return pairs(ic, zic), pairs(bt, zbt), terms
+
+
 _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_binomial": _Dispersion,
-            "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival}
+            "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival,
+            "zero_inflated_poisson": _ZeroInflated, "zero_inflated_negative_binomial": _ZeroInflated}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -1174,6 +1262,36 @@ def _lognormal_terms(y, eta, s):
     r = torch.where(event, z, lam) * sinv
     q = torch.where(event, z * z - 1.0, z * lam)
     return ll, r, q
+
+
+def _zero_inflated_terms(y, eta, zeta, a=None):
+    """The per-row terms of a zero-inflated count model, ``[n, K, 2]`` (column 0: eta, 1: zeta): ``ll`` (in column 0,
+    0 in column 1), ``(dll/deta, dll/dzeta)`` and, with ``a = log alpha`` (negative binomial; ``None``: Poisson),
+    ``dll/da`` (in column 0).  ``(l, r, q)`` are the plain family's terms, ``l = log f(y)`` without
+    ``-lgamma(y + 1)``:
+
+        y > 0:  ll = l - softplus(zeta),       dll/deta = r,       dll/dzeta = -sigmoid(zeta)
+        y = 0:  ll = logaddexp(zeta, l) - softplus(zeta),  dll/deta = w0 r,  w0 = sigmoid(l - zeta),
+                dll/dzeta = -sigmoid(zeta - l) sigmoid(-zeta) expm1(l)
+
+    and ``dll/da = q`` (y > 0) or ``w0 q`` (y = 0)."""
+    import torch
+
+    if a is None:
+        mu = torch.exp(eta)
+        l, r, q = y * eta - mu, y - mu, None
+    else:
+        l, r, q = _negative_binomial_terms(y, eta, a)
+    zero = y == 0
+    sp = torch.logaddexp(zeta, torch.zeros_like(zeta))
+    w0 = torch.where(zero, torch.sigmoid(l - zeta), torch.ones_like(l))
+    ll = torch.where(zero, torch.logaddexp(zeta, l), l) - sp
+    rz = torch.where(zero, -torch.sigmoid(zeta - l) * torch.sigmoid(-zeta) * torch.expm1(l), -torch.sigmoid(zeta))
+    pair = lambda u, v: torch.stack([u, v], dim=2)
+    out = [pair(ll, torch.zeros_like(ll)), pair(w0 * r, rz)]
+    if q is not None:
+        out.append(pair(w0 * q, torch.zeros_like(q)))
+    return out
 
 
 _DISPERSION_TERMS = {"gaussian_scale": _gaussian_scale_terms, "negative_binomial": _negative_binomial_terms,
@@ -1342,6 +1460,35 @@ def synth_negative_binomial_shard(n_rows: int, n_features: int, *, alpha: float,
         lam = torch._standard_gamma(torch.full_like(mu, float(alpha)), generator=gen) * (mu / alpha)
         y[r0:r1] = torch.poisson(lam, generator=gen).float()
     return X, y, beta_true
+
+
+def synth_zero_inflated_shard(n_rows: int, n_features: int, *, seed: int, device, alpha: Optional[float] = None,
+                              chunk_rows: int = 1 << 20, beta_scale: float = 0.05, intercept: float = 0.5,
+                              zi_intercept: float = -1.0, zi_beta_scale: float = 0.05):
+    """Synthetic zero-inflated count shard generated on the device in chunks: bf16 ``X ~ N(0,1)``, a structural zero
+    with probability ``pi = sigmoid(X zi_beta* + zi_intercept)``, else a count from ``Poisson(mu)`` (``alpha`` None)
+    or ``NegativeBinomial(mean mu, variance mu + mu^2 / alpha)`` (a gamma-Poisson mixture), ``mu = exp(X beta* +
+    intercept)``, stored as float32.  Returns ``(X, y, beta*, zi_beta*)``."""
+    import torch
+
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    zi_true = (torch.randn(n_features, generator=gen, device=device) * zi_beta_scale).float()
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        xf = xb.float()
+        lam = torch.exp(xf @ beta_true + intercept).double()
+        if alpha is not None:
+            lam = torch._standard_gamma(torch.full_like(lam, float(alpha)), generator=gen) * (lam / alpha)
+        counts = torch.poisson(lam, generator=gen)
+        zero = torch.rand(r1 - r0, generator=gen, device=device) < torch.sigmoid(xf @ zi_true + zi_intercept)
+        y[r0:r1] = torch.where(zero, torch.zeros_like(counts), counts).float()
+    return X, y, beta_true, zi_true
 
 
 def synth_ordinal_shard(n_rows: int, n_features: int, n_classes: int, *, seed: int, device, chunk_rows: int = 1 << 20,

@@ -199,12 +199,15 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 //   ZeroInflatedDisp  the zero-inflated negative binomial: ZeroInflated over negbin_loglik, with Dispersion's theta and
 //                     output layout (both theta rows of a pair end in log alpha; the table of column 2p is used, q
 //                     comes from column 2p and column 2p + 1 writes q = 0).
+//   Positive          the positive-response families with a log link to the mean (tc::gamma_loglik /
+//                     tc::inverse_gaussian_loglik): Dispersion's layout with log_dispersion = log shape; log y (and
+//                     1 / y) computed once per row and shared by its chains, the family a launch-uniform branch.
 // Column layouts follow the wgmma accumulator fragment (thread lane owns columns 8j + 2 (lane % 4) + {0, 1}), so
 // that one thread holds every term of the chains it works on.
-enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp };
+enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp, Positive };
 
 __host__ __device__ constexpr bool has_dispersion(Epi e) {
-    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp;
+    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp || e == Epi::Positive;
 }
 
 constexpr Epi epilogue(int family) {
@@ -216,11 +219,12 @@ constexpr Epi epilogue(int family) {
         case kGlmWeibull: case kGlmLogNormal: return Epi::Survival;
         case kGlmZeroInflatedPoisson: return Epi::ZeroInflated;
         case kGlmZeroInflatedNegBinomial: return Epi::ZeroInflatedDisp;
+        case kGlmGamma: case kGlmInverseGaussian: return Epi::Positive;
         default: return Epi::Scalar;
     }
 }
 static_assert([] {
-    for (int code = 0; code <= kGlmZeroInflatedNegBinomial; ++code)
+    for (int code = 0; code <= kGlmInverseGaussian; ++code)
         if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
     return true;
 }(), "the epilogue's theta and output layout must match the family's");
@@ -259,7 +263,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
     constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
-                   SURV = E == Epi::Survival, HVP = E == Epi::Hvp,
+                   SURV = E == Epi::Survival, HVP = E == Epi::Hvp, POS = E == Epi::Positive,
                    ZI = E == Epi::ZeroInflated || E == Epi::ZeroInflatedDisp, ZNB = E == Epi::ZeroInflatedDisp;
     constexpr int C8 = cfg(KC).C8;
     constexpr int N1 = cfg(KC).N1;
@@ -398,6 +402,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         if constexpr (SURV)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 survival_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
+        else if constexpr (POS)
+            for (int k = threadIdx.x; k < KC; k += blockDim.x)
+                positive_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         else if constexpr (DISP)   // families 4 and 5, and 10, whose table is family 5's (any code but 4)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
@@ -675,6 +682,14 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                             sv_event = !signbit(y);
                             sv_lt = logf(fabsf(y));
                         }
+                        // POS: log y and 1 / y of the row, shared by its chains (as in SURV, a row past the segment
+                        // reads y = 0 and is dropped below, a masked row's NaN or negative y is removed by the weight's
+                        // select); 1 / y only for the inverse Gaussian family (launch-uniform)
+                        float pv_lt = 0.f, pv_iy = 0.f;
+                        if constexpr (POS) {
+                            pv_lt = logf(y);
+                            if (prm.family == kGlmInverseGaussian) pv_iy = __frcp_rn(y);
+                        }
                         // SOFTMAX: the row's log-sum-exp per chain over the quad; every lane takes part, whether its
                         // row is valid or not (a row past the segment is dropped below, as in the other families)
                         float sm_ll[2 * NJ], sm_r[2 * NJ];
@@ -755,6 +770,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                         if constexpr (SURV) {
                                             if (prm.family == 7) weibull_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
                                             else lognormal_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
+                                        } else if constexpr (POS) {
+                                            if (prm.family == kGlmGamma) gamma_loglik(pv_lt, et, dt, ll, r, dq);
+                                            else inverse_gaussian_loglik(y, pv_lt, pv_iy, et, dt, ll, r, dq);
                                         } else {
                                             if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
                                             else negbin_loglik(y, et, dt, ll, r, dq);
@@ -966,6 +984,7 @@ LaunchFn pick(tc::Epi e, int kc, bool rows) {
         default: return pick<Epi::Scalar>(kc, rows);
         case Epi::ZeroInflated: return pick<Epi::ZeroInflated>(kc, rows);
         case Epi::ZeroInflatedDisp: return pick<Epi::ZeroInflatedDisp>(kc, rows);
+        case Epi::Positive: return pick<Epi::Positive>(kc, rows);
     }
 }
 }  // namespace

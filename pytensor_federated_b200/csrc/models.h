@@ -34,8 +34,8 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12: [.., log_dispersion])
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12: [K][G+P+1])
     int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
@@ -67,6 +67,8 @@ enum GlmFamilyCode : int {
     kGlmLogNormal = 8,       //   y = +t for an event, -t for a censored row
     kGlmZeroInflatedPoisson = 9,       // zero-inflated counts: pair p is column 2p (count eta) and 2p + 1 (zero logit
     kGlmZeroInflatedNegBinomial = 10,  //   zeta); family 10 adds NB2's log_dispersion = log alpha
+    kGlmGamma = 11,          // positive responses, log link to the mean, log_dispersion = log shape (nu, lambda):
+    kGlmInverseGaussian = 12,  //   Var(y) = mu^2 / nu (gamma), mu^3 / lambda (inverse Gaussian)
 };
 
 // How a family's columns make up n_chains: one per chain, one per chain and class (column k C + c is class c of chain
@@ -94,6 +96,8 @@ constexpr GlmFamily glm_family(int code) {
         case kGlmZeroInflatedPoisson: return {"zero_inflated_poisson", true, false, GlmColumns::kPair, 1, 1, true};
         case kGlmZeroInflatedNegBinomial:
             return {"zero_inflated_negative_binomial", true, true, GlmColumns::kPair, 1, 1, true};
+        case kGlmGamma: return {"gamma", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmInverseGaussian: return {"inverse_gaussian", true, true, GlmColumns::kOne, 1, 1, true};
         default: return {"", false, false, GlmColumns::kOne, 1, 1, true};   // 0 to 2: every GLM kernel
     }
 }

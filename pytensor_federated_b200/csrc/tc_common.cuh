@@ -10,6 +10,7 @@
 
 #include "fed_comm.cuh"
 #include "glm_link.cuh"
+#include "models.h"
 
 namespace tc {
 
@@ -578,6 +579,87 @@ __device__ __forceinline__ void lognormal_loglik(bool event, float lt, float eta
                                : 0.398942280401432678f * g / (1.f - h);      // phi(z) / Phi(-z)
     r = lam * sinv;
     q = z * lam;
+}
+
+// Positive responses with a log link to the mean (families 11 and 12): mu = e^eta, a = log_dispersion = log of the
+// shape (nu for the gamma family, lambda for the inverse Gaussian one), z = log y - eta, log y and 1 / y computed once
+// per row.  Per-chain table words, from a at setup in double:
+//   gamma:             nu, C(nu) = nu log nu - nu - lgamma(nu), Q(nu) = nu (log nu - psi(nu))
+//   inverse Gaussian:  lambda, a / 2 - log(2 pi) / 2
+// C and Q come from the Stirling series at nu' = nu + m >= 8, with the shift and series of dispersion_constants (kept
+// as a separate copy there: sharing one helper changes the SASS of the negative-binomial instantiations):
+//   C(nu) = nu (log nu - log nu') + (1/2 - m) log nu' + m - log(2 pi) / 2 - S(nu') + log prod_{j<m} (nu + j)
+//   Q(nu) = nu (log nu - log nu' - T(nu') + sum_{j<m} 1 / (nu + j))
+// (S and T as at kDwCl / kDwCd), so that for nu >= 8 (m = 0) nothing of size nu log nu is formed: C -> (log nu -
+// log 2 pi) / 2 and Q -> 1/2 as nu grows.
+constexpr int kDwShape = 0;    // nu or lambda
+constexpr int kDwC0 = 1;       // C(nu), or a / 2 - log(2 pi) / 2
+constexpr int kDwQ0 = 2;       // Q(nu) (gamma only)
+
+__device__ inline void positive_constants(int family, float ld, float* t) {
+    const double l = (double)ld;
+    const double shape = exp(l);
+    t[kDwShape] = (float)shape;
+    if (family == kGlmInverseGaussian) {
+        t[kDwC0] = (float)(0.5 * l - 0.918938533204672742);
+        return;
+    }
+    const int m = shape < 8.0 ? (int)ceil(8.0 - shape) : 0;
+    const double sp = shape + m;
+    double lp = 0.0, sr = 0.0;
+    for (int j = 0; j < m; ++j) {
+        lp += log(shape + j);
+        sr += 1.0 / (shape + j);
+    }
+    const double i1 = 1.0 / sp, i2 = i1 * i1;
+    const double S = i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260)));
+    const double T = -0.5 * i1 - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252)));
+    const double lsp = m > 0 ? log(sp) : l;   // log nu'
+    const double dl = l - lsp;                  // log nu - log nu', exactly 0 for m = 0
+    t[kDwC0] = (float)(shape * dl + (0.5 - m) * lsp + m - 0.918938533204672742 - S + lp);
+    t[kDwQ0] = (float)(shape * (dl - T + sr));
+}
+
+// Family 11 of one row, lt = log y:
+//   ll = nu g(z) + C(nu) - log y,   r = dll/deta = nu expm1(z),   q = dll/da = nu g(z) + Q(nu),   g(z) = 1 + z - e^z.
+// g(z) = z - expm1(z) loses about 2 eps / |z| of its relative accuracy near z = 0, which is where the rows sit at a
+// large shape (z ~ nu^-1/2), so below |z| = 1/2 it is the series -z^2 (1/2! + z / 3! + ... + z^6 / 8!), whose
+// truncation error there is below 2 (1/2)^7 / 9! = 4.3e-8 of g, and expm1(z) = z - g(z) (no cancellation: |g| < |z| / 3).
+// From |z| = 1/2 up, e^z - 1 and z - (e^z - 1) lose at most a few eps.  One expf per row and chain.
+__device__ __forceinline__ void gamma_loglik(float lt, float eta, const float* t, float& ll, float& r, float& q) {
+    const float nu = t[kDwShape];
+    const float z = lt - eta;
+    const float ez = expf(z);
+    float gs = fmaf(z, 1.f / 40320, 1.f / 5040);
+    gs = fmaf(z, gs, 1.f / 720);
+    gs = fmaf(z, gs, 1.f / 120);
+    gs = fmaf(z, gs, 1.f / 24);
+    gs = fmaf(z, gs, 1.f / 6);
+    gs = fmaf(z, gs, 0.5f);
+    gs = -(z * z) * gs;
+    const bool small = fabsf(z) < 0.5f;
+    const float em = small ? z - gs : ez - 1.f;
+    const float g = small ? gs : z - em;
+    const float ng = nu * g;
+    ll = (ng + t[kDwC0]) - lt;
+    r = nu * em;
+    q = ng + t[kDwQ0];
+}
+
+// Family 12 of one row, lt = log y, iy = 1 / y:
+//   ll = a / 2 - log(2 pi) / 2 - (3/2) log y - lambda expm1(z)^2 / (2 y),
+//   r = dll/deta = lambda e^-eta expm1(z) = lambda (y - mu) / mu^2,   q = dll/da = 1/2 - lambda expm1(z)^2 / (2 y).
+// expm1(z) = y e^-eta - 1 comes from one FMA (the product is not rounded before the subtraction), and expm1(z)^2 / y
+// is formed as em (em / y): em / y <= e^-eta, so nothing overflows before the result does.  One expf per row and chain.
+__device__ __forceinline__ void inverse_gaussian_loglik(float y, float lt, float iy, float eta, const float* t, float& ll,
+                                                        float& r, float& q) {
+    const float lam = t[kDwShape];
+    const float ei = expf(-eta);
+    const float em = fmaf(y, ei, -1.f);
+    const float h = 0.5f * lam * (em * (em * iy));
+    ll = (fmaf(-1.5f, lt, t[kDwC0])) - h;
+    r = lam * (ei * em);
+    q = 0.5f - h;
 }
 
 

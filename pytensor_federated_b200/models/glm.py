@@ -9,7 +9,7 @@ Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
 
 How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
 oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
-``_Ordinal``, ``_Survival``, ``_Hvp``, ``_ZeroInflated`` below); :class:`GlmShards` and its callers are generic over it.
+``_Ordinal``, ``_Survival``, ``_Positive``, ``_Hvp``, ``_ZeroInflated`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -22,7 +22,8 @@ import numpy as np
 from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
-            "ordinal": 6, "weibull": 7, "lognormal": 8, "zero_inflated_poisson": 9, "zero_inflated_negative_binomial": 10}
+            "ordinal": 6, "weibull": 7, "lognormal": 8, "zero_inflated_poisson": 9, "zero_inflated_negative_binomial": 10,
+            "gamma": 11, "inverse_gaussian": 12}
 
 
 #: dynamic shared memory one CTA may opt in to on the H100 (227 KB), less 256 bytes for a kernel's static variables
@@ -189,6 +190,26 @@ class GlmShards(ShardModel):
         every family.  Only the bf16 tensor-core kernel evaluates these families, with the shape limits of the
         multinomial one; ``n_classes``, ``events`` and ``hvp`` are rejected, and so is a shape whose 2K-column
         launch gets fewer than two pipeline stages (checked when an engine attaches the model).
+
+        ``"gamma"`` and ``"inverse_gaussian"`` are regression for positive, right-skewed continuous responses with a
+        model for the MEAN (R's ``Gamma(link="log")`` / ``inverse.gaussian(link="log")``, brms' ``Gamma`` /
+        ``inverse.gaussian``, PyMC's ``Gamma`` / ``Wald``): claim severities, costs, incomes, amounts, concentrations,
+        durations.  The inputs and gradients are those of ``negative_binomial``: ``(intercept, beta,
+        log_dispersion)``, one chain or batched.  With ``eta = intercept[group] + x' beta + o``, ``mu = e^eta`` is the
+        mean of y, and ``a = log_dispersion`` is the log of the SHAPE (a larger shape, less dispersion, as ``log
+        alpha`` of the negative binomial).  With ``z = log y - eta``:
+
+            gamma, nu = e^a, Var(y) = mu^2 / nu:
+                ll = nu (1 + z - e^z) + nu log nu - nu - lgamma(nu) - log y
+            inverse_gaussian, lambda = e^a, Var(y) = mu^3 / lambda:
+                ll = a / 2 - log(2 pi) / 2 - (3/2) log y - lambda (y - mu)^2 / (2 mu^2 y)
+
+        LL is the full density, ``-log y`` terms included, so it equals ``scipy.stats.gamma(a=nu, scale=mu /
+        nu).logpdf(y)`` and ``scipy.stats.invgauss(mu=mu / lambda, scale=lambda).logpdf(y)``.  At ``a = 0`` the gamma
+        family is the exponential distribution with mean mu.  Responses must be finite and > 0 on every row of
+        non-zero weight (a row of weight 0 may carry any y); offsets and weights work as for every family.  Only the
+        bf16 tensor-core kernel evaluates these families, with the shape limits of the multinomial one;
+        ``n_classes``, ``events`` and ``hvp`` are rejected.
     events
         Per-row event indicators of the survival families (see ``family``).
     hvp
@@ -758,6 +779,18 @@ def _check_integers(m, what: str, valid: str, below) -> None:
             raise ValueError(f"{what} of segment {si} must be integers in {valid} on every row of non-zero weight")
 
 
+def _check_positive(m, what: str) -> None:
+    """Every row of non-zero weight holds a finite y > 0."""
+    import torch
+
+    for si, (y, w) in enumerate(zip(m.ys, m.weights)):
+        bad = ~(torch.isfinite(y) & (y > 0))   # NaN fails the comparison
+        if w is not None:
+            bad &= w != 0   # a masked row may carry anything
+        if bool(torch.any(bad)):
+            raise ValueError(f"{what} of segment {si} must be finite and > 0 on every row of non-zero weight")
+
+
 def _labels(y, w):
     """Integer labels of a chunk; masked rows may carry NaN or out-of-range labels: any valid class will do."""
     import torch
@@ -964,18 +997,26 @@ class _Survival(_Dispersion):
         import torch
 
         super().__init__(m, n_classes)
+        _check_positive(m, "times")
         signed = []
         for si, (t, ev, w) in enumerate(zip(m.ys, m.events, m.weights)):
-            keep = torch.ones_like(t, dtype=torch.bool) if w is None else w != 0   # a masked row may carry anything
-            if bool(torch.any(keep & ~(torch.isfinite(t) & (t > 0)))):
-                raise ValueError(f"times of segment {si} must be finite and > 0 on every row of non-zero weight")
             if ev is None:
                 signed.append(t)
                 continue
+            keep = torch.ones_like(t, dtype=torch.bool) if w is None else w != 0   # a masked row may carry anything
             if bool(torch.any(keep & ~((ev == 0) | (ev == 1)))):
                 raise ValueError(f"events of segment {si} must be 0 or 1 on every row of non-zero weight")
             signed.append(_aligned16(torch.where(ev == 0, -t, t).contiguous()))
         self.kernel_ys = signed
+
+
+class _Positive(_Dispersion):
+    """``gamma`` and ``inverse_gaussian``: the layout of :class:`_Dispersion` with ``log_dispersion`` the log of the
+    shape (nu, lambda).  Every row of non-zero weight must hold a finite y > 0."""
+
+    def __init__(self, m, n_classes) -> None:
+        super().__init__(m, n_classes)
+        _check_positive(m, "responses")
 
 
 class _Softmax(_Layout):
@@ -1177,7 +1218,8 @@ class _ZeroInflated(_Layout):
 
 _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_binomial": _Dispersion,
             "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival,
-            "zero_inflated_poisson": _ZeroInflated, "zero_inflated_negative_binomial": _ZeroInflated}
+            "zero_inflated_poisson": _ZeroInflated, "zero_inflated_negative_binomial": _ZeroInflated,
+            "gamma": _Positive, "inverse_gaussian": _Positive}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -1264,6 +1306,69 @@ def _lognormal_terms(y, eta, s):
     return ll, r, q
 
 
+#: 1 / k! for k = 2 .. 16: the series of -g(z) / z^2, g(z) = 1 + z - e^z, to a truncation error below 1e-17 of g at
+#: |z| < 1/2
+_G_SERIES = [1.0 / float(np.prod(np.arange(1, k + 1))) for k in range(2, 17)]
+
+
+def _gamma_g(z):
+    """``g(z) = 1 + z - e^z``, relatively accurate near z = 0 (where ``z - expm1(z)`` loses ``2 eps / |z|``): a power
+    series below |z| = 1/2, ``z - expm1(z)`` above."""
+    import torch
+
+    small = z.abs() < 0.5
+    zs = torch.where(small, z, torch.zeros_like(z))
+    acc = torch.full_like(z, _G_SERIES[-1])
+    for c in reversed(_G_SERIES[:-1]):
+        acc = acc * zs + c
+    return torch.where(small, -(zs * zs) * acc, z - torch.expm1(z))
+
+
+def _gamma_shape_terms(a):
+    """``(nu, C(nu), Q(nu))`` per chain in float64: ``C = nu log nu - nu - lgamma(nu)`` and ``Q = nu (log nu -
+    psi(nu))``, from their Stirling series at nu >= 1e3 (truncation error < 1e-24), where the direct forms would
+    subtract values of size nu log nu.  Both stay O(1): ``C -> (a - log 2 pi) / 2``, ``Q -> 1/2``."""
+    import torch
+
+    a = a.double()
+    nu = torch.exp(a)
+    big = nu >= 1e3
+    nb = torch.where(big, nu, torch.full_like(nu, 1e3))
+    ns = torch.where(big, torch.ones_like(nu), nu)
+    i2 = 1.0 / (nb * nb)
+    S = (1.0 / 12 - i2 * (1.0 / 360 - i2 / 1260)) / nb
+    T = -0.5 / nb - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 / 252))
+    C = torch.where(big, 0.5 * a - _LOG_SQRT_2PI - S, ns * torch.log(ns) - ns - torch.lgamma(ns))
+    Q = torch.where(big, -nb * T, ns * (torch.log(ns) - torch.digamma(ns)))
+    return nu, C, Q
+
+
+def _gamma_terms(y, eta, a):
+    """``(ll, dll/deta, dll/da)`` of the gamma family with mean ``mu = exp(eta)`` and shape ``nu = exp(a)``:
+    ``ll = nu g(z) + C(nu) - log y``, ``dll/deta = nu expm1(z)``, ``dll/da = nu g(z) + Q(nu)`` with ``z = log y -
+    eta`` (:func:`_gamma_g`, :func:`_gamma_shape_terms`; the shape's terms in float64 whatever the dtype)."""
+    import torch
+
+    nu, C, Q = (v.to(eta.dtype) for v in _gamma_shape_terms(a))
+    lt = torch.log(y)
+    z = lt - eta
+    ng = nu * _gamma_g(z)
+    return ng + C - lt, nu * torch.expm1(z), ng + Q
+
+
+def _inverse_gaussian_terms(y, eta, a):
+    """``(ll, dll/deta, dll/da)`` of the inverse Gaussian family with mean ``mu = exp(eta)`` and shape ``lambda =
+    exp(a)``: with ``h = lambda expm1(z)^2 / (2 y)`` (= lambda (y - mu)^2 / (2 mu^2 y)), ``ll = a / 2 - log(2 pi) / 2 -
+    (3/2) log y - h``, ``dll/deta = lambda e^-eta expm1(z)``, ``dll/da = 1/2 - h``."""
+    import torch
+
+    lam = torch.exp(a)
+    lt = torch.log(y)
+    em = torch.expm1(lt - eta)
+    h = 0.5 * lam * em * (em / y)
+    return 0.5 * a - _LOG_SQRT_2PI - 1.5 * lt - h, lam * torch.exp(-eta) * em, 0.5 - h
+
+
 def _zero_inflated_terms(y, eta, zeta, a=None):
     """The per-row terms of a zero-inflated count model, ``[n, K, 2]`` (column 0: eta, 1: zeta): ``ll`` (in column 0,
     0 in column 1), ``(dll/deta, dll/dzeta)`` and, with ``a = log alpha`` (negative binomial; ``None``: Poisson),
@@ -1295,7 +1400,8 @@ def _zero_inflated_terms(y, eta, zeta, a=None):
 
 
 _DISPERSION_TERMS = {"gaussian_scale": _gaussian_scale_terms, "negative_binomial": _negative_binomial_terms,
-                     "weibull": _weibull_terms, "lognormal": _lognormal_terms}
+                     "weibull": _weibull_terms, "lognormal": _lognormal_terms, "gamma": _gamma_terms,
+                     "inverse_gaussian": _inverse_gaussian_terms}
 
 
 def quantize_block_fp8(X, block: int = 32):
@@ -1561,6 +1667,57 @@ def synth_survival_shard(n_rows: int, n_features: int, *, family: str, sigma: fl
         time[r0:r1] = torch.exp(torch.where(ev, log_t, log_c)).float()
         event[r0:r1] = ev.float()
     return X, time, event, beta_true
+
+
+def _check_positive_args(family: str, shape: float) -> None:
+    if family not in ("gamma", "inverse_gaussian"):
+        raise ValueError(f"family must be 'gamma' or 'inverse_gaussian', got {family!r}")
+    if not shape > 0:
+        raise ValueError(f"shape must be > 0, got {shape}")
+
+
+def draw_positive(mu, *, family: str, shape: float, generator):
+    """float32 draws with mean ``mu`` (a float64 tensor) and shape ``shape``: ``Gamma(shape, scale mu / shape)``
+    (``family="gamma"``) or inverse Gaussian ``IG(mu, lambda = shape)`` (``"inverse_gaussian"``, Michael-Schucany-Haas:
+    with ``n ~ N(0, 1)`` and ``c = mu n^2 / (2 lambda)``, the smaller root ``x = mu / (1 + c + sqrt(c (2 + c)))``, free
+    of cancellation, taken with probability ``mu / (mu + x)``, else ``mu^2 / x``), drawn in float64 and clamped into
+    the positive finite float32 range."""
+    import torch
+
+    _check_positive_args(family, shape)
+    if family == "gamma":
+        v = torch._standard_gamma(torch.full_like(mu, float(shape)), generator=generator) * (mu / shape)
+    else:
+        n = torch.randn(mu.shape, generator=generator, device=mu.device, dtype=torch.float64)
+        c = mu * n * n / (2.0 * shape)
+        x = mu / (1.0 + c + torch.sqrt(c * (2.0 + c)))
+        u = torch.rand(mu.shape, generator=generator, device=mu.device, dtype=torch.float64)
+        v = torch.where(u * (mu + x) <= mu, x, mu * mu / x)
+    fi = torch.finfo(torch.float32)
+    return v.clamp(fi.tiny, fi.max).float()
+
+
+def synth_positive_shard(n_rows: int, n_features: int, *, family: str, shape: float, seed: int, device,
+                         chunk_rows: int = 1 << 20, beta_scale: float = 0.05, intercept: float = 0.5):
+    """Synthetic positive-response shard generated on the device in chunks: bf16 ``X ~ N(0,1)`` and y with mean
+    ``mu = exp(X beta* + intercept)`` and shape ``shape``: ``Gamma(shape, scale mu / shape)`` (``family="gamma"``) or
+    inverse Gaussian ``IG(mu, lambda = shape)`` (``"inverse_gaussian"``, Michael-Schucany-Haas in a cancellation-free
+    form), drawn in float64 by :func:`draw_positive` and stored as float32 > 0.  Returns ``(X, y, beta*)``."""
+    import torch
+
+    _check_positive_args(family, shape)
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        mu = torch.exp(xb.float() @ beta_true + intercept).double()
+        y[r0:r1] = draw_positive(mu, family=family, shape=shape, generator=gen)
+    return X, y, beta_true
 
 
 def synth_logistic_shard_fp8(n_rows: int, n_features: int, *, seed: int, device, chunk_rows: int = 1 << 20):

@@ -6,11 +6,15 @@ the rest of the kernel's per-tile chain (wait -> MMA #1 -> epilogue -> barrier -
 faster than the HBM stream.  This script measures that chain on its own: a model of the same row count whose
 segments all point at one 32K x 256 bf16 matrix (16 MB, resident in the 50 MB L2), so X costs almost no HBM
 traffic, timed in windows that alternate with the flagship shape in one process: read as bf16 (``bf16``, as with
-``B200FED_NO_PACKED_X=1``) and in its packed form (``packed``), the two checked to compute the same bits.
+``B200FED_NO_PACKED_X=1``) and in its packed form (``packed``), the two checked to compute the same bits.  The same
+L2-resident model is also read packed (``l2-packed``): all its segments share one packed copy of the matrix (about
+12 MB), so it measures the packed kernel's on-chip ceiling (decode, hand-off and consumer chain) without the HBM
+stream; it is checked bitwise against ``l2``.  ``l2-packed`` well above ``packed`` means the HBM stream binds the
+packed kernel; close to it, the on-chip chain does.
 
-Prints one JSON line: device-timed evaluations/s of the three models, the rows/s of each, the bytes each reads per
-evaluation over its time, the packed / bf16 and l2 / bf16 ratios, and the card's name, power limit and NVML-sampled
-SM clock.
+Prints one JSON line: device-timed evaluations/s of the four models, the rows/s of each, the bytes each reads per
+evaluation over its time, the packed / bf16, l2 / bf16 and packed / l2-packed ratios, and the card's name, power limit
+and NVML-sampled SM clock.
 
     python benchmarks/bench_glm_packed.py [--shards 8] [--rows 10000000] [--features 256] [--chains 1] [--steps 30]
                                           [--rounds 5] [--no-l2]
@@ -46,6 +50,7 @@ def main() -> None:
     from bench import ClockSampler
     from benchmarks.bench_glm_row_data import card_info
     from pytensor_federated_b200.models import GlmShards, synth_logistic_shard
+    from pytensor_federated_b200.models.glm import pack_x12
     from pytensor_federated_b200.parallel import FederatedEngine
 
     dev = torch.device("cuda:0")
@@ -64,6 +69,11 @@ def main() -> None:
     if not args.no_l2:
         X2, y2, _ = synth_logistic_shard(args.l2_rows, P, seed=77, device=dev)
         models["l2"] = GlmShards([X2] * n_l2, [y2] * n_l2, kernel="tc", n_chains=K)
+        # one packed copy for every segment, as the bf16 segments share one matrix: packing each segment on its own
+        # would make n_l2 copies (29 GB at the flagship shape), which would not stay in L2
+        models["l2-packed"] = GlmShards([X2] * n_l2, [y2] * n_l2, kernel="tc", n_chains=K)
+        models["l2-packed"]._packs = [pack_x12(X2)] * n_l2
+    packed_models = ("packed", "l2-packed")
     torch.cuda.synchronize()
     rows = {k: m.n_rows for k, m in models.items()}
     rng = np.random.default_rng(7)
@@ -76,7 +86,7 @@ def main() -> None:
     saved = os.environ.get("B200FED_NO_PACKED_X")
     try:
         for k, m in models.items():   # the switch is read when an engine attaches the model
-            os.environ["B200FED_NO_PACKED_X"] = "0" if k == "packed" else "1"
+            os.environ["B200FED_NO_PACKED_X"] = "0" if k in packed_models else "1"
             engines[k] = FederatedEngine(m)
     finally:
         if saved is None:
@@ -84,19 +94,25 @@ def main() -> None:
         else:
             os.environ["B200FED_NO_PACKED_X"] = saved
     result = {"config": f"{args.shards} x {args.rows} x {P} bf16 logistic (bf16, packed)"
-                        + ("" if args.no_l2 else f" against {n_l2} x {args.l2_rows} x {P} segments of one matrix (l2)")
+                        + ("" if args.no_l2 else f" against {n_l2} x {args.l2_rows} x {P} segments of one matrix "
+                                                 "(l2, l2-packed)")
                         + f", tc kernel, K = {K}, 1 GPU",
               "steps": args.steps, "rounds": args.rounds}
     try:
-        # both models must compute what the oracle computes before their times mean anything
-        assert models["packed"].packed_x and not any(m.packed_x for k, m in models.items() if k != "packed")
-        raw = {k: np.asarray(engines[k].evaluate_raw(list(theta)), dtype=np.float64) for k in ("bf16", "packed")}
-        result["packed_bitwise_equal"] = raw["bf16"].tobytes() == raw["packed"].tobytes()
-        if not result["packed_bitwise_equal"]:
-            print(json.dumps({"error": "packed and bf16 results differ"}), flush=True)
-            raise SystemExit(1)
+        # every model must compute what the oracle computes before its time means anything; a packed model, the bits
+        # of its bf16 twin
+        assert all(m.packed_x == (k in packed_models) for k, m in models.items())
+        raw = {k: np.asarray(engines[k].evaluate_raw(list(theta)), dtype=np.float64) for k in models}
+        for pk, twin in (("packed", "bf16"), ("l2-packed", "l2")):
+            if pk not in models:
+                continue
+            key = "packed_bitwise_equal" if pk == "packed" else "l2_packed_bitwise_equal"
+            result[key] = raw[twin].tobytes() == raw[pk].tobytes()
+            if not result[key]:
+                print(json.dumps({"error": f"{pk} and {twin} results differ"}), flush=True)
+                raise SystemExit(1)
         for k, m in models.items():
-            if k == "packed":
+            if k in packed_models:
                 continue
             assert m.selected_kernel == "tc"
             got = np.asarray(engines[k].evaluate_raw(list(theta)), dtype=np.float64)
@@ -146,6 +162,7 @@ def main() -> None:
     # rows per second, so that the l2 model's slightly different row count does not bias the ratio
     if "l2" in models:
         result["l2_over_bf16_rows_per_s"] = round(result["l2_grows_per_s"] / result["bf16_grows_per_s"], 4)
+        result["packed_over_l2_packed_rows_per_s"] = round(result["packed_grows_per_s"] / result["l2-packed_grows_per_s"], 4)
     print(json.dumps(result), flush=True)
 
 

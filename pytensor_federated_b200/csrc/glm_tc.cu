@@ -514,6 +514,10 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             // once all 96 threads' stores are in, and arrive on full[stage] after a proxy fence.
             if (PK) {
                 const int td = threadIdx.x - 32;
+                // panels per load group: 2 where the registers it needs do not push the instantiation into spills
+                // (ptxas -v; the consumers' epilogue sets the register count), else 1
+                constexpr int kDecGroup = KC <= 4 && !ORD ? 2 : 1;
+                static_assert(kDecGroup <= 2, "a packed launch may have only 2 compressed slots");
                 int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
                 Ring stage, xs;
                 uint32_t fb = 0;
@@ -532,37 +536,48 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                         mbar_wait(&bar_empty[stage.idx], stage.phase ^ 1);
                         unsigned char* dst = smem + (size_t)stage.idx * L.stage_bytes;
                         int* foot = reinterpret_cast<int*>(smem + L.off_xfoot + fb * kXFoot);
-                        for (int pnl = 0; pnl < panels; ++pnl) {
-                            mbar_wait(&bar_xfull[xs.idx], xs.phase);
-                            const unsigned char* src = smem + L.off_x + (size_t)xs.idx * L.xslot_bytes;
-                            if (pnl == 0) {
-                                if (td < kXFoot / 4) foot[td] = reinterpret_cast<const int*>(src + kXBlock)[td];
-                                const float* rsrc = reinterpret_cast<const float*>(src + kXBlock + kXFoot);
-                                float* rdst = reinterpret_cast<float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
-                                for (int i = td; i < (int)L.row_bytes / 4; i += kDecThreads) rdst[i] = rsrc[i];
-                            }
-                            // all of this thread's loads of the panel first, then the decodes and stores: one warp
-                            // per scheduler runs this, so the shared-memory latency is hidden by ILP, not by warps
-                            unsigned char* pd = dst + pnl * kPanelBytes;
+                        // panels in groups of kDecGroup: all of this thread's loads of a group's panels first, then
+                        // their decodes and stores.  One warp per scheduler runs this, so the shared-memory latency is
+                        // hidden by ILP, not by warps: a group keeps kDecGroup panels of loads in flight.  A group holds
+                        // kDecGroup slots at once: a packed launch has at least 2 slots (launch() refuses fewer) and 2 or
+                        // 4 panels, so a group of 2 always fits and divides the tile.
+                        for (int pnl = 0; pnl < panels; pnl += kDecGroup) {
                             constexpr int kPer = (kTileM * 8 + kDecThreads - 1) / kDecThreads;
-                            uint2 lo[kPer];
-                            uint32_t cw[kPer];
+                            uint2 lo[kDecGroup][kPer];
+                            uint32_t cw[kDecGroup][kPer];
+                            int xi[kDecGroup];
 #pragma unroll
-                            for (int k = 0; k < kPer; ++k) {
-                                const int i = td + k * kDecThreads;
-                                if (k < kPer - 1 || i < kTileM * 8) {
-                                    lo[k] = reinterpret_cast<const uint2*>(src)[i];
-                                    cw[k] = reinterpret_cast<const uint32_t*>(src + kTileM * kPanel)[i];
+                            for (int h = 0; h < kDecGroup; ++h) {
+                                mbar_wait(&bar_xfull[xs.idx], xs.phase);
+                                const unsigned char* src = smem + L.off_x + (size_t)xs.idx * L.xslot_bytes;
+                                if (pnl + h == 0) {
+                                    if (td < kXFoot / 4) foot[td] = reinterpret_cast<const int*>(src + kXBlock)[td];
+                                    const float* rsrc = reinterpret_cast<const float*>(src + kXBlock + kXFoot);
+                                    float* rdst = reinterpret_cast<float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
+                                    for (int i = td; i < (int)L.row_bytes / 4; i += kDecThreads) rdst[i] = rsrc[i];
                                 }
+#pragma unroll
+                                for (int k = 0; k < kPer; ++k) {
+                                    const int i = td + k * kDecThreads;
+                                    if (k < kPer - 1 || i < kTileM * 8) {
+                                        lo[h][k] = reinterpret_cast<const uint2*>(src)[i];
+                                        cw[h][k] = reinterpret_cast<const uint32_t*>(src + kTileM * kPanel)[i];
+                                    }
+                                }
+                                xi[h] = xs.idx;
+                                xs.advance((int)L.xslots);
                             }
 #pragma unroll
-                            for (int k = 0; k < kPer; ++k) {
-                                const int i = td + k * kDecThreads;
-                                if (k < kPer - 1 || i < kTileM * 8)
-                                    *reinterpret_cast<uint4*>(pd + x12_chunk_offset(i)) = x12_decode8(lo[k], cw[k], tab);
+                            for (int h = 0; h < kDecGroup; ++h) {
+                                unsigned char* pd = dst + (pnl + h) * kPanelBytes;
+#pragma unroll
+                                for (int k = 0; k < kPer; ++k) {
+                                    const int i = td + k * kDecThreads;
+                                    if (k < kPer - 1 || i < kTileM * 8)
+                                        *reinterpret_cast<uint4*>(pd + x12_chunk_offset(i)) = x12_decode8(lo[h][k], cw[h][k], tab);
+                                }
+                                mbar_arrive(&bar_xempty[xi[h]]);
                             }
-                            mbar_arrive(&bar_xempty[xs.idx]);
-                            xs.advance((int)L.xslots);
                         }
                         named_sync(2, kDecThreads);   // the tile's decoded chunks and its footer are in
                         const int n_ex = min(foot[0], kXMaxExceptions);
@@ -648,6 +663,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                     for (int v = 0; v < N1 / 2; ++v) eacc[v] = 0.f;
                     wgmma_fence();
+                    // not unrolled: nvcc's unrolled copies of this runtime-bound loop move accumulator registers
+                    // between the wgmmas, and ptxas then waits for each wgmma before issuing the next (C7515)
+#pragma unroll 1
                     for (int pnl = 0; pnl < panels; ++pnl) {
 #pragma unroll
                         for (int ks = 0; ks < kPanel / 16; ++ks) {

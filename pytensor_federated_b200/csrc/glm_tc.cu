@@ -202,12 +202,28 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 //   Positive          the positive-response families with a log link to the mean (tc::gamma_loglik /
 //                     tc::inverse_gaussian_loglik): Dispersion's layout with log_dispersion = log shape; log y (and
 //                     1 / y) computed once per row and shared by its chains, the family a launch-uniform branch.
+//   LocationScale     the Gaussian location-scale family (tc::location_scale_loglik): ZeroInflated's pair plumbing,
+//                     with column 2p the mean mu (theta row (intercept, beta), the only one that takes the offset) and
+//                     column 2p + 1 s = log sigma (theta row (sigma_intercept, sigma_beta)); column 2p gets ll and
+//                     dll/dmu, column 2p + 1 ll = 0 and dll/ds.  No KC = 1 instance.
+//   StudentT          the Student-t family (tc::student_t_loglik): LocationScale with ZeroInflatedDisp's theta and
+//                     output layout (both theta rows of a pair end in log nu; the table of column 2p is used, q =
+//                     dll/dlog_nu comes from column 2p and column 2p + 1 writes q = 0).
 // Column layouts follow the wgmma accumulator fragment (thread lane owns columns 8j + 2 (lane % 4) + {0, 1}), so
 // that one thread holds every term of the chains it works on.
-enum class Epi { Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp, Positive };
+enum class Epi {
+    Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp, Positive, LocationScale, StudentT
+};
 
 __host__ __device__ constexpr bool has_dispersion(Epi e) {
-    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp || e == Epi::Positive;
+    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp || e == Epi::Positive ||
+           e == Epi::StudentT;
+}
+
+// The epilogues whose chain k is the column pair (2k, 2k + 1), both predictors formed in one thread before either
+// column's values (Hvp pairs its columns too, but evaluates them one at a time)
+__host__ __device__ constexpr bool pair_epilogue(Epi e) {
+    return e == Epi::ZeroInflated || e == Epi::ZeroInflatedDisp || e == Epi::LocationScale || e == Epi::StudentT;
 }
 
 constexpr Epi epilogue(int family) {
@@ -220,11 +236,13 @@ constexpr Epi epilogue(int family) {
         case kGlmZeroInflatedPoisson: return Epi::ZeroInflated;
         case kGlmZeroInflatedNegBinomial: return Epi::ZeroInflatedDisp;
         case kGlmGamma: case kGlmInverseGaussian: return Epi::Positive;
+        case kGlmGaussianLocationScale: return Epi::LocationScale;
+        case kGlmStudentT: return Epi::StudentT;
         default: return Epi::Scalar;
     }
 }
 static_assert([] {
-    for (int code = 0; code <= kGlmInverseGaussian; ++code)
+    for (int code = 0; code <= kGlmStudentT; ++code)
         if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
     return true;
 }(), "the epilogue's theta and output layout must match the family's");
@@ -264,7 +282,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
     constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
                    SURV = E == Epi::Survival, HVP = E == Epi::Hvp, POS = E == Epi::Positive,
-                   ZI = E == Epi::ZeroInflated || E == Epi::ZeroInflatedDisp, ZNB = E == Epi::ZeroInflatedDisp;
+                   PAIR = pair_epilogue(E), ZNB = E == Epi::ZeroInflatedDisp, STT = E == Epi::StudentT;
     constexpr int C8 = cfg(KC).C8;
     constexpr int N1 = cfg(KC).N1;
     constexpr int N2 = cfg(KC).N2;
@@ -405,6 +423,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         else if constexpr (POS)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 positive_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
+        else if constexpr (STT)
+            for (int k = threadIdx.x; k < KC; k += blockDim.x)
+                student_t_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         else if constexpr (DISP)   // families 4 and 5, and 10, whose table is family 5's (any code but 4)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
@@ -747,11 +768,11 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc) {
                             float hv_h = 0.f;   // HVP: h = d2ll / deta2 of the pair's theta column (e = 0), for e = 1
-                            // ZI: the pair's values (columns k0 = 8 jc + 2 q and k0 + 1), from both predictors, before
-                            // the column loop; offset and weight as in ROWS (the offset to eta only).  n_chains is even,
-                            // so k0 < nch covers both columns.
-                            float zi_ll = 0.f, zi_rc = 0.f, zi_rz = 0.f, zi_q = 0.f;
-                            if constexpr (ZI) {
+                            // PAIR: the pair's values (columns k0 = 8 jc + 2 q and k0 + 1), from both predictors, before
+                            // the column loop; offset and weight as in ROWS (the offset to the first predictor only).
+                            // n_chains is even, so k0 < nch covers both columns.
+                            float pr_ll = 0.f, pr_r0 = 0.f, pr_r1 = 0.f, pr_q = 0.f;
+                            if constexpr (PAIR) {
                                 const int k0 = 8 * jc + 2 * q;
                                 if (valid && k0 < nch) {
                                     float et = ((eacc[4 * jc + 2 * h] + eacc[4 * (NJ + jc) + 2 * h]) +
@@ -759,12 +780,17 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                     if constexpr (ROWS) et = __fadd_rn(et, o);
                                     const float zt = ((eacc[4 * jc + 2 * h + 1] + eacc[4 * (NJ + jc) + 2 * h + 1]) +
                                                       eacc[4 * (2 * NJ + jc) + 2 * h + 1]) + icpt[k0 + 1];
-                                    zero_inflated_loglik<ZNB>(y, et, zt, disp + k0 * kDispWords, zi_ll, zi_rc, zi_rz, zi_q);
+                                    if constexpr (E == Epi::LocationScale)
+                                        location_scale_loglik(y, et, zt, pr_ll, pr_r0, pr_r1);
+                                    else if constexpr (STT)
+                                        student_t_loglik(y, et, zt, disp + k0 * kDispWords, pr_ll, pr_r0, pr_r1, pr_q);
+                                    else
+                                        zero_inflated_loglik<ZNB>(y, et, zt, disp + k0 * kDispWords, pr_ll, pr_r0, pr_r1, pr_q);
                                     if constexpr (ROWS) {
-                                        apply_weight(wt, zi_ll);
-                                        apply_weight(wt, zi_rc);
-                                        apply_weight(wt, zi_rz);
-                                        apply_weight(wt, zi_q);
+                                        apply_weight(wt, pr_ll);
+                                        apply_weight(wt, pr_r0);
+                                        apply_weight(wt, pr_r1);
+                                        apply_weight(wt, pr_q);
                                     }
                                 }
                             }
@@ -775,11 +801,12 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
                                 float ll = 0.f, r = 0.f, dq = 0.f;
                                 if (valid && k < nch) {
-                                    if constexpr (ZI) {
-                                        // column 2p: the pair's ll, dll/deta (and dll/dlog_alpha); 2p + 1: dll/dzeta
-                                        ll = e == 0 ? zi_ll : 0.f;
-                                        r = e == 0 ? zi_rc : zi_rz;
-                                        dq = e == 0 ? zi_q : 0.f;
+                                    if constexpr (PAIR) {
+                                        // column 2p: the pair's ll, the first predictor's r (and dll/dlog_dispersion);
+                                        // 2p + 1: the second predictor's r
+                                        ll = e == 0 ? pr_ll : 0.f;
+                                        r = e == 0 ? pr_r0 : pr_r1;
+                                        dq = e == 0 ? pr_q : 0.f;
                                     } else if constexpr (DISP) {
                                         // offset and weight as in ROWS, the weight applied to all three values
                                         float et = eta + icpt[k];
@@ -975,16 +1002,14 @@ int launch(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm
                           n_chunks, work_counter);
 }
 
-// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax, Hvp and the zero-inflated ones (two
+// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax, Hvp and the pair epilogues (two
 // columns at least) in KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are
 // instantiated, which is the order of the cases here: later epilogues go after the default.
 template <tc::Epi E>
 LaunchFn pick(int kc, bool rows) {
     switch (kc) {
         case 1:
-            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp || E == tc::Epi::ZeroInflated ||
-                          E == tc::Epi::ZeroInflatedDisp)
-                return nullptr;
+            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp || tc::pair_epilogue(E)) return nullptr;
             else return rows ? launch<1, true, E> : launch<1, false, E>;
         case 4: return rows ? launch<4, true, E> : launch<4, false, E>;
         case 8: return rows ? launch<8, true, E> : launch<8, false, E>;
@@ -1003,6 +1028,8 @@ LaunchFn pick(tc::Epi e, int kc, bool rows) {
         case Epi::ZeroInflated: return pick<Epi::ZeroInflated>(kc, rows);
         case Epi::ZeroInflatedDisp: return pick<Epi::ZeroInflatedDisp>(kc, rows);
         case Epi::Positive: return pick<Epi::Positive>(kc, rows);
+        case Epi::LocationScale: return pick<Epi::LocationScale>(kc, rows);
+        case Epi::StudentT: return pick<Epi::StudentT>(kc, rows);
     }
 }
 }  // namespace

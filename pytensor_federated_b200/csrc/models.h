@@ -34,8 +34,8 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12, 14: [.., log_dispersion])
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12, 14: [K][G+P+1])
     int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
@@ -69,11 +69,14 @@ enum GlmFamilyCode : int {
     kGlmZeroInflatedNegBinomial = 10,  //   zeta); family 10 adds NB2's log_dispersion = log alpha
     kGlmGamma = 11,          // positive responses, log link to the mean, log_dispersion = log shape (nu, lambda):
     kGlmInverseGaussian = 12,  //   Var(y) = mu^2 / nu (gamma), mu^3 / lambda (inverse Gaussian)
+    kGlmGaussianLocationScale = 13,  // location-scale: pair p is column 2p (mean mu, identity link) and 2p + 1
+    kGlmStudentT = 14,               //   (log sigma); family 14 adds log_dispersion = log nu
 };
 
 // How a family's columns make up n_chains: one per chain, one per chain and class (column k C + c is class c of chain
 // k), one per chain and cutpoint (column k (C - 1) + j is cutpoint j of chain k), for C = n_classes, or two per chain
-// (column 2k and 2k + 1: the zero-inflated families' count and zero predictors)
+// (column 2k and 2k + 1: the zero-inflated families' count and zero predictors, the location-scale families' mean and
+// log sigma)
 enum class GlmColumns { kOne, kPerClass, kPerCutpoint, kPair };
 
 // What the runtime and the bf16 tensor-core kernel need to know about a family code.
@@ -98,6 +101,9 @@ constexpr GlmFamily glm_family(int code) {
             return {"zero_inflated_negative_binomial", true, true, GlmColumns::kPair, 1, 1, true};
         case kGlmGamma: return {"gamma", true, true, GlmColumns::kOne, 1, 1, true};
         case kGlmInverseGaussian: return {"inverse_gaussian", true, true, GlmColumns::kOne, 1, 1, true};
+        case kGlmGaussianLocationScale:
+            return {"gaussian_location_scale", true, false, GlmColumns::kPair, 1, 1, true};
+        case kGlmStudentT: return {"student_t", true, true, GlmColumns::kPair, 1, 1, true};
         default: return {"", false, false, GlmColumns::kOne, 1, 1, true};   // 0 to 2: every GLM kernel
     }
 }

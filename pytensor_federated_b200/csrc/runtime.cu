@@ -603,7 +603,7 @@ int b200_engine_set_glm(void* h, int n_segments, const void** X, const float** y
         }
         if (f.columns == GlmColumns::kPair && (n_chains < 2 || n_chains > 16 || n_chains % 2 != 0)) {
             g_last_error = std::string("the ") + f.name +
-                           " family needs an even n_chains in [2, 16] (a count and a zero-inflation column per chain)";
+                           " family needs an even n_chains in [2, 16] (two columns per chain)";
             return -44;
         }
         for (int s = 0; s < n_segments && offsets && !f.offsets; ++s)

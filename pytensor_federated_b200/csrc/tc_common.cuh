@@ -662,5 +662,117 @@ __device__ __forceinline__ void inverse_gaussian_loglik(float y, float lt, float
     q = 0.5f - h;
 }
 
+// Location-scale regression (families 13 and 14), one row of a pair: mean mu (identity link, offset included) and
+// s = log sigma, each its own linear predictor; z = (y - mu) e^-s with e^-s one expf per row and pair.
+// Family 13, the Gaussian:  ll = -z^2 / 2 - s - log(2 pi) / 2,  rm = dll/dmu = z e^-s,  rs = dll/ds = z^2 - 1.
+// The order of operations is gaussian_scale_loglik's and expf(-0) is exactly 1, so at s = 0 ll and rm are family 2's
+// bits.  Once z^2 / 2 overflows, ll is -inf, the correctly rounded value.
+__device__ __forceinline__ void location_scale_loglik(float y, float mu, float s, float& ll, float& rm, float& rs) {
+    const float sinv = expf(-s);
+    const float dn = (y - mu) * sinv;
+    ll = (-0.5f * dn * dn - 0.918938533204672742f) - s;
+    rm = dn * sinv;
+    rs = dn * dn - 1.f;
+}
+
+// Family 14, Student-t with nu = e^a degrees of freedom (a = log_dispersion), q = z^2 / nu, p = q / (1 + q):
+//   ll = C(nu) - s - (nu + 1) / 2 log1p(q),   rm = (nu + 1) z e^-s / (nu + z^2),   rs = (nu + 1) p - 1,
+//   q_a = dll/da = Q(nu) + p / 2 - (nu / 2) h(q),   h(q) = log1p(q) - p,
+//   C(nu) = lgamma((nu + 1) / 2) - lgamma(nu / 2) - log(nu pi) / 2,   Q(nu) = (nu / 2) [psi((nu + 1) / 2) - psi(nu / 2)] - 1/2.
+// Per-chain table words, from a at setup in double.  Below nu = 1e3, C and Q come from the Stirling series at
+// b' = nu / 2 + m >= 8 and a' = b' + 1/2, shifted back by the recurrences (the shift and series of
+// dispersion_constants, in a separate copy for the reason given at positive_constants):
+//   C = b' log1p(1 / (2 b')) - 1/2 + log(b') / 2 - log(nu pi) / 2 + S(a') - S(b') - sum_{j<m} log1p(1 / (2 (nu / 2 + j)))
+//   Q = (nu / 2) [log1p(1 / (2 b')) + T(a') - T(b') + sum_{j<m} (1 / (nu / 2 + j) - 1 / (nu / 2 + j + 1/2))] - 1/2
+// (S and T as at kDwCl / kDwCd): no lgamma or psi value is formed, and the largest cancellation, b' log1p(1 / (2 b'))
+// against 1/2, costs a factor 4 b' < 2e3 of double precision.  From nu = 1e3 both are their asymptotic series,
+//   C = -log(2 pi) / 2 - 1 / (4 nu) + 1 / (24 nu^3) - 1 / (20 nu^5),   Q = 1 / (4 nu) - 1 / (8 nu^3) + 1 / (4 nu^5),
+// whose truncation error there is below 1e-20, so no difference of values of size nu log nu is ever taken.
+constexpr int kStNu = 0;     // nu
+constexpr int kStNp1 = 1;    // nu + 1
+constexpr int kStC1 = 2;     // (nu + 1) / nu
+constexpr int kStIsq = 3;    // nu^-1/2
+constexpr int kStHn = 4;     // nu / 2
+constexpr int kStC = 5;      // C(nu)
+constexpr int kStQ = 6;      // Q(nu)
+
+__device__ inline void student_t_constants(float ld, float* t) {
+    const double l = (double)ld;
+    const double nu = exp(l);
+    double C, Q;
+    if (nu < 1e3) {
+        const double b = 0.5 * nu;
+        const int m = b < 8.0 ? (int)ceil(8.0 - b) : 0;
+        const double bp = b + m, ap = bp + 0.5;
+        double ls = 0.0, rs = 0.0;
+        for (int j = 0; j < m; ++j) {
+            ls += log1p(0.5 / (b + j));
+            rs += 1.0 / (b + j) - 1.0 / (b + j + 0.5);
+        }
+        const auto S = [](double z) {
+            const double i1 = 1.0 / z, i2 = i1 * i1;
+            return i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260)));
+        };
+        const auto T = [](double z) {
+            const double i1 = 1.0 / z, i2 = i1 * i1;
+            return -0.5 * i1 - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252)));
+        };
+        const double l1 = log1p(0.5 / bp);
+        C = (bp * l1 - 0.5) + 0.5 * (log(bp) - l - 1.1447298858494002) + (S(ap) - S(bp)) - ls;   // log pi
+        Q = b * (l1 + (T(ap) - T(bp)) + rs) - 0.5;
+    } else {
+        const double x = 1.0 / nu, x2 = x * x;
+        C = -0.918938533204672742 - x * (0.25 - x2 * (1.0 / 24 - x2 * (1.0 / 20)));
+        Q = x * (0.25 - x2 * (0.125 - x2 * 0.25));
+    }
+    t[kStNu] = (float)nu;
+    t[kStNp1] = (float)(nu + 1.0);
+    t[kStC1] = (float)((nu + 1.0) / nu);
+    t[kStIsq] = (float)(1.0 / sqrt(nu));
+    t[kStHn] = (float)(0.5 * nu);
+    t[kStC] = (float)C;
+    t[kStQ] = (float)Q;
+}
+
+// Family 14 of one row (see student_t_constants), with u = |z| nu^-1/2 = sqrt(q):
+// - q < 2^24 (u < 2^12): log1p(q), p = q / (1 + q) and z / (nu + z^2) = (z / (1 + q)) / nu directly;
+// - q >= 2^24, where z^2 may overflow (|z| up to ~1e30 and beyond stays finite): with 1 / q = (nu / z) / z,
+//   log1p(q) = 2 log u + log1p(1 / q), where log1p(1 / q) = 1 / q to within 2^-49, p = 1 / (1 + 1 / q) and
+//   z / (nu + z^2) = (1 / z) p, so rm -> 0 as |z| grows (bounded influence) and nothing overflows.
+// log u is taken as log1p(u - 1) (u - 1 is exact for u >= 2^12), so a row costs one log1p whichever branch it takes.
+// h(q) = log1p(q) - p loses about 2 eps / q to cancellation for small q, where the rows sit at a large nu (q ~ 1 / nu),
+// so below q = 1/4 (p < 1/5) it is the series of -log1p(-p) - p = sum_{k>=2} p^k / k, all terms positive, to k = 12:
+// the truncation error is below 2 (1/5)^11 / 13 / (4/5) < 4e-9 of h.  From q = 1/4 up the difference loses < 8 eps.
+__device__ __forceinline__ void student_t_loglik(float y, float mu, float s, const float* t, float& ll, float& rm,
+                                                 float& rs, float& qa) {
+    const float sinv = expf(-s);
+    const float z = (y - mu) * sinv;
+    const float u = fabsf(z) * t[kStIsq];
+    const float q = u * u;
+    const bool big = u >= 4096.f;
+    const float rz = __frcp_rn(z);
+    const float iq = (t[kStNu] * rz) * rz;                 // 1 / q (big rows)
+    const float d = __frcp_rn(1.f + (big ? iq : q));       // big: p, else 1 / (1 + q)
+    const float p = big ? d : q * d;
+    const float lg = log1pf(big ? u - 1.f : q);
+    const float L = big ? fmaf(2.f, lg, iq) : lg;          // log1p(q)
+    float hs = fmaf(p, 1.f / 12, 1.f / 11);
+    hs = fmaf(p, hs, 1.f / 10);
+    hs = fmaf(p, hs, 1.f / 9);
+    hs = fmaf(p, hs, 1.f / 8);
+    hs = fmaf(p, hs, 1.f / 7);
+    hs = fmaf(p, hs, 1.f / 6);
+    hs = fmaf(p, hs, 1.f / 5);
+    hs = fmaf(p, hs, 1.f / 4);
+    hs = fmaf(p, hs, 1.f / 3);
+    hs = fmaf(p, hs, 0.5f);
+    const float h = q < 0.25f ? (p * p) * hs : L - p;
+    const float np1 = t[kStNp1];
+    ll = fmaf(-0.5f * np1, L, t[kStC]) - s;
+    rm = (big ? np1 * (rz * p) : t[kStC1] * (z * d)) * sinv;
+    rs = fmaf(np1, p, -1.f);
+    qa = fmaf(-t[kStHn], h, fmaf(0.5f, p, t[kStQ]));
+}
+
 
 }  // namespace tc

@@ -9,7 +9,7 @@ Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
 
 How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
 oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
-``_Ordinal``, ``_Survival``, ``_Positive``, ``_Hvp``, ``_ZeroInflated`` below); :class:`GlmShards` and its callers are generic over it.
+``_Ordinal``, ``_Survival``, ``_Positive``, ``_Hvp``, ``_ZeroInflated``, ``_LocationScale`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
             "ordinal": 6, "weibull": 7, "lognormal": 8, "zero_inflated_poisson": 9, "zero_inflated_negative_binomial": 10,
-            "gamma": 11, "inverse_gaussian": 12}
+            "gamma": 11, "inverse_gaussian": 12, "gaussian_location_scale": 13, "student_t": 14}
 
 
 #: dynamic shared memory one CTA may opt in to on the H100 (227 KB), less 256 bytes for a kernel's static variables
@@ -210,6 +210,29 @@ class GlmShards(ShardModel):
         non-zero weight (a row of weight 0 may carry any y); offsets and weights work as for every family.  Only the
         bf16 tensor-core kernel evaluates these families, with the shape limits of the multinomial one;
         ``n_classes``, ``events`` and ``hvp`` are rejected.
+
+        ``"gaussian_location_scale"`` and ``"student_t"`` are location-scale (distributional) regression for a
+        continuous response on the real line: the scale gets its own linear predictor (brms' ``bf(y ~ x, sigma ~
+        x)``, GAMLSS, per-group variances), and ``student_t`` is robust regression with learned degrees of freedom
+        (PyMC's robust linear regression, brms' ``student()``), whose bounded influence keeps gross outliers from
+        pulling beta.  The mean ``mu = intercept[group] + x' beta + o`` (identity link; the offset goes into mu only)
+        and ``s = log sigma = sigma_intercept[group] + x' sigma_beta``.  With ``z = (y - mu) e^-s``:
+
+            gaussian_location_scale:   ll = -z^2 / 2 - s - log(2 pi) / 2
+            student_t, nu = e^a:       ll = lgamma((nu + 1) / 2) - lgamma(nu / 2) - log(nu pi) / 2 - s
+                                            - (nu + 1) / 2 log1p(z^2 / nu)
+
+        LL is the full density: it equals ``scipy.stats.norm(mu, sigma).logpdf(y)`` and ``scipy.stats.t(df=nu,
+        loc=mu, scale=sigma).logpdf(y)``.  At nu = 1 Student-t is the Cauchy distribution, and as nu grows it tends to
+        the Gaussian family.  The inputs per call are ``(intercept, beta, sigma_intercept, sigma_beta)``, shapes
+        ``[G]``, ``[P]``, ``[G]`` and ``[P]`` (a scalar intercept when G = 1), and for Student-t a trailing scalar
+        ``log_dispersion = log nu``; batched with a leading K (at most 8).  Gradients come back in the shapes of the
+        inputs.  Chain k runs as the kernel columns 2k (mu) and 2k + 1 (s) of a 2K-column launch, so X is read once
+        for both predictors.  A constant scale is ``sigma_beta = 0``, held fixed (its gradient ignored); it costs the
+        same launch.  Responses must be finite on every row of non-zero weight (a row of weight 0 may carry any y);
+        offsets and weights work as for every family.  Only the bf16 tensor-core kernel evaluates these families, with
+        the shape limits of the multinomial one; ``n_classes``, ``events`` and ``hvp`` are rejected, and so is a shape
+        whose 2K-column launch gets fewer than two pipeline stages (checked when an engine attaches the model).
     events
         Per-row event indicators of the survival families (see ``family``).
     hvp
@@ -791,6 +814,18 @@ def _check_positive(m, what: str) -> None:
             raise ValueError(f"{what} of segment {si} must be finite and > 0 on every row of non-zero weight")
 
 
+def _check_finite(m, what: str) -> None:
+    """Every row of non-zero weight holds a finite y."""
+    import torch
+
+    for si, (y, w) in enumerate(zip(m.ys, m.weights)):
+        bad = ~torch.isfinite(y)
+        if w is not None:
+            bad &= w != 0   # a masked row may carry anything
+        if bool(torch.any(bad)):
+            raise ValueError(f"{what} of segment {si} must be finite on every row of non-zero weight")
+
+
 def _labels(y, w):
     """Integer labels of a chunk; masked rows may carry NaN or out-of-range labels: any valid class will do."""
     import torch
@@ -1156,29 +1191,28 @@ class _Ordinal(_Layout):
         return (*self._matrices(inputs), terms)
 
 
-class _ZeroInflated(_Layout):
-    """``zero_inflated_poisson`` and ``zero_inflated_negative_binomial``: inputs ``(intercept[G], beta[P],
-    zi_intercept[G], zi_beta[P])`` and, for the negative binomial, a trailing ``log_dispersion``.  Chain k runs as
-    kernel columns 2k, with the theta row ``(intercept, beta[, log_dispersion])`` and the output block ``[LL,
-    d intercept[G], d beta[P](, d log_dispersion)]``, and 2k + 1, with the theta row ``(zi_intercept, zi_beta[,
-    log_dispersion])`` and the output block ``[0, d zi_intercept[G], d zi_beta[P](, 0)]``.  Only the count columns
-    take the offset."""
+class _Pair(_Layout):
+    """Two linear predictors per chain over one read of X: inputs ``(intercept[G], beta[P], intercept2[G], beta2[P])``
+    and, where ``disp``, a trailing ``log_dispersion``.  Chain k runs as kernel columns 2k, with the theta row
+    ``(intercept, beta[, log_dispersion])`` and the output block ``[LL, d intercept[G], d beta[P](, d log_dispersion)]``,
+    and 2k + 1, with the theta row ``(intercept2, beta2[, log_dispersion])`` and the output block ``[0, d intercept2[G],
+    d beta2[P](, 0)]``.  Only the first predictor takes the offset.  Subclasses give the validation and
+    :meth:`_pair_terms`, the oracle's per-row terms."""
 
     columns = 2
     offset_columns = slice(0, None, 2)
     pairs = True
 
-    def __init__(self, m, n_classes) -> None:
+    def __init__(self, m, n_classes, predictors: str, disp: bool) -> None:
         self._no_classes(n_classes)
         _tc_kernel_only(m)
         if not 1 <= m.n_chains <= 8:
-            raise ValueError(f"the {m.family} family takes n_chains in [1, 8] (each chain's count and zero-inflation "
-                             f"predictors are two of the tensor-core kernel's 16 columns per launch), got {m.n_chains}")
-        _check_integers(m, "counts", "[0, 2^24]", lambda y: y <= 2.0 ** 24)
+            raise ValueError(f"the {m.family} family takes n_chains in [1, 8] (each chain's {predictors} predictors are "
+                             f"two of the tensor-core kernel's 16 columns per launch), got {m.n_chains}")
         super().__init__(m)
-        self.nb = m.family == "zero_inflated_negative_binomial"
-        self.shapes = self.shapes * 2 + ([()] if self.nb else [])
-        self.words += int(self.nb)
+        self.disp = disp
+        self.shapes = self.shapes * 2 + ([()] if disp else [])
+        self.words += int(disp)
 
     def pack(self, inputs, out: np.ndarray):
         G, P = self.G, self.P
@@ -1188,7 +1222,7 @@ class _ZeroInflated(_Layout):
         th[:, 0, G : G + P] = xs[1].reshape(self.K, P)
         th[:, 1, :G] = xs[2].reshape(self.K, G)
         th[:, 1, G : G + P] = xs[3].reshape(self.K, P)
-        if self.nb:
+        if self.disp:
             th[:, :, G + P] = xs[4].reshape(self.K, 1)   # both rows: every column's table is built from its own row
         return self.call_context(xs)
 
@@ -1206,20 +1240,54 @@ class _ZeroInflated(_Layout):
         import torch
 
         ic, bt = self._matrices(inputs[:2])
-        zic, zbt = self._matrices(inputs[2:4])
-        pairs = lambda a, b: torch.stack([a, b], dim=2).reshape(a.shape[0], -1)   # column 2k: eta, 2k + 1: zeta
-        ld = _f64(inputs[4]).reshape(self.K).to(device, dtype) if self.nb else None
+        ic2, bt2 = self._matrices(inputs[2:4])
+        pairs = lambda a, b: torch.stack([a, b], dim=2).reshape(a.shape[0], -1)   # column 2k: first, 2k + 1: second
+        ld = _f64(inputs[4]).reshape(self.K).to(device, dtype) if self.disp else None
 
         def terms(y, w, eta):
-            return _zero_inflated_terms(y.to(eta.dtype).unsqueeze(1), eta[:, 0::2], eta[:, 1::2], ld)
+            return self._pair_terms(y.to(eta.dtype).unsqueeze(1), eta[:, 0::2], eta[:, 1::2], ld)
 
-        return pairs(ic, zic), pairs(bt, zbt), terms
+        return pairs(ic, ic2), pairs(bt, bt2), terms
+
+    @staticmethod
+    def _pair_terms(y, first, second, a):
+        """The per-row terms ``[n, K, 2]`` of :meth:`_Layout.oracle` from both predictors (and log_dispersion)."""
+        raise NotImplementedError
+
+
+class _ZeroInflated(_Pair):
+    """``zero_inflated_poisson`` and ``zero_inflated_negative_binomial``: the pair layout with the count predictor
+    ``(intercept, beta)``, the zero-inflation logit ``(zi_intercept, zi_beta)`` and, for the negative binomial,
+    ``log_dispersion = log alpha``."""
+
+    def __init__(self, m, n_classes) -> None:
+        super().__init__(m, n_classes, "count and zero-inflation", m.family == "zero_inflated_negative_binomial")
+        _check_integers(m, "counts", "[0, 2^24]", lambda y: y <= 2.0 ** 24)
+
+    @staticmethod
+    def _pair_terms(y, eta, zeta, a):
+        return _zero_inflated_terms(y, eta, zeta, a)
+
+
+class _LocationScale(_Pair):
+    """``gaussian_location_scale`` and ``student_t``: the pair layout with the mean ``(intercept, beta)``, the log scale
+    ``(sigma_intercept, sigma_beta)`` and, for Student-t, ``log_dispersion = log nu``.  Every row of non-zero weight
+    must hold a finite y."""
+
+    def __init__(self, m, n_classes) -> None:
+        super().__init__(m, n_classes, "mean and log-scale", m.family == "student_t")
+        _check_finite(m, "responses")
+
+    @staticmethod
+    def _pair_terms(y, mu, s, a):
+        return _location_scale_terms(y, mu, s, a)
 
 
 _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_binomial": _Dispersion,
             "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival,
             "zero_inflated_poisson": _ZeroInflated, "zero_inflated_negative_binomial": _ZeroInflated,
-            "gamma": _Positive, "inverse_gaussian": _Positive}
+            "gamma": _Positive, "inverse_gaussian": _Positive, "gaussian_location_scale": _LocationScale,
+            "student_t": _LocationScale}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -1397,6 +1465,73 @@ def _zero_inflated_terms(y, eta, zeta, a=None):
     if q is not None:
         out.append(pair(w0 * q, torch.zeros_like(q)))
     return out
+
+
+_LOG_PI = 1.1447298858494002
+
+
+def _student_t_constants(a):
+    """``(nu, C(nu), Q(nu))`` per chain in float64 for ``nu = exp(a)``: ``C = lgamma((nu + 1) / 2) - lgamma(nu / 2) -
+    log(nu pi) / 2`` and ``Q = (nu / 2) [psi((nu + 1) / 2) - psi(nu / 2)] - 1/2``, from their asymptotic series at
+    nu >= 1e3 (truncation error < 1e-20), where the direct forms subtract values of size nu log nu: ``C = -log(2 pi) / 2
+    - 1 / (4 nu) + 1 / (24 nu^3) - 1 / (20 nu^5)``, ``Q = 1 / (4 nu) - 1 / (8 nu^3) + 1 / (4 nu^5)``."""
+    import torch
+
+    a = a.double()
+    nu = torch.exp(a)
+    big = nu >= 1e3
+    ns = torch.where(big, torch.ones_like(nu), nu)
+    x = 1.0 / torch.where(big, nu, torch.full_like(nu, 1e3))
+    x2 = x * x
+    c_small = torch.lgamma(0.5 * (ns + 1)) - torch.lgamma(0.5 * ns) - 0.5 * (torch.log(ns) + _LOG_PI)
+    q_small = 0.5 * ns * (torch.digamma(0.5 * (ns + 1)) - torch.digamma(0.5 * ns)) - 0.5
+    C = torch.where(big, -_LOG_SQRT_2PI - x * (0.25 - x2 * (1.0 / 24 - x2 / 20)), c_small)
+    Q = torch.where(big, x * (0.25 - x2 * (0.125 - x2 * 0.25)), q_small)
+    return nu, C, Q
+
+
+#: 1 / k for k = 2 .. 30: the series h = sum_k p^k / k of h(q) = log1p(q) - q / (1 + q) in p = q / (1 + q), to a
+#: truncation error below 1e-19 of h at q < 1/4
+_H_SERIES = [1.0 / k for k in range(2, 31)]
+
+
+def _location_scale_terms(y, mu, s, a=None):
+    """The per-row terms of a location-scale model, ``[n, K, 2]`` (column 0: the mean mu, 1: s = log sigma), with ``z =
+    (y - mu) e^-s``: ``ll`` (in column 0, 0 in column 1), ``(dll/dmu, dll/ds)`` and, with ``a = log nu`` (Student-t;
+    ``None``: Gaussian), ``dll/da`` (in column 0).  Gaussian: ``ll = -z^2 / 2 - s - log(2 pi) / 2``, ``dll/dmu = z
+    e^-s``, ``dll/ds = z^2 - 1``.  Student-t, with ``q = z^2 / nu``, ``p = q / (1 + q)`` and :func:`_student_t_constants`:
+
+        ll = C - s - (nu + 1) / 2 log1p(q),   dll/dmu = (nu + 1) z e^-s / (nu + z^2),   dll/ds = (nu + 1) p - 1,
+        dll/da = Q + p / 2 - (nu / 2) h(q),   h(q) = log1p(q) - p.
+
+    From ``u = |z| nu^-1/2 = 2^12`` up, where z^2 may overflow float32, ``log1p(q) = 2 log u + log1p(1 / q)`` and
+    ``z / (nu + z^2) = p / z`` with ``1 / q = (nu / z) / z``; below q = 1/4, h is its series in p (``h = p^2 / 2 + p^3 /
+    3 + ...``), since the difference loses about ``2 eps / q``.  Valid in float64 and float32."""
+    import torch
+
+    sinv = torch.exp(-s)
+    z = (y - mu) * sinv
+    pair = lambda u, v: torch.stack([u, v], dim=2)
+    if a is None:
+        ll = -0.5 * z * z - s - _LOG_SQRT_2PI
+        return [pair(ll, torch.zeros_like(ll)), pair(z * sinv, z * z - 1.0)]
+    nu, C, Q = (v.to(z.dtype) for v in _student_t_constants(a))
+    u = z.abs() / torch.sqrt(nu)
+    big = u >= 4096.0
+    zb = torch.where(big, z, torch.ones_like(z))          # every branch finite where it is not taken
+    q = torch.where(big, torch.zeros_like(u), u * u)
+    iq = torch.where(big, (nu / zb) / zb, torch.ones_like(z))
+    p = torch.where(big, 1.0 / (1.0 + iq), q / (1.0 + q))
+    L = torch.where(big, 2.0 * torch.log(torch.where(big, u, torch.ones_like(u))) + torch.log1p(iq), torch.log1p(q))
+    zr = torch.where(big, p / zb, z / (nu * (1.0 + q)))   # z / (nu + z^2)
+    ps = torch.where(q < 0.25, p, torch.zeros_like(p))
+    acc = torch.full_like(ps, _H_SERIES[-1])
+    for c in reversed(_H_SERIES[:-1]):
+        acc = acc * ps + c
+    h = torch.where(big | (q >= 0.25), L - p, ps * ps * acc)
+    ll = C - s - 0.5 * (nu + 1.0) * L
+    qa = Q + 0.5 * p - 0.5 * nu * h
+    return [pair(ll, torch.zeros_like(ll)), pair((nu + 1.0) * zr * sinv, (nu + 1.0) * p - 1.0), pair(qa, torch.zeros_like(qa))]
 
 
 _DISPERSION_TERMS = {"gaussian_scale": _gaussian_scale_terms, "negative_binomial": _negative_binomial_terms,
@@ -1718,6 +1853,42 @@ def synth_positive_shard(n_rows: int, n_features: int, *, family: str, shape: fl
         mu = torch.exp(xb.float() @ beta_true + intercept).double()
         y[r0:r1] = draw_positive(mu, family=family, shape=shape, generator=gen)
     return X, y, beta_true
+
+
+def synth_location_scale_shard(n_rows: int, n_features: int, *, family: str, seed: int, device, nu: Optional[float] = None,
+                               chunk_rows: int = 1 << 20, beta_scale: float = 0.05, intercept: float = 0.5,
+                               sigma_intercept: float = 0.0, sigma_beta_scale: float = 0.05):
+    """Synthetic location-scale shard generated on the device in chunks: bf16 ``X ~ N(0,1)`` and ``y = mu + sigma
+    eps`` with ``mu = X beta* + intercept`` and ``log sigma = X sigma_beta* + sigma_intercept``, ``eps ~ N(0, 1)``
+    (``family="gaussian_location_scale"``) or Student-t with ``nu`` degrees of freedom (``"student_t"``, drawn as
+    ``N(0, 1) / sqrt(chi2_nu / nu)`` with the chi-square a ``Gamma(nu / 2, scale 2)`` draw), in float64 and stored as
+    float32 (clamped into its finite range).  Returns ``(X, y, beta*, sigma_beta*)``."""
+    import torch
+
+    if family not in ("gaussian_location_scale", "student_t"):
+        raise ValueError(f"family must be 'gaussian_location_scale' or 'student_t', got {family!r}")
+    if (family == "student_t") != (nu is not None) or (nu is not None and not nu > 0):
+        raise ValueError(f"nu > 0 is for family='student_t' only, got nu={nu} for {family!r}")
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    sigma_true = (torch.randn(n_features, generator=gen, device=device) * sigma_beta_scale).float()
+    fmax = torch.finfo(torch.float32).max
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        xd = xb.double()
+        mu = xd @ beta_true.double() + intercept
+        sigma = torch.exp(xd @ sigma_true.double() + sigma_intercept)
+        eps = torch.randn(r1 - r0, generator=gen, device=device, dtype=torch.float64)
+        if nu is not None:
+            chi2 = 2.0 * torch._standard_gamma(torch.full_like(eps, 0.5 * nu), generator=gen)
+            eps = eps / torch.sqrt(chi2 / nu)
+        y[r0:r1] = (mu + sigma * eps).clamp(-fmax, fmax).float()   # a heavy tail at a small nu stays finite
+    return X, y, beta_true, sigma_true
 
 
 def synth_logistic_shard_fp8(n_rows: int, n_features: int, *, seed: int, device, chunk_rows: int = 1 << 20):

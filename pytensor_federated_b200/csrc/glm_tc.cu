@@ -209,15 +209,19 @@ __host__ __device__ inline int row_arrays(bool rows, int row_data) {
 //   StudentT          the Student-t family (tc::student_t_loglik): LocationScale with ZeroInflatedDisp's theta and
 //                     output layout (both theta rows of a pair end in log nu; the table of column 2p is used, q =
 //                     dll/dlog_nu comes from column 2p and column 2p + 1 writes q = 0).
+//   Beta              beta regression for proportions in (0, 1) (tc::beta_loglik): Dispersion's layout with
+//                     log_dispersion = log precision; log y and log(1 - y) computed once per row and shared by its
+//                     chains.
 // Column layouts follow the wgmma accumulator fragment (thread lane owns columns 8j + 2 (lane % 4) + {0, 1}), so
 // that one thread holds every term of the chains it works on.
 enum class Epi {
-    Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp, Positive, LocationScale, StudentT
+    Scalar, Softmax, Dispersion, Ordinal, Survival, Hvp, ZeroInflated, ZeroInflatedDisp, Positive, LocationScale, StudentT,
+    Beta
 };
 
 __host__ __device__ constexpr bool has_dispersion(Epi e) {
     return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp || e == Epi::Positive ||
-           e == Epi::StudentT;
+           e == Epi::StudentT || e == Epi::Beta;
 }
 
 // The epilogues whose chain k is the column pair (2k, 2k + 1), both predictors formed in one thread before either
@@ -238,11 +242,12 @@ constexpr Epi epilogue(int family) {
         case kGlmGamma: case kGlmInverseGaussian: return Epi::Positive;
         case kGlmGaussianLocationScale: return Epi::LocationScale;
         case kGlmStudentT: return Epi::StudentT;
+        case kGlmBeta: return Epi::Beta;
         default: return Epi::Scalar;
     }
 }
 static_assert([] {
-    for (int code = 0; code <= kGlmStudentT; ++code)
+    for (int code = 0; code <= kGlmBeta; ++code)
         if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
     return true;
 }(), "the epilogue's theta and output layout must match the family's");
@@ -282,7 +287,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
     constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
                    SURV = E == Epi::Survival, HVP = E == Epi::Hvp, POS = E == Epi::Positive,
-                   PAIR = pair_epilogue(E), ZNB = E == Epi::ZeroInflatedDisp, STT = E == Epi::StudentT;
+                   PAIR = pair_epilogue(E), ZNB = E == Epi::ZeroInflatedDisp, STT = E == Epi::StudentT,
+                   BT = E == Epi::Beta;
     constexpr int C8 = cfg(KC).C8;
     constexpr int N1 = cfg(KC).N1;
     constexpr int N2 = cfg(KC).N2;
@@ -426,6 +432,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         else if constexpr (STT)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 student_t_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
+        else if constexpr (BT)
+            for (int k = threadIdx.x; k < KC; k += blockDim.x)
+                beta_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         else if constexpr (DISP)   // families 4 and 5, and 10, whose table is family 5's (any code but 4)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
@@ -537,7 +546,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 const int td = threadIdx.x - 32;
                 // panels per load group: 2 where the registers it needs do not push the instantiation into spills
                 // (ptxas -v; the consumers' epilogue sets the register count), else 1
-                constexpr int kDecGroup = KC <= 4 && !ORD ? 2 : 1;
+                constexpr int kDecGroup = KC <= 4 && !ORD && !BT ? 2 : 1;
                 static_assert(kDecGroup <= 2, "a packed launch may have only 2 compressed slots");
                 int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
                 Ring stage, xs;
@@ -698,6 +707,17 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                     wgmma_commit();
                     wgmma_wait<0>();
                     fence_regs(eacc);
+                    // BT: eta of the thread's columns (the sum of the three bf16 terms), formed once so that the
+                    // accumulator fragment is dead during the long per-column evaluations below
+                    float bt_eta[2 * 2 * NJ];
+                    if constexpr (BT) {
+#pragma unroll
+                        for (int i = 0; i < 4 * NJ; ++i) {
+                            const int h = i / (2 * NJ), jc = (i % (2 * NJ)) >> 1, e = i & 1;
+                            bt_eta[i] = (eacc[4 * jc + 2 * h + e] + eacc[4 * (NJ + jc) + 2 * h + e]) +
+                                        eacc[4 * (2 * NJ + jc) + 2 * h + e];
+                        }
+                    }
                     // ---- link, likelihood, residual -> (hi, lo) bf16 columns of R (element (row, n) at
                     // (n / 8) * 2048 + (row / 8) * 128 + (n % 8) * 16 + (row % 8) * 2)
                     unsigned char* rbuf = r_buf + rb * L.r_bytes;
@@ -728,6 +748,13 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                         if constexpr (POS) {
                             pv_lt = logf(y);
                             if (prm.family == kGlmInverseGaussian) pv_iy = __frcp_rn(y);
+                        }
+                        // BT: log y and log(1 - y) of the row, shared by its chains (a row past the segment and a masked
+                        // row's y outside (0, 1) are dropped below, as in POS)
+                        float bt_ly = 0.f, bt_l1y = 0.f;
+                        if constexpr (BT) {
+                            bt_ly = logf(y);
+                            bt_l1y = log1pf(-y);
                         }
                         // SOFTMAX: the row's log-sum-exp per chain over the quad; every lane takes part, whether its
                         // row is valid or not (a row past the segment is dropped below, as in the other families)
@@ -765,6 +792,43 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                             ordinal_loglik<2 * NJ, KC>(z, od_chain, od_cut, od_chains, od_ncut, yi, icpt, 1,
                                                        od_ll, od_r);
                         }
+                        if constexpr (BT) {
+                            // one column at a time (a rolled loop; its eta and accumulators are picked by selects, so
+                            // they stay in registers): beta_loglik is long, and K = 16 has no registers for two of
+                            // them in flight.  Each column gets the values and additions of the unrolled loop below.
+#pragma unroll 1
+                            for (int s = 0; s < 2 * NJ; ++s) {
+                                const int k = 8 * (s >> 1) + 2 * q + (s & 1);
+                                float eta = 0.f;
+#pragma unroll
+                                for (int i = 0; i < 2 * NJ; ++i) eta = i == s ? bt_eta[2 * NJ * h + i] : eta;
+                                float ll = 0.f, r = 0.f, dq = 0.f;
+                                if (valid && k < nch) {
+                                    // offset and weight as in ROWS, the weight applied to all three values
+                                    float et = eta + icpt[k];
+                                    if constexpr (ROWS) et = __fadd_rn(et, o);
+                                    beta_loglik(y, bt_ly, bt_l1y, et, disp + k * kDispWords, ll, r, dq);
+                                    if constexpr (ROWS) {
+                                        apply_weight(wt, ll);
+                                        apply_weight(wt, r);
+                                        apply_weight(wt, dq);
+                                    }
+                                }
+#pragma unroll
+                                for (int i = 0; i < 2 * NJ; ++i) {
+                                    ll_acc[i] += i == s ? ll : 0.f;
+                                    gi_acc[i] += i == s ? r : 0.f;
+                                    ds_acc[i] += i == s ? dq : 0.f;
+                                }
+                                if (k < N2 / 2) {
+                                    const __nv_bfloat16 hi = __float2bfloat16_rn(r);
+                                    const __nv_bfloat16 lo = __float2bfloat16_rn(r - __bfloat162float(hi));
+                                    unsigned char* p0 = rbuf + ((2 * k) / 8) * 2048 + (row / 8) * 128 + (row % 8) * 2;
+                                    *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k) % 8) * 16) = hi;
+                                    *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k + 1) % 8) * 16) = lo;
+                                }
+                            }
+                        } else {
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc) {
                             float hv_h = 0.f;   // HVP: h = d2ll / deta2 of the pair's theta column (e = 0), for e = 1
@@ -884,6 +948,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                     *reinterpret_cast<__nv_bfloat16*>(p0 + ((2 * k + 1) % 8) * 16) = lo;
                                 }
                             }
+                        }
                         }
                     }
                     fence_proxy_async();
@@ -1030,6 +1095,7 @@ LaunchFn pick(tc::Epi e, int kc, bool rows) {
         case Epi::Positive: return pick<Epi::Positive>(kc, rows);
         case Epi::LocationScale: return pick<Epi::LocationScale>(kc, rows);
         case Epi::StudentT: return pick<Epi::StudentT>(kc, rows);
+        case Epi::Beta: return pick<Epi::Beta>(kc, rows);
     }
 }
 }  // namespace

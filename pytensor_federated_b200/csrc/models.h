@@ -34,8 +34,8 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12, 14: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12, 14: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12, 14, 15: [.., log_dispersion])
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12, 14, 15: [K][G+P+1])
     int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)
@@ -71,6 +71,8 @@ enum GlmFamilyCode : int {
     kGlmInverseGaussian = 12,  //   Var(y) = mu^2 / nu (gamma), mu^3 / lambda (inverse Gaussian)
     kGlmGaussianLocationScale = 13,  // location-scale: pair p is column 2p (mean mu, identity link) and 2p + 1
     kGlmStudentT = 14,               //   (log sigma); family 14 adds log_dispersion = log nu
+    kGlmBeta = 15,           // proportions in (0, 1), logit link to the mean, log_dispersion = log precision phi:
+                             //   Var(y) = mu (1 - mu) / (1 + phi)
 };
 
 // How a family's columns make up n_chains: one per chain, one per chain and class (column k C + c is class c of chain
@@ -104,6 +106,7 @@ constexpr GlmFamily glm_family(int code) {
         case kGlmGaussianLocationScale:
             return {"gaussian_location_scale", true, false, GlmColumns::kPair, 1, 1, true};
         case kGlmStudentT: return {"student_t", true, true, GlmColumns::kPair, 1, 1, true};
+        case kGlmBeta: return {"beta", true, true, GlmColumns::kOne, 1, 1, true};
         default: return {"", false, false, GlmColumns::kOne, 1, 1, true};   // 0 to 2: every GLM kernel
     }
 }

@@ -774,5 +774,151 @@ __device__ __forceinline__ void student_t_loglik(float y, float mu, float s, con
     qa = fmaf(-t[kStHn], h, fmaf(0.5f, p, t[kStQ]));
 }
 
+// Beta regression (family 15): y in (0, 1), mu = sigmoid(eta), phi = e^a the precision (a = log_dispersion),
+// A = mu phi, B = (1 - mu) phi, y ~ Beta(A, B).  With the Stirling tail S(z) = lgamma(z) - [(z - 1/2) log z - z +
+// log(2 pi) / 2], tau(z) = psi(z) - log z and the Bernoulli divergence KL = mu log(mu / y) + (1 - mu) log((1 - mu) /
+// (1 - y)) >= 0, the density is grouped so that nothing of size phi log phi is formed:
+//   ll = C(phi) + (log mu + log(1 - mu)) / 2 - log y - log(1 - y) - phi KL - S(A) - S(B),
+//   r  = dll/deta = phi mu (1 - mu) (logit y - logit mu) - (1 - mu) A tau(A) + mu B tau(B),
+//   q  = dll/da   = Q(phi) - phi KL - A tau(A) - B tau(B),
+// C(phi) = (a - log 2 pi) / 2 + S(phi) and Q(phi) = phi tau(phi) per chain, from a at setup in double: below phi = 8
+// through the recurrence to phi' = phi + m >= 8, from 8 up as their asymptotic series, so Q -> -1/2 is never the
+// difference of values of size phi.
+constexpr int kBtPhi = 0;    // phi
+constexpr int kBtC = 1;      // C(phi)
+constexpr int kBtQ = 2;      // Q(phi)
+constexpr int kBtA = 3;      // a = log phi
+
+__device__ inline void beta_constants(float ld, float* t) {
+    const double l = (double)ld;
+    const double phi = exp(l);
+    double S, Q;
+    if (phi < 8.0) {
+        const int m = (int)ceil(8.0 - phi);
+        const double pp = phi + m;
+        double lp = 0.0, sr = 0.0;   // the factors phi + j, j = 1 .. m - 1 (j = 0 is taken through l = log phi)
+        for (int j = 1; j < m; ++j) {
+            lp += log(phi + j);
+            sr += 1.0 / (phi + j);
+        }
+        const double i1 = 1.0 / pp, i2 = i1 * i1, lpp = log(pp);
+        const double Sp = i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260 - i2 * (1.0 / 1680))));
+        const double Tp = -0.5 * i1 - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252 - i2 * (1.0 / 240))));
+        S = Sp + (pp - 0.5) * lpp - (phi + 0.5) * l - m - lp;
+        Q = phi * (Tp + (lpp - l) - sr) - 1.0;
+    } else {
+        const double i1 = 1.0 / phi, i2 = i1 * i1;
+        S = i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260 - i2 * (1.0 / 1680))));
+        Q = -0.5 - i1 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252 - i2 * (1.0 / 240))));
+    }
+    t[kBtPhi] = (float)phi;
+    t[kBtC] = (float)(0.5 * (l - 1.83787706640934548) + S);   // log 2 pi
+    t[kBtQ] = (float)Q;
+    t[kBtA] = ld;
+}
+
+// S(z) and z tau(z) of one z > 0 that changes from row to row, lz = log z given (z = A or B may underflow where its
+// logarithm does not).  Below z = 8 the argument is shifted to z' = z + m, m = ceil(8 - z) in 1 .. 8:
+//   S(z) = S(z') + (z' - 1/2) log z' - (z + 1/2) log z - m - log prod_{j=1}^{m-1} (z + j),
+//   z tau(z) = z [T(z') + log z' - log z - sum_{j=1}^{m-1} 1 / (z + j)] - 1,
+// with the j = 0 factor taken analytically (its log is lz, z / z = 1), so a z near 0 costs nothing in accuracy.
+// The factors run as a fixed, predicated loop of 7 steps in two products of at most 4 (no loop length depends on
+// the row, and the products stay below 16^4): one __logf and one division each.  S and T are the series of kDwCl /
+// kDwCd at z' >= 8.
+__device__ __forceinline__ void beta_tails(float z, float lz, float& S, float& zt) {
+    const int m = z < 8.f ? (int)ceilf(8.f - z) : 0;
+    float lp = 0.f, sr = 0.f;
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+        float pr = 1.f, nu = 0.f;   // prod f and (sum 1 / f) prod f over this group's factors
+#pragma unroll
+        for (int j = 4 * g + 1; j < 4 * g + 5 && j < 8; ++j)
+            if (j < m) {
+                const float f = z + (float)j;
+                nu = fmaf(nu, f, pr);
+                pr = pr * f;
+            }
+        lp += __logf(pr);
+        sr += __fdividef(nu, pr);
+    }
+    const float zp = z + (float)m;
+    const float iz = __frcp_rn(zp), iz2 = iz * iz;
+    const float Sz = iz * (1.f / 12 - iz2 * (1.f / 360 - iz2 * (1.f / 1260)));
+    const float Tz = -0.5f * iz - iz2 * (1.f / 12 - iz2 * (1.f / 120 - iz2 * (1.f / 252)));
+    const float lzp = logf(zp);
+    const bool shift = m > 0;
+    S = shift ? Sz + ((fmaf(zp - 0.5f, lzp, -(float)m) - lp) - (z + 0.5f) * lz) : Sz;
+    zt = shift ? fmaf(z, (Tz - sr) + (lzp - lz), -1.f) : z * Tz;
+}
+
+// k(x) = x - log1p(x) >= 0 for |x| < 1/2 from s = x / (2 + x) (log1p(x) = 2 atanh(s), x - 2 s = x s):
+//   k(x) = x s - 2 s^3 (1/3 + s^2 / 5 + ... + s^12 / 15),
+// no cancellation (2 s^3 / 3 < x s / 16 for x > 0; both terms >= 0 for x < 0) and a truncation error below 5e-9 of
+// k at |s| <= 1/3, where x - log1pf(x) would lose about 2 eps / |x| of k.
+__device__ __forceinline__ float beta_kl_series(float x) {
+    const float s = x * __frcp_rn(2.f + x), s2 = s * s;
+    float p = fmaf(s2, 1.f / 15, 1.f / 13);
+    p = fmaf(s2, p, 1.f / 11);
+    p = fmaf(s2, p, 1.f / 9);
+    p = fmaf(s2, p, 1.f / 7);
+    p = fmaf(s2, p, 1.f / 5);
+    p = fmaf(s2, p, 1.f / 3);
+    return fmaf(x, s, -2.f * (s * s2) * p);
+}
+
+// Family 15 of one row (see beta_constants), ly = log y and l1y = log(1 - y) computed once per row.  mu and 1 - mu
+// both come from e = exp(-|eta|) (1 - mu is never 1 - mu rounded), and so do log mu = -softplus(-eta), log(1 - mu)
+// and 1 / mu, 1 / (1 - mu).  The relative differences u = (y - mu) / mu and v = (mu - y) / (1 - mu) give
+//   logit y - logit mu = log1p(u) - log1p(v),   phi KL = A k(u) + B k(v)   (mu u + (1 - mu) v = 0),
+// so neither cancels at y ~ mu, where the rows sit at a large phi (|y - mu| ~ phi^-1/2): below |x| = 1/2, k is
+// beta_kl_series and log1p(x) = x - k(x); from 1/2 up, log1p(u) = log y - log mu (and log1p(v) = log(1 - y) -
+// log(1 - mu)), which stays finite where 1 + u loses all its digits, and A k(u) = phi (y - mu) - A log1p(u).  y - mu is
+// formed as (1 - mu) - (1 - y) for mu >= 1/2, exact where the two are close.  log A = log mu + a is never log of A.
+__device__ __forceinline__ void beta_loglik(float y, float ly, float l1y, float eta, const float* t, float& ll, float& r,
+                                            float& q) {
+    const float phi = t[kBtPhi];
+    const float e = expf(-fabsf(eta));
+    const float l1e = log1pf(e);
+    const float inv = __frcp_rn(1.f + e);
+    const bool pos = eta >= 0.f;
+    const float mu = pos ? inv : e * inv, nmu = pos ? e * inv : inv;              // mu, 1 - mu
+    const float lmu = pos ? -l1e : eta - l1e, l1mu = pos ? -eta - l1e : -l1e;      // log mu, log(1 - mu)
+    const float d = pos ? nmu - (1.f - y) : y - mu;                                 // y - mu
+    const float pd = phi * d;
+    // the terms that do not involve the tails first, each side (u, then v) finished before the next starts, and each
+    // tail folded into ll, r and q as soon as it is known: few values stay live at once
+    float kl, dlg;   // phi KL, logit y - logit mu
+    {
+        const float A = mu * phi;
+        const float u = d * (pos ? 1.f + e : 1.f + __frcp_rn(e));                   // (y - mu) / mu
+        const bool su = fabsf(u) < 0.5f;
+        const float ku = beta_kl_series(u);
+        const float lu = su ? u - ku : ly - lmu;                                     // log1p(u)
+        kl = su ? A * ku : fmaf(-A, lu, pd);
+        dlg = lu;
+    }
+    {
+        const float B = nmu * phi;
+        const float v = -d * (pos ? 1.f + __frcp_rn(e) : 1.f + e);                  // (mu - y) / (1 - mu)
+        const bool sv = fabsf(v) < 0.5f;
+        const float kv = beta_kl_series(v);
+        const float lv = sv ? v - kv : l1y - l1mu;                                   // log1p(v)
+        kl += sv ? B * kv : fmaf(-B, lv, -pd);
+        dlg -= lv;
+    }
+    ll = (fmaf(0.5f, lmu + l1mu, t[kBtC]) - (ly + l1y)) - kl;
+    r = (mu * phi) * nmu * dlg;
+    q = t[kBtQ] - kl;
+    float S, zt;
+    beta_tails(mu * phi, lmu + t[kBtA], S, zt);
+    ll -= S;
+    r = fmaf(-nmu, zt, r);
+    q -= zt;
+    beta_tails(nmu * phi, l1mu + t[kBtA], S, zt);
+    ll -= S;
+    r = fmaf(mu, zt, r);
+    q -= zt;
+}
+
 
 }  // namespace tc

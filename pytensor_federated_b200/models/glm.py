@@ -9,7 +9,7 @@ Result per chain: ``[LL, dLL/dintercept[G], dLL/dbeta[P]]`` (float64).
 
 How a family's inputs map to the kernel (the input shapes, the theta words, the kernel's output blocks and the
 oracle's per-row terms) is decided by one layout object per family (``_Scalar``, ``_Softmax``, ``_Dispersion``,
-``_Ordinal``, ``_Survival``, ``_Positive``, ``_Hvp``, ``_ZeroInflated``, ``_LocationScale`` below); :class:`GlmShards` and its callers are generic over it.
+``_Ordinal``, ``_Survival``, ``_Positive``, ``_Beta``, ``_Hvp``, ``_ZeroInflated``, ``_LocationScale`` below); :class:`GlmShards` and its callers are generic over it.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ from .base import ShardModel
 
 FAMILIES = {"logistic": 0, "poisson": 1, "gaussian": 2, "multinomial": 3, "gaussian_scale": 4, "negative_binomial": 5,
             "ordinal": 6, "weibull": 7, "lognormal": 8, "zero_inflated_poisson": 9, "zero_inflated_negative_binomial": 10,
-            "gamma": 11, "inverse_gaussian": 12, "gaussian_location_scale": 13, "student_t": 14}
+            "gamma": 11, "inverse_gaussian": 12, "gaussian_location_scale": 13, "student_t": 14, "beta": 15}
 
 
 #: dynamic shared memory one CTA may opt in to on the H100 (227 KB), less 256 bytes for a kernel's static variables
@@ -233,6 +233,23 @@ class GlmShards(ShardModel):
         offsets and weights work as for every family.  Only the bf16 tensor-core kernel evaluates these families, with
         the shape limits of the multinomial one; ``n_classes``, ``events`` and ``hvp`` are rejected, and so is a shape
         whose 2K-column launch gets fewer than two pipeline stages (checked when an engine attaches the model).
+
+        ``"beta"`` is beta regression for continuous proportions strictly between 0 and 1 (Ferrari and Cribari-Neto;
+        R's ``betareg``, brms' ``Beta()``, statsmodels' ``BetaModel``): market shares, budget fractions, percent
+        cover, pass rates, allele frequencies.  The family name is not the coefficient input ``beta``.  The inputs and
+        gradients are those of ``negative_binomial``: ``(intercept, beta, log_dispersion)``, one chain or batched.
+        With ``eta = intercept[group] + x' beta + o``, the mean is ``mu = sigmoid(eta)`` (logit link), and ``a =
+        log_dispersion`` is the log of the PRECISION phi (a larger phi, less dispersion: ``Var(y) = mu (1 - mu) / (1 +
+        phi)``, as the log shape of ``gamma``).  With ``A = mu phi`` and ``B = (1 - mu) phi``:
+
+            ll = lgamma(phi) - lgamma(A) - lgamma(B) + (A - 1) log y + (B - 1) log(1 - y)
+
+        LL is the full density: it equals ``scipy.stats.beta(a=A, b=B).logpdf(y)``.  Unlike logistic regression on
+        fractional y (quasi-binomial), it is a density with a learned dispersion, so the posterior's width follows the
+        data.  Responses must be finite with ``0 < y < 1`` on every row of non-zero weight (a row of weight 0 may carry
+        any y, 0 and 1 included); offsets and weights work as for every family.  Only the bf16 tensor-core kernel
+        evaluates this family, with the shape limits of the multinomial one; ``n_classes``, ``events`` and ``hvp``
+        are rejected.
     events
         Per-row event indicators of the survival families (see ``family``).
     hvp
@@ -826,6 +843,18 @@ def _check_finite(m, what: str) -> None:
             raise ValueError(f"{what} of segment {si} must be finite on every row of non-zero weight")
 
 
+def _check_unit_interval(m, what: str) -> None:
+    """Every row of non-zero weight holds a finite y with 0 < y < 1."""
+    import torch
+
+    for si, (y, w) in enumerate(zip(m.ys, m.weights)):
+        bad = ~((y > 0) & (y < 1))   # NaN fails the comparisons
+        if w is not None:
+            bad &= w != 0   # a masked row may carry anything
+        if bool(torch.any(bad)):
+            raise ValueError(f"{what} of segment {si} must be finite with 0 < y < 1 on every row of non-zero weight")
+
+
 def _labels(y, w):
     """Integer labels of a chunk; masked rows may carry NaN or out-of-range labels: any valid class will do."""
     import torch
@@ -1052,6 +1081,15 @@ class _Positive(_Dispersion):
     def __init__(self, m, n_classes) -> None:
         super().__init__(m, n_classes)
         _check_positive(m, "responses")
+
+
+class _Beta(_Dispersion):
+    """``beta``: the layout of :class:`_Dispersion` with ``log_dispersion`` the log of the precision phi.  Every row
+    of non-zero weight must hold a finite y with 0 < y < 1."""
+
+    def __init__(self, m, n_classes) -> None:
+        super().__init__(m, n_classes)
+        _check_unit_interval(m, "responses")
 
 
 class _Softmax(_Layout):
@@ -1287,7 +1325,7 @@ _LAYOUTS = {"multinomial": _Softmax, "gaussian_scale": _Dispersion, "negative_bi
             "ordinal": _Ordinal, "weibull": _Survival, "lognormal": _Survival,
             "zero_inflated_poisson": _ZeroInflated, "zero_inflated_negative_binomial": _ZeroInflated,
             "gamma": _Positive, "inverse_gaussian": _Positive, "gaussian_location_scale": _LocationScale,
-            "student_t": _LocationScale}
+            "student_t": _LocationScale, "beta": _Beta}
 
 
 _LOG_SQRT_2PI = 0.918938533204672742
@@ -1534,9 +1572,100 @@ def _location_scale_terms(y, mu, s, a=None):
     return [pair(ll, torch.zeros_like(ll)), pair((nu + 1.0) * zr * sinv, (nu + 1.0) * p - 1.0), pair(qa, torch.zeros_like(qa))]
 
 
+#: the Stirling tail S(z) = lgamma(z) - [(z - 1/2) log z - z + log(2 pi) / 2] = sum_k c_k z^(1 - 2k) and z (psi(z) -
+#: log z) = -1/2 + sum_k d_k z^(1 - 2k): truncation errors below 1e-15 from z = 8 up
+_S_SERIES = [1.0 / 12, -1.0 / 360, 1.0 / 1260, -1.0 / 1680, 1.0 / 1188, -691.0 / 360360, 1.0 / 156]
+_T_SERIES = [-1.0 / 12, 1.0 / 120, -1.0 / 252, 1.0 / 240, -1.0 / 132, 691.0 / 32760, -1.0 / 12]
+#: 1 / (2 j + 3), j = 0 .. 17: the series of k(x) = x - log1p(x) in s = x / (2 + x) (see :func:`_kl_series`), to a
+#: truncation error below 1e-17 of k at |x| < 1/2
+_K_SERIES = [1.0 / (2 * j + 3) for j in range(18)]
+
+
+def _poly(x, coeffs):
+    """``sum_k coeffs[k] x^k`` by Horner's rule."""
+    import torch
+
+    acc = torch.full_like(x, coeffs[-1])
+    for c in reversed(coeffs[:-1]):
+        acc = acc * x + c
+    return acc
+
+
+def _beta_tails(z, lz):
+    """``(S(z), z tau(z))`` with ``S`` the Stirling tail of lgamma and ``tau(z) = psi(z) - log z``, ``lz = log z``
+    given: their asymptotic series from z = 8 up, ``lgamma`` and ``digamma`` below (where neither is large)."""
+    import torch
+
+    big = z >= 8.0
+    zb = torch.where(big, z, torch.full_like(z, 8.0))
+    zs = torch.where(big, torch.ones_like(z), z)
+    ls = torch.where(big, torch.zeros_like(z), lz)
+    i1 = 1.0 / zb
+    i2 = i1 * i1
+    S = torch.where(big, i1 * _poly(i2, _S_SERIES), torch.lgamma(zs) - (zs - 0.5) * ls + zs - _LOG_SQRT_2PI)
+    zt = torch.where(big, -0.5 + i1 * _poly(i2, _T_SERIES), zs * (torch.digamma(zs) - ls))
+    return S, zt
+
+
+def _beta_constants(a):
+    """``(phi, C(phi), Q(phi))`` per chain in float64 for ``phi = exp(a)``: ``C = (a - log 2 pi) / 2 + S(phi)`` and
+    ``Q = phi tau(phi)`` (:func:`_beta_tails`), both O(1) however large phi is: ``Q -> -1/2``."""
+    import torch
+
+    a = a.double()
+    phi = torch.exp(a)
+    S, Q = _beta_tails(phi, a)
+    return phi, 0.5 * a - _LOG_SQRT_2PI + S, Q
+
+
+def _kl_series(x):
+    """``k(x) = x - log1p(x)`` for |x| < 1/2, relatively accurate near 0 (where the difference loses ``2 eps / |x|``):
+    with ``s = x / (2 + x)``, ``log1p(x) = 2 atanh(s)`` and ``k = x s - 2 s^3 (1/3 + s^2 / 5 + s^4 / 7 + ...)``."""
+    s = x / (2.0 + x)
+    s2 = s * s
+    return x * s - 2.0 * s * s2 * _poly(s2, _K_SERIES)
+
+
+def _beta_terms(y, eta, a):
+    """``(ll, dll/deta, dll/da)`` of beta regression, ``mu = sigmoid(eta)``, precision ``phi = exp(a)``, ``A = mu
+    phi``, ``B = (1 - mu) phi``, in the grouped form that has no large cancellation (valid in float64 and float32):
+
+        ll = C(phi) + (log mu + log(1 - mu)) / 2 - log y - log(1 - y) - phi KL - S(A) - S(B),
+        dll/deta = phi mu (1 - mu) (logit y - logit mu) - (1 - mu) A tau(A) + mu B tau(B),
+        dll/da = Q(phi) - phi KL - A tau(A) - B tau(B),
+
+    with ``KL = mu log(mu / y) + (1 - mu) log((1 - mu) / (1 - y))`` (:func:`_beta_constants`, :func:`_beta_tails`).
+    ``logit y - logit mu = log1p(u) - log1p(v)`` and ``phi KL = A k(u) + B k(v)`` come from the relative differences
+    ``u = (y - mu) / mu`` and ``v = (mu - y) / (1 - mu)``: below |x| = 1/2 from :func:`_kl_series`, above from the logs
+    (``log1p(u) = log y - log mu``).  ``log mu = -softplus(-eta)``, ``1 - mu = sigmoid(-eta)``.  In float32 (the
+    collective backend) ``A`` and ``B`` underflow once ``|eta| + |a|`` nears 87; every test of that path stays inside."""
+    import torch
+
+    phi, C, Q = (v.to(eta.dtype) for v in _beta_constants(a))
+    a = a.to(eta.dtype)
+    ly, l1y = torch.log(y), torch.log1p(-y)
+    lmu, l1mu = -torch.nn.functional.softplus(-eta), -torch.nn.functional.softplus(eta)
+    mu, nmu = torch.sigmoid(eta), torch.sigmoid(-eta)
+    d = torch.where(eta >= 0, nmu - (1.0 - y), y - mu)   # y - mu, exact where y ~ mu
+    u, v = d / mu, -d / nmu
+    su, sv = u.abs() < 0.5, v.abs() < 0.5
+    ku = _kl_series(torch.where(su, u, torch.zeros_like(u)))
+    kv = _kl_series(torch.where(sv, v, torch.zeros_like(v)))
+    lu = torch.where(su, u - ku, ly - lmu)
+    lv = torch.where(sv, v - kv, l1y - l1mu)
+    lA, lB = lmu + a, l1mu + a
+    A, B = torch.exp(lA), torch.exp(lB)
+    kl = torch.where(su, A * ku, phi * d - A * lu) + torch.where(sv, B * kv, -phi * d - B * lv)
+    SA, tA = _beta_tails(A, lA)
+    SB, tB = _beta_tails(B, lB)
+    ll = C + 0.5 * (lmu + l1mu) - ly - l1y - kl - SA - SB
+    r = A * nmu * (lu - lv) - nmu * tA + mu * tB
+    return ll, r, Q - kl - tA - tB
+
+
 _DISPERSION_TERMS = {"gaussian_scale": _gaussian_scale_terms, "negative_binomial": _negative_binomial_terms,
                      "weibull": _weibull_terms, "lognormal": _lognormal_terms, "gamma": _gamma_terms,
-                     "inverse_gaussian": _inverse_gaussian_terms}
+                     "inverse_gaussian": _inverse_gaussian_terms, "beta": _beta_terms}
 
 
 def quantize_block_fp8(X, block: int = 32):
@@ -1852,6 +1981,38 @@ def synth_positive_shard(n_rows: int, n_features: int, *, family: str, shape: fl
         X[r0:r1] = xb
         mu = torch.exp(xb.float() @ beta_true + intercept).double()
         y[r0:r1] = draw_positive(mu, family=family, shape=shape, generator=gen)
+    return X, y, beta_true
+
+
+def synth_beta_shard(n_rows: int, n_features: int, *, phi: float, seed: int, device, chunk_rows: int = 1 << 20,
+                     beta_scale: float = 0.05, intercept: float = 0.5):
+    """Synthetic proportion shard generated on the device in chunks: bf16 ``X ~ N(0,1)`` and ``y ~ Beta(mu phi, (1 -
+    mu) phi)`` with ``mu = sigmoid(X beta* + intercept)``, drawn in float64 as ``sigmoid(log G_A - log G_B)`` from two
+    standard gamma draws taken in log space (``log G(c) = log G(c + 1) + log(U) / c``, which does not underflow at a
+    tiny shape c), and clamped into the open interval ``(0, 1)`` of float32 (``[2^-126, 1 - 2^-24]``).  Returns
+    ``(X, y, beta*)``."""
+    import torch
+
+    if not phi > 0:
+        raise ValueError(f"phi must be > 0, got {phi}")
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    beta_true = (torch.randn(n_features, generator=gen, device=device) * beta_scale).float()
+    X = torch.empty(n_rows, n_features, dtype=torch.bfloat16, device=device)
+    y = torch.empty(n_rows, dtype=torch.float32, device=device)
+    lo, hi = torch.finfo(torch.float32).tiny, 1.0 - 2.0 ** -24
+    for r0 in range(0, n_rows, chunk_rows):
+        r1 = min(n_rows, r0 + chunk_rows)
+        xb = torch.randn(r1 - r0, n_features, generator=gen, device=device, dtype=torch.float32).to(torch.bfloat16)
+        X[r0:r1] = xb
+        mu = torch.sigmoid(xb.float() @ beta_true + intercept).double()
+
+        def log_gamma_draw(c):
+            u = torch.rand(c.shape, generator=gen, device=device, dtype=torch.float64).clamp(min=1e-300)
+            return torch.log(torch._standard_gamma(c + 1.0, generator=gen)) + torch.log(u) / c
+
+        d = log_gamma_draw(mu * phi) - log_gamma_draw((1.0 - mu) * phi)
+        y[r0:r1] = torch.sigmoid(d).clamp(lo, hi).float()
     return X, y, beta_true
 
 

@@ -165,7 +165,8 @@ def glm_batch_fn(engine, n_groups: int) -> BatchFn:
 
     ``theta`` per chain is the model's inputs flattened row-major and concatenated
     (:meth:`~pytensor_federated_b200.models.GlmShards.inputs_from_theta`): ``[intercept (G, C), beta (P, C)]`` for a
-    multinomial engine, ``[intercept[G], beta[P], log_dispersion]`` for one with a dispersion parameter and
+    multinomial engine, ``[intercept[G], beta[P], log_dispersion]`` for one with a dispersion parameter (``beta``
+    regression's is the log precision) and
     ``[intercept[G], beta[P], cutpoints[C-1]]`` for an ordinal one, ``[intercept[G], beta[P], zi_intercept[G],
     zi_beta[P](, log_dispersion)]`` for a zero-inflated one and ``[intercept[G], beta[P], sigma_intercept[G],
     sigma_beta[P](, log_dispersion)]`` for a location-scale one.  ``n_groups`` is the model's G.  Gradients come back in

@@ -219,15 +219,33 @@ enum class Epi {
     Beta
 };
 
-__host__ __device__ constexpr bool has_dispersion(Epi e) {
-    return e == Epi::Dispersion || e == Epi::Survival || e == Epi::ZeroInflatedDisp || e == Epi::Positive ||
-           e == Epi::StudentT || e == Epi::Beta;
+// What the host and the kernel's shared code need to know about an epilogue
+struct EpiTraits {
+    bool disp;           // theta rows of stride G + P + 1, kDispWords per-chain constants (chain_constants), q
+    bool pair;           // chain k is the column pair (2k, 2k + 1), both predictors formed in one thread (not Hvp)
+    bool two_columns;    // at least two columns: no KC = 1 instance
+    bool group_panels;   // packed X: the decoders' registers allow two panels per load group
+};
+__host__ __device__ constexpr EpiTraits traits(Epi e) {
+    switch (e) {   // {disp, pair, two_columns, group_panels}
+        case Epi::Softmax: case Epi::Hvp: return {false, false, true, true};
+        case Epi::Dispersion: case Epi::Survival: case Epi::Positive: return {true, false, false, true};
+        case Epi::Ordinal: return {false, false, false, false};
+        case Epi::ZeroInflated: case Epi::LocationScale: return {false, true, true, true};
+        case Epi::ZeroInflatedDisp: case Epi::StudentT: return {true, true, true, true};
+        case Epi::Beta: return {true, false, false, false};
+        default: return {false, false, false, true};   // Scalar
+    }
 }
 
-// The epilogues whose chain k is the column pair (2k, 2k + 1), both predictors formed in one thread before either
-// column's values (Hvp pairs its columns too, but evaluates them one at a time)
-__host__ __device__ constexpr bool pair_epilogue(Epi e) {
-    return e == Epi::ZeroInflated || e == Epi::ZeroInflatedDisp || e == Epi::LocationScale || e == Epi::StudentT;
+// The per-chain constants of a traits(E).disp epilogue from the chain's log_dispersion ld
+template <Epi E>
+__device__ __forceinline__ void chain_constants(int family, float ld, float* t) {
+    if constexpr (E == Epi::Survival) survival_constants(ld, t);
+    else if constexpr (E == Epi::Positive) positive_constants(family, ld, t);
+    else if constexpr (E == Epi::StudentT) student_t_constants(ld, t);
+    else if constexpr (E == Epi::Beta) beta_constants(ld, t);
+    else dispersion_constants(family, ld, t);   // Dispersion; ZeroInflatedDisp: family 10's table is family 5's
 }
 
 constexpr Epi epilogue(int family) {
@@ -248,7 +266,7 @@ constexpr Epi epilogue(int family) {
 }
 static_assert([] {
     for (int code = 0; code <= kGlmBeta; ++code)
-        if (has_dispersion(epilogue(code)) != glm_family(code).dispersion) return false;
+        if (traits(epilogue(code)).disp != glm_family(code).dispersion) return false;
     return true;
 }(), "the epilogue's theta and output layout must match the family's");
 
@@ -285,10 +303,9 @@ template <int KC, bool ROWS, Epi E>
 __global__ void __launch_bounds__(kThreads, 1)
 fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams prm, const CUtensorMap* __restrict__ tmaps,
                   const GlmChunk* __restrict__ chunks, int n_chunks, unsigned int* __restrict__ work_counter) {
-    constexpr bool SOFTMAX = E == Epi::Softmax, DISP = has_dispersion(E), ORD = E == Epi::Ordinal,
+    constexpr bool SOFTMAX = E == Epi::Softmax, DISP = traits(E).disp, ORD = E == Epi::Ordinal,
                    SURV = E == Epi::Survival, HVP = E == Epi::Hvp, POS = E == Epi::Positive,
-                   PAIR = pair_epilogue(E), ZNB = E == Epi::ZeroInflatedDisp, STT = E == Epi::StudentT,
-                   BT = E == Epi::Beta;
+                   ZNB = E == Epi::ZeroInflatedDisp, STT = E == Epi::StudentT, BT = E == Epi::Beta;
     constexpr int C8 = cfg(KC).C8;
     constexpr int N1 = cfg(KC).N1;
     constexpr int N2 = cfg(KC).N2;
@@ -423,21 +440,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         for (size_t i = threadIdx.x; i < sum_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
             icpt_table[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
-        if constexpr (SURV)
+        if constexpr (DISP)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
-                survival_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
-        else if constexpr (POS)
-            for (int k = threadIdx.x; k < KC; k += blockDim.x)
-                positive_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
-        else if constexpr (STT)
-            for (int k = threadIdx.x; k < KC; k += blockDim.x)
-                student_t_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
-        else if constexpr (BT)
-            for (int k = threadIdx.x; k < KC; k += blockDim.x)
-                beta_constants(k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
-        else if constexpr (DISP)   // families 4 and 5, and 10, whose table is family 5's (any code but 4)
-            for (int k = threadIdx.x; k < KC; k += blockDim.x)
-                dispersion_constants(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
+                chain_constants<E>(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
         // Theta^T as the K-major, 128B-swizzled B operand of MMA #1: row n = term * C8 + chain
         for (int idx = threadIdx.x; idx < panels * N1 * 8; idx += blockDim.x) {
             const int j = idx & 7;              // 16-byte chunk (8 features) within the 128-byte row
@@ -546,7 +551,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 const int td = threadIdx.x - 32;
                 // panels per load group: 2 where the registers it needs do not push the instantiation into spills
                 // (ptxas -v; the consumers' epilogue sets the register count), else 1
-                constexpr int kDecGroup = KC <= 4 && !ORD && !BT ? 2 : 1;
+                constexpr int kDecGroup = KC <= 4 && traits(E).group_panels ? 2 : 1;
                 static_assert(kDecGroup <= 2, "a packed launch may have only 2 compressed slots");
                 int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
                 Ring stage, xs;
@@ -832,11 +837,11 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
 #pragma unroll
                         for (int jc = 0; jc < NJ; ++jc) {
                             float hv_h = 0.f;   // HVP: h = d2ll / deta2 of the pair's theta column (e = 0), for e = 1
-                            // PAIR: the pair's values (columns k0 = 8 jc + 2 q and k0 + 1), from both predictors, before
-                            // the column loop; offset and weight as in ROWS (the offset to the first predictor only).
+                            // traits(E).pair: the pair's values (columns k0 = 8 jc + 2 q and k0 + 1), from both predictors,
+                            // before the column loop; offset and weight as in ROWS (the offset to the first predictor only).
                             // n_chains is even, so k0 < nch covers both columns.
                             float pr_ll = 0.f, pr_r0 = 0.f, pr_r1 = 0.f, pr_q = 0.f;
-                            if constexpr (PAIR) {
+                            if constexpr (traits(E).pair) {
                                 const int k0 = 8 * jc + 2 * q;
                                 if (valid && k0 < nch) {
                                     float et = ((eacc[4 * jc + 2 * h] + eacc[4 * (NJ + jc) + 2 * h]) +
@@ -865,7 +870,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                                   eacc[4 * (2 * NJ + jc) + 2 * h + e];
                                 float ll = 0.f, r = 0.f, dq = 0.f;
                                 if (valid && k < nch) {
-                                    if constexpr (PAIR) {
+                                    if constexpr (traits(E).pair) {
                                         // column 2p: the pair's ll, the first predictor's r (and dll/dlog_dispersion);
                                         // 2p + 1: the second predictor's r
                                         ll = e == 0 ? pr_ll : 0.f;
@@ -877,13 +882,13 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                                         if constexpr (ROWS) et = __fadd_rn(et, o);
                                         const float* dt = disp + k * kDispWords;   // k < nch <= KC: inside the table
                                         if constexpr (SURV) {
-                                            if (prm.family == 7) weibull_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
+                                            if (prm.family == kGlmWeibull) weibull_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
                                             else lognormal_loglik(sv_event, sv_lt, et, dt, ll, r, dq);
                                         } else if constexpr (POS) {
                                             if (prm.family == kGlmGamma) gamma_loglik(pv_lt, et, dt, ll, r, dq);
                                             else inverse_gaussian_loglik(y, pv_lt, pv_iy, et, dt, ll, r, dq);
                                         } else {
-                                            if (prm.family == 4) gaussian_scale_loglik(y, et, dt, ll, r, dq);
+                                            if (prm.family == kGlmGaussianScale) gaussian_scale_loglik(y, et, dt, ll, r, dq);
                                             else negbin_loglik(y, et, dt, ll, r, dq);
                                         }
                                         if constexpr (ROWS) {
@@ -1050,7 +1055,7 @@ int chains_bucket(int k) { return k <= 1 ? 1 : (k <= 4 ? 4 : (k <= 8 ? 8 : (k <=
 // The shared-memory layout of a launch in bucket kc with epilogue e (the kernel derives the same one)
 tc::SmemLayout launch_layout(int n_features, int kc, tc::Epi e, int n_theta, bool rows, int row_data, bool packed = false) {
     return tc::smem_layout((n_features + 127) & ~127, tc::cfg(kc).N1, tc::cfg(kc).N2, n_theta,
-                           tc::has_dispersion(e) ? tc::kDispWords : 0, kc, tc::row_arrays(rows, row_data), packed);
+                           tc::traits(e).disp ? tc::kDispWords : 0, kc, tc::row_arrays(rows, row_data), packed);
 }
 
 using LaunchFn = int (*)(const FedComm*, const GlmSegment*, const GlmParams*, const void*, const void*, int, unsigned int*,
@@ -1067,14 +1072,14 @@ int launch(const FedComm* comm, const GlmSegment* segs_dev, const GlmParams* prm
                           n_chunks, work_counter);
 }
 
-// The kernel's instantiations: each epilogue in every K bucket, but none of Softmax, Hvp and the pair epilogues (two
-// columns at least) in KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are
+// The kernel's instantiations: each epilogue in every K bucket, but none that needs two columns at least
+// (traits().two_columns) in KC = 1 (null).  nvcc's code for a few of them depends on the order in which they are
 // instantiated, which is the order of the cases here: later epilogues go after the default.
 template <tc::Epi E>
 LaunchFn pick(int kc, bool rows) {
     switch (kc) {
         case 1:
-            if constexpr (E == tc::Epi::Softmax || E == tc::Epi::Hvp || tc::pair_epilogue(E)) return nullptr;
+            if constexpr (tc::traits(E).two_columns) return nullptr;
             else return rows ? launch<1, true, E> : launch<1, false, E>;
         case 4: return rows ? launch<4, true, E> : launch<4, false, E>;
         case 8: return rows ? launch<8, true, E> : launch<8, false, E>;
@@ -1168,7 +1173,7 @@ extern "C" int b200_glm_tc_chunk_table(const long long* n_rows, int n_segments, 
 // doubles in the partial array of the tensor-core kernel: one row of (hi, lo) pairs + per-warp LL slots per CTA
 extern "C" size_t b200_glm_tc_partial_row_doubles(int n_vals, int n_chains, int n_out, int n_groups, int family) {
     return tc::partial_row_doubles(n_vals, chains_bucket(n_chains), n_out > 0 ? n_out : 1, n_groups,
-                                   tc::has_dispersion(tc::epilogue(family)) ? 1 : 0);
+                                   tc::traits(tc::epilogue(family)).disp ? 1 : 0);
 }
 
 // Stages of the TMA ring the launch of this shape gets (host only; tests/test_glm_row_stream.py).  The launch

@@ -34,8 +34,8 @@ struct GlmParams {
     int n_segments;
     int n_features;       // P
     int ld;               // row stride of X in elements
-    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain (families 4, 5, 7, 8, 10 to 12, 14, 15: [.., log_dispersion])
-    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], families 4, 5, 7, 8, 10 to 12, 14, 15: [K][G+P+1])
+    int n_groups;         // G intercepts; theta = [intercept[G], beta[P]] per chain ([.., log_dispersion] where glm_family().dispersion)
+    int n_chains;         // K parameter vectors evaluated per launch (theta is [K][G+P], [K][G+P+1] with a dispersion word)
     int family;           // a GlmFamilyCode, or kGlmHvp | (0, 1 or 2)
     long long total_tiles;
     int n_out;            // output blocks: 1 = everything summed; > 1 = one [K][1+G+P] block per node (tensor-core kernel)

@@ -359,11 +359,12 @@ __device__ __forceinline__ double2 ld_cg_f64x2(const double* p) {
 constexpr unsigned int kReduceGroup = 16;   // CTAs per level-1 reduction group
 
 // Fixed-order sum of value v over rows [first, first + count) of a partial array with `stride` doubles per
-// row.  DD: rows hold (hi, lo) pairs and the result is a pair; otherwise plain doubles (lo stays 0).
-template <bool DD>
+// row.  DD: rows hold (hi, lo) pairs and the result is a pair; otherwise plain doubles (lo stays 0).  kWideDD: (hi, lo)
+// pairs of loads in flight per thread; the order of the additions does not depend on it.
+template <bool DD, unsigned int kWideDD = 16>
 __device__ __forceinline__ void sum_rows(const double* rows, size_t stride, int v, unsigned int first, unsigned int count,
                                          double& hi, double& lo) {
-    constexpr unsigned int kWide = DD ? 16 : 37;   // loads in flight per thread
+    constexpr unsigned int kWide = DD ? kWideDD : 37;   // loads in flight per thread
     hi = 0.0;
     lo = 0.0;
     for (unsigned int b = 0; b < count; b += kWide) {
@@ -391,7 +392,8 @@ __device__ __forceinline__ void sum_rows(const double* rows, size_t stride, int 
 // the critical path); the last group to finish sums the group partials, exchanges the node partial with the
 // root over NVLink, and the root publishes the result to the host.  Returns true in the one CTA that ran the
 // final stage (it may reset per-launch kernel state such as work counters).  Must be called by all threads.
-template <bool DD>
+// kWideDD: see sum_rows (a kernel that runs at 128 registers per thread needs fewer than 16 pairs in flight).
+template <bool DD, unsigned int kWideDD = 16>
 __device__ __forceinline__ bool epilogue_t(const FedComm& c, const Prologue& pro, unsigned long long status_in,
                                            size_t row_stride, double* group_buf) {
     __shared__ int s_last;
@@ -473,7 +475,7 @@ __device__ __forceinline__ bool epilogue_t(const FedComm& c, const Prologue& pro
     if (computed) {
         for (int v = threadIdx.x; v < nv; v += blockDim.x) {
             double hi, lo;
-            sum_rows<DD>(c.cta_partials, row_stride, v, grp_first, grp_size, hi, lo);
+            sum_rows<DD, kWideDD>(c.cta_partials, row_stride, v, grp_first, grp_size, hi, lo);
             group_buf[((size_t)grp * nv + v) * kW] = hi;
             if constexpr (DD) group_buf[((size_t)grp * nv + v) * kW + 1] = lo;
         }
@@ -529,7 +531,7 @@ __device__ __forceinline__ bool epilogue_t(const FedComm& c, const Prologue& pro
     }
     auto node_value = [&](int v) {
         double hi, lo;
-        sum_rows<DD>(group_buf, (size_t)nv * kW, v, 0u, n_groups, hi, lo);
+        sum_rows<DD, kWideDD>(group_buf, (size_t)nv * kW, v, 0u, n_groups, hi, lo);
         return hi + lo;   // DD: the one rounding of this node's partial
     };
 

@@ -14,7 +14,8 @@
 //
 // so the gradient GEMM costs no second pass over X.  Chains are batched along N (the MMA is
 // otherwise idle: the kernel is HBM-bound), which is what makes tensor cores pay here.
-// Roles: warp 0 = TMA producer; consumer warpgroups 1 and 2 (warps 4-11) share every tile: warpgroup c
+// Roles: warp 0 = TMA producer (packed X: warps 1-3 and 12-15 decode); consumer warpgroups 1 and 2 (warps 4-11), which
+// setmaxnreg gives 168 registers per thread against 88 for warpgroups 0 and 3, share every tile: warpgroup c
 // computes eta / the residuals of rows 64c .. 64c + 63 and the gradient of features c P/2 .. (c + 1) P/2 - 1,
 // so every gradient value has one owner thread.  One 256-thread barrier per tile publishes R; the two R
 // buffers alternate, so a buffer is rewritten only after both warpgroups have passed the next tile's barrier.
@@ -38,7 +39,12 @@ namespace tc {
 constexpr int kTileM = 128;          // rows per tile
 constexpr int kPanel = 64;           // features per 128-byte swizzle span
 constexpr int kPanelBytes = kTileM * 128;  // 16 KB
-constexpr int kThreads = 384;        // warpgroup 0: TMA producer (warp 0 only), warpgroups 1, 2: consumers
+constexpr int kThreads = 512;        // warpgroup 0: TMA producer (warp 0), packed-X decoders (warps 1 to 3);
+                                     // warpgroups 1, 2: consumers; warpgroup 3: packed-X decoders
+constexpr int kRegs = 65536 / kThreads;   // registers per thread at launch (128), and in the CTA's shared code
+constexpr int kConsumerRegs = 168;   // registers per thread of the consumer warpgroups in their role (setmaxnreg) ...
+constexpr int kOtherRegs = 88;       // ... and of warpgroups 0 and 3 in theirs: 256 x 168 + 256 x 88 = 65536
+static_assert(256 * kConsumerRegs + 256 * kOtherRegs == 65536, "the register split must fill the register file");
 constexpr int kConsumerWarps = 8;
 constexpr int kMaxChunk = 32;        // tiles per chunk at most (= tiles accumulated in fp32 registers before a flush)
 constexpr int kMinChunk = 4;
@@ -51,13 +57,13 @@ constexpr int kLLRows = 16;          // per-warp log-likelihood slot rows (>= kC
 // feature in the low nibble), code c < 15 standing for the high byte in entry c of the segment's table (entry 0 is
 // 0x00, which padding uses) and 15 for an exception.  A tile's kXFoot-byte footer holds the exception count and up
 // to kXMaxExceptions words (position in the tile << 8 | high byte), position = panel * 8192 + row * 64 + feature.
-// The producer (warp 0) streams the blocks into a ring of kXSlots slots with cp.async.bulk; warps 1 to 3 decode
-// each panel into the 128B-swizzled image TMA would have written, so the consumers see the same stage bytes.
+// The producer (warp 0) streams the blocks into a ring of kXSlots slots with cp.async.bulk; warps 1 to 3 and 12 to 15
+// decode each panel into the 128B-swizzled image TMA would have written, so the consumers see the same stage bytes.
 constexpr int kXBlock = kTileM * kPanel * 3 / 2;   // 12 KB
 constexpr int kXFoot = 256;
 constexpr int kXMaxExceptions = kXFoot / 4 - 1;
 constexpr int kXSlots = 6;                           // compressed panel slots at most
-constexpr int kDecThreads = 96;                      // warps 1 to 3
+constexpr int kDecThreads = 224;                     // warps 1 to 3 and 12 to 15
 
 // prmt.b32 (byte permute; selector nibble bit 3 replicates the sign of the selected byte)
 __host__ __device__ __forceinline__ uint32_t x12_prmt(uint32_t a, uint32_t b, uint32_t s) {
@@ -321,7 +327,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     const int panels = PP / kPanel;
     // row slot of a stage: y, then the offsets and the weights when some segment of the launch has them
     const int o_slot = 1, w_slot = ROWS && (prm.row_data & kGlmRowOffsets) ? 2 : 1;
-    const bool PK = prm.packed_x != 0;   // X packed: warp 0 loads compressed panels, warps 1 to 3 decode them
+    const bool PK = prm.packed_x != 0;   // X packed: warp 0 loads compressed panels, warps 1 to 3 and 12 to 15 decode them
     const SmemLayout L = smem_layout(PP, N1, N2, comm.n_theta, DISP ? kDispWords : 0, KC, row_arrays(ROWS, prm.row_data), PK);
     const int S = (int)L.stages;
     const int nch = prm.n_chains < KC ? prm.n_chains : KC;  // chains actually present in theta
@@ -423,23 +429,41 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         }
     }
 
-    fed::Prologue pro = fed::prologue(comm, theta_f);   // contains __syncthreads()
-    const bool active = !pro.stop && !pro.timed_out;
+    // Nothing that lives from here to the CTA's tail may stay in a register across the role loops below: there it
+    // would take one of the consumers' registers in their setmaxnreg region, and at K = 16 it would be spilled.  So
+    // the prologue's result waits in shared memory (thread 0 writes it, every thread reads it after the barrier before
+    // the tail), and this CTA's row of the partial array is recomputed from the launch parameters and the block index
+    // where it is used (opaque() keeps the compiler from merging the copies into one long-lived value).
+    __shared__ fed::Prologue s_pro;
+    bool active;
+    {
+        const fed::Prologue pro = fed::prologue(comm, theta_f);   // contains __syncthreads()
+        if (threadIdx.x == 0) s_pro = pro;
+        active = !pro.stop && !pro.timed_out;
+    }
     const int NOUT = prm.n_out;       // output blocks (1 = everything summed; else one per node)
     const int NS1 = 1 + G + DISP;     // warp-level values per (block, chain): LL, the G intercept gradients (and q)
-    const size_t row_doubles = partial_row_doubles(comm.n_vals, KC, NOUT, G, DISP);
-    double* out = comm.cta_partials + (size_t)blockIdx.x * row_doubles;   // this CTA's running sums, (hi, lo) pairs
-    const size_t sum_doubles = partial_sum_doubles(comm.n_vals, KC, NOUT, G, DISP);
+    auto row_doubles = [&] { return partial_row_doubles(opaque(comm.n_vals), KC, NOUT, G, DISP); };
+    // this CTA's running sums, (hi, lo) pairs
+    auto cta_row = [&]() -> double* { return comm.cta_partials + (size_t)blockIdx.x * row_doubles(); };
     // [KC][G] intercepts, in global memory so that the shared memory budget does not grow with G: written in the
     // setup below, read by this CTA only (after __syncthreads), one column into `icpt` per chunk
-    float* icpt_table = reinterpret_cast<float*>(out + sum_doubles);
-    double* ll_slots = out + 2 * (size_t)comm.n_vals;                     // [kLLRows][NOUT][KC][NS1] pairs
+    auto icpt_table = [&]() -> float* {
+        return reinterpret_cast<float*>(cta_row() + partial_sum_doubles(opaque(comm.n_vals), KC, NOUT, G, DISP));
+    };
+    // [kLLRows][NOUT][KC][NS1] pairs
+    auto ll_slots = [&]() -> double* { return cta_row() + 2 * (size_t)opaque(comm.n_vals); };
 
     if (active) {
         // ---------------- theta-dependent setup --------------------------------------------------
-        for (size_t i = threadIdx.x; i < sum_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
+        {
+            double* out = cta_row();
+            const size_t sum_doubles = partial_sum_doubles(comm.n_vals, KC, NOUT, G, DISP);
+            for (size_t i = threadIdx.x; i < sum_doubles / 2; i += blockDim.x) reinterpret_cast<double2*>(out)[i] = make_double2(0.0, 0.0);
+        }
+        float* const itab = icpt_table();
         for (int i = threadIdx.x; i < KC * G; i += blockDim.x)
-            icpt_table[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
+            itab[i] = (i / G) < nch ? theta_f[(i / G) * (G + P + DISP) + (i % G)] : 0.f;   // theta row stride G + P (+ 1)
         if constexpr (DISP)
             for (int k = threadIdx.x; k < KC; k += blockDim.x)
                 chain_constants<E>(prm.family, k < nch ? theta_f[k * (G + P + 1) + G + P] : 0.f, disp + k * kDispWords);
@@ -491,144 +515,160 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
             // the intercepts of the chunk's group (ring entry .w); every reader of the previous column has passed the
             // barrier above
             if (threadIdx.x >= 128 && threadIdx.x < 128 + KC && !*pipeline_fault() && ring[slot].x >= 0)
-                icpt[threadIdx.x - 128] = __ldcg(icpt_table + (threadIdx.x - 128) * G + ring[slot].w);
+                icpt[threadIdx.x - 128] = __ldcg(icpt_table() + (threadIdx.x - 128) * G + ring[slot].w);
             named_sync(1, 256);
             return *chunk_decided;
         };
 
-        if (warp == 0) {
-            // ================= TMA producer + chunk scheduler ==================================
-            // The role loops are warp-uniform (all 32 lanes wait and count); only the issue is predicated on
-            // elect.sync, so the compiler keeps addresses / descriptors in uniform registers.
-            Ring stage, xs;
-            unsigned int claim = claim0, ahead = 0;   // the first chunk was claimed before theta arrived
-            for (int j = 0;; ++j) {
-                const bool have = claim < (unsigned int)n_chunks;
-                GlmChunk ch{};
-                if (have) ch = chunks[claim];
-                if (lane == 0) {
-                    ring[j & (kRing - 1)] = have ? make_int4(ch.seg, ch.first_tile * kTileM, ch.n_tiles, segs_g[ch.seg].group)
-                                                 : make_int4(-1, 0, 0, 0);
-                    mbar_arrive(&bar_ring[j & (kRing - 1)]);
-                    if (have) ahead = atomicAdd(work_counter, 1u);   // next claim: the round trip hides behind this chunk
-                }
-                __syncwarp();
-                if (!have) break;
-                const int rows = seg_row_mask(ch.seg);
-                for (int t = 0; t < ch.n_tiles && PK; ++t)
-                    for (int pnl = 0; pnl < panels; ++pnl) {
-                        const int k = t * panels + pnl;
-                        if (!(j == 0 && k < preloaded)) {   // else already in flight (early loads)
-                            mbar_wait(&bar_xempty[xs.idx], xs.phase ^ 1);
-                            if (j == 0 && k == preloaded && lane == 0) fed::stamp(comm, 3);
-                            if (elect_one()) load_xpanel(xs.idx, ch.seg, ch.first_tile + t, pnl, rows);
-                            __syncwarp();
-                        }
-                        xs.advance((int)L.xslots);
-                    }
-                for (int t = 0; t < ch.n_tiles && !PK; ++t) {
-                    const int st = stage.idx;
-                    if (j == 0 && t < preloaded) {   // already in flight (early loads)
-                        stage.advance(S);
-                        continue;
-                    }
-                    mbar_wait(&bar_empty[st], stage.phase ^ 1);
-                    if (j == 0 && t == preloaded && lane == 0) fed::stamp(comm, 3);
-                    if (elect_one()) load_tile(st, ch.seg, (ch.first_tile + t) * kTileM, rows);
-                    __syncwarp();
-                    stage.advance(S);
-                }
-                claim = __shfl_sync(0xffffffffu, ahead, 0);
-            }
-            if (lane == 0) fed::stamp(comm, 4);
-        } else if (warp < 4) {
-            // ================= PK: decoders (warps 1 to 3) ==========================================
-            // Per tile: wait for a free stage, decode its panels in order as their compressed slots land (the slot is
-            // released right after), copy the footer (double-buffered by tile parity: the barrier below orders every
-            // read of buffer b before its next write, two tiles later) and the row data, then patch the exceptions
-            // once all 96 threads' stores are in, and arrive on full[stage] after a proxy fence.
-            if (PK) {
-                const int td = threadIdx.x - 32;
-                // panels per load group: 2 where the registers it needs do not push the instantiation into spills
-                // (ptxas -v; the consumers' epilogue sets the register count), else 1
-                constexpr int kDecGroup = KC <= 4 && traits(E).group_panels ? 2 : 1;
-                static_assert(kDecGroup <= 2, "a packed launch may have only 2 compressed slots");
-                int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
+        // Registers go where the work needs them: the consumer warpgroups' epilogues get kConsumerRegs per thread, the
+        // producer and the decoders (warpgroups 0 and 3) kOtherRegs.  setmaxnreg is per warpgroup, so each side
+        // changes its count at the top of its branch (warp 0 together with warps 1 to 3) and returns to kRegs at its
+        // end, before the CTA's shared tail below, on every path (packed or not, and after a stalled pipeline).
+        // Warpgroups 0 and 3 take their registers back only after barrier 3, which the consumers reach once they have
+        // returned theirs: an idle warpgroup (bf16 X, or a CTA without work) that took them back at once could leave
+        // a consumer warpgroup waiting for registers forever, and the other one with it at their named barrier.
+        if (warp < 4 || warp >= 12) {
+            setmaxnreg<kRegs, kOtherRegs>();
+            if (warp == 0) {
+                // ================= TMA producer + chunk scheduler ==================================
+                // The role loops are warp-uniform (all 32 lanes wait and count); only the issue is predicated on
+                // elect.sync, so the compiler keeps addresses / descriptors in uniform registers.
                 Ring stage, xs;
-                uint32_t fb = 0;
+                unsigned int claim = claim0, ahead = 0;   // the first chunk was claimed before theta arrived
                 for (int j = 0;; ++j) {
-                    // decide each chunk together, as the consumers do: a decoder warp leaving on a stalled pipeline
-                    // while the others wait at the barrier below would hang
-                    mbar_wait(&bar_ring[j & (kRing - 1)], (uint32_t)((j / kRing) & 1));
-                    named_sync(2, kDecThreads);
-                    if (td == 0) *decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[j & (kRing - 1)];
-                    named_sync(2, kDecThreads);
-                    const int4 ch = *decided;
-                    if (ch.x < 0) break;
-                    const uint32_t tab[4] = {segs_g[ch.x].xtab[0], segs_g[ch.x].xtab[1], segs_g[ch.x].xtab[2],
-                                             segs_g[ch.x].xtab[3]};
-                    for (int t = 0; t < ch.z; ++t) {
-                        mbar_wait(&bar_empty[stage.idx], stage.phase ^ 1);
-                        unsigned char* dst = smem + (size_t)stage.idx * L.stage_bytes;
-                        int* foot = reinterpret_cast<int*>(smem + L.off_xfoot + fb * kXFoot);
-                        // panels in groups of kDecGroup: all of this thread's loads of a group's panels first, then
-                        // their decodes and stores.  One warp per scheduler runs this, so the shared-memory latency is
-                        // hidden by ILP, not by warps: a group keeps kDecGroup panels of loads in flight.  A group holds
-                        // kDecGroup slots at once: a packed launch has at least 2 slots (launch() refuses fewer) and 2 or
-                        // 4 panels, so a group of 2 always fits and divides the tile.
-                        for (int pnl = 0; pnl < panels; pnl += kDecGroup) {
-                            constexpr int kPer = (kTileM * 8 + kDecThreads - 1) / kDecThreads;
-                            uint2 lo[kDecGroup][kPer];
-                            uint32_t cw[kDecGroup][kPer];
-                            int xi[kDecGroup];
-#pragma unroll
-                            for (int h = 0; h < kDecGroup; ++h) {
-                                mbar_wait(&bar_xfull[xs.idx], xs.phase);
-                                const unsigned char* src = smem + L.off_x + (size_t)xs.idx * L.xslot_bytes;
-                                if (pnl + h == 0) {
-                                    if (td < kXFoot / 4) foot[td] = reinterpret_cast<const int*>(src + kXBlock)[td];
-                                    const float* rsrc = reinterpret_cast<const float*>(src + kXBlock + kXFoot);
-                                    float* rdst = reinterpret_cast<float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
-                                    for (int i = td; i < (int)L.row_bytes / 4; i += kDecThreads) rdst[i] = rsrc[i];
-                                }
-#pragma unroll
-                                for (int k = 0; k < kPer; ++k) {
-                                    const int i = td + k * kDecThreads;
-                                    if (k < kPer - 1 || i < kTileM * 8) {
-                                        lo[h][k] = reinterpret_cast<const uint2*>(src)[i];
-                                        cw[h][k] = reinterpret_cast<const uint32_t*>(src + kTileM * kPanel)[i];
-                                    }
-                                }
-                                xi[h] = xs.idx;
-                                xs.advance((int)L.xslots);
+                    const bool have = claim < (unsigned int)n_chunks;
+                    GlmChunk ch{};
+                    if (have) ch = chunks[claim];
+                    if (lane == 0) {
+                        ring[j & (kRing - 1)] = have ? make_int4(ch.seg, ch.first_tile * kTileM, ch.n_tiles, segs_g[ch.seg].group)
+                                                     : make_int4(-1, 0, 0, 0);
+                        mbar_arrive(&bar_ring[j & (kRing - 1)]);
+                        if (have) ahead = atomicAdd(work_counter, 1u);   // next claim: the round trip hides behind this chunk
+                    }
+                    __syncwarp();
+                    if (!have) break;
+                    const int rows = seg_row_mask(ch.seg);
+                    for (int t = 0; t < ch.n_tiles && PK; ++t)
+                        for (int pnl = 0; pnl < panels; ++pnl) {
+                            const int k = t * panels + pnl;
+                            if (!(j == 0 && k < preloaded)) {   // else already in flight (early loads)
+                                mbar_wait(&bar_xempty[xs.idx], xs.phase ^ 1);
+                                if (j == 0 && k == preloaded && lane == 0) fed::stamp(comm, 3);
+                                if (elect_one()) load_xpanel(xs.idx, ch.seg, ch.first_tile + t, pnl, rows);
+                                __syncwarp();
                             }
-#pragma unroll
-                            for (int h = 0; h < kDecGroup; ++h) {
-                                unsigned char* pd = dst + (pnl + h) * kPanelBytes;
-#pragma unroll
-                                for (int k = 0; k < kPer; ++k) {
-                                    const int i = td + k * kDecThreads;
-                                    if (k < kPer - 1 || i < kTileM * 8)
-                                        *reinterpret_cast<uint4*>(pd + x12_chunk_offset(i)) = x12_decode8(lo[h][k], cw[h][k], tab);
-                                }
-                                mbar_arrive(&bar_xempty[xi[h]]);
-                            }
+                            xs.advance((int)L.xslots);
                         }
-                        named_sync(2, kDecThreads);   // the tile's decoded chunks and its footer are in
-                        const int n_ex = min(foot[0], kXMaxExceptions);
-                        for (int e = td; e < n_ex; e += kDecThreads) {
-                            const uint32_t v = (uint32_t)foot[1 + e];
-                            if ((v >> 8) < (uint32_t)panels * kTileM * kPanel) dst[x12_high_byte_offset(v >> 8)] = (unsigned char)(v & 0xFFu);
+                    for (int t = 0; t < ch.n_tiles && !PK; ++t) {
+                        const int st = stage.idx;
+                        if (j == 0 && t < preloaded) {   // already in flight (early loads)
+                            stage.advance(S);
+                            continue;
                         }
-                        fence_proxy_async();
-                        mbar_arrive(&bar_full[stage.idx]);
+                        mbar_wait(&bar_empty[st], stage.phase ^ 1);
+                        if (j == 0 && t == preloaded && lane == 0) fed::stamp(comm, 3);
+                        if (elect_one()) load_tile(st, ch.seg, (ch.first_tile + t) * kTileM, rows);
+                        __syncwarp();
                         stage.advance(S);
-                        fb ^= 1u;
+                    }
+                    claim = __shfl_sync(0xffffffffu, ahead, 0);
+                }
+                if (lane == 0) fed::stamp(comm, 4);
+            } else {
+                // ================= PK: decoders (warps 1 to 3 and 12 to 15) =============================
+                // Per tile: wait for a free stage, decode its panels in order as their compressed slots land (the slot is
+                // released right after), copy the footer (double-buffered by tile parity: the barrier below orders every
+                // read of buffer b before its next write, two tiles later) and the row data, then patch the exceptions
+                // once all 224 threads' stores are in, and arrive on full[stage] after a proxy fence.  Every decoder thread
+                // reads every slot (the chunks of a panel are strided over all 224), so every one of them releases it.
+                if (PK) {
+                    const int td = warp < 4 ? threadIdx.x - 32 : threadIdx.x - (12 * 32 - 96);   // 0 to 95, 96 to 223
+                    // panels per load group: 2 where the registers it needs did not push the instantiation into
+                    // spills when the whole kernel had one register count (ptxas -v), else 1.  With seven decoder warps
+                    // and kOtherRegs of their own, groups of 1 measured slower at K = 1 (docs/KERNELS.md)
+                    constexpr int kDecGroup = KC <= 4 && traits(E).group_panels ? 2 : 1;
+                    static_assert(kDecGroup <= 2, "a packed launch may have only 2 compressed slots");
+                    int4* decided = reinterpret_cast<int4*>(smem + L.off_bars + 144);
+                    Ring stage, xs;
+                    uint32_t fb = 0;
+                    for (int j = 0;; ++j) {
+                        // decide each chunk together, as the consumers do: a decoder warp leaving on a stalled pipeline
+                        // while the others wait at the barrier below would hang
+                        mbar_wait(&bar_ring[j & (kRing - 1)], (uint32_t)((j / kRing) & 1));
+                        named_sync(2, kDecThreads);
+                        if (td == 0) *decided = *pipeline_fault() ? make_int4(-1, 0, 0, 0) : ring[j & (kRing - 1)];
+                        named_sync(2, kDecThreads);
+                        const int4 ch = *decided;
+                        if (ch.x < 0) break;
+                        const uint32_t tab[4] = {segs_g[ch.x].xtab[0], segs_g[ch.x].xtab[1], segs_g[ch.x].xtab[2],
+                                                 segs_g[ch.x].xtab[3]};
+                        for (int t = 0; t < ch.z; ++t) {
+                            mbar_wait(&bar_empty[stage.idx], stage.phase ^ 1);
+                            unsigned char* dst = smem + (size_t)stage.idx * L.stage_bytes;
+                            int* foot = reinterpret_cast<int*>(smem + L.off_xfoot + fb * kXFoot);
+                            // panels in groups of kDecGroup: all of this thread's loads of a group's panels first,
+                            // then their decodes and stores.  Two decoder warps share each scheduler but warp 0's (one),
+                            // so the shared-memory latency is hidden by those warps and by ILP: a group keeps kDecGroup
+                            // panels of loads in flight.  A group holds kDecGroup slots at once: a packed launch has at
+                            // least 2 slots (launch() refuses fewer) and 2 or 4 panels, so a group of 2 always fits and
+                            // divides the tile.
+                            for (int pnl = 0; pnl < panels; pnl += kDecGroup) {
+                                constexpr int kPer = (kTileM * 8 + kDecThreads - 1) / kDecThreads;
+                                uint2 lo[kDecGroup][kPer];
+                                uint32_t cw[kDecGroup][kPer];
+                                int xi[kDecGroup];
+#pragma unroll
+                                for (int h = 0; h < kDecGroup; ++h) {
+                                    mbar_wait(&bar_xfull[xs.idx], xs.phase);
+                                    const unsigned char* src = smem + L.off_x + (size_t)xs.idx * L.xslot_bytes;
+                                    if (pnl + h == 0) {
+                                        if (td < kXFoot / 4) foot[td] = reinterpret_cast<const int*>(src + kXBlock)[td];
+                                        const float* rsrc = reinterpret_cast<const float*>(src + kXBlock + kXFoot);
+                                        float* rdst = reinterpret_cast<float*>(smem + L.off_rows + (size_t)stage.idx * L.row_bytes);
+                                        for (int i = td; i < (int)L.row_bytes / 4; i += kDecThreads) rdst[i] = rsrc[i];
+                                    }
+#pragma unroll
+                                    for (int k = 0; k < kPer; ++k) {
+                                        const int i = td + k * kDecThreads;
+                                        if (k < kPer - 1 || i < kTileM * 8) {
+                                            lo[h][k] = reinterpret_cast<const uint2*>(src)[i];
+                                            cw[h][k] = reinterpret_cast<const uint32_t*>(src + kTileM * kPanel)[i];
+                                        }
+                                    }
+                                    xi[h] = xs.idx;
+                                    xs.advance((int)L.xslots);
+                                }
+#pragma unroll
+                                for (int h = 0; h < kDecGroup; ++h) {
+                                    unsigned char* pd = dst + (pnl + h) * kPanelBytes;
+#pragma unroll
+                                    for (int k = 0; k < kPer; ++k) {
+                                        const int i = td + k * kDecThreads;
+                                        if (k < kPer - 1 || i < kTileM * 8)
+                                            *reinterpret_cast<uint4*>(pd + x12_chunk_offset(i)) = x12_decode8(lo[h][k], cw[h][k], tab);
+                                    }
+                                    mbar_arrive(&bar_xempty[xi[h]]);
+                                }
+                            }
+                            named_sync(2, kDecThreads);   // the tile's decoded chunks and its footer are in
+                            const int n_ex = min(foot[0], kXMaxExceptions);
+                            for (int e = td; e < n_ex; e += kDecThreads) {
+                                const uint32_t v = (uint32_t)foot[1 + e];
+                                if ((v >> 8) < (uint32_t)panels * kTileM * kPanel) dst[x12_high_byte_offset(v >> 8)] = (unsigned char)(v & 0xFFu);
+                            }
+                            fence_proxy_async();
+                            mbar_arrive(&bar_full[stage.idx]);
+                            stage.advance(S);
+                            fb ^= 1u;
+                        }
                     }
                 }
             }
+            named_sync(3, kThreads);   // every consumer has returned its registers
+            setmaxnreg<kOtherRegs, kRegs>();
         } else {
-            // ================= consumer warpgroups ===============================================
+            // ================= consumer warpgroups (warps 4 to 11) ===============================
+            setmaxnreg<kRegs, kConsumerRegs>();
             const int c = (warp >> 2) - 1;          // rows 64c .. 64c + 63 of every tile, gradient features c PP/2 ..
             const int w = warp & 3;                 // warp within the group: accumulator rows 16w .. 16w + 15
             const int q = lane & 3;                 // column pair of the accumulator fragment
@@ -983,6 +1023,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                 // per-thread fp32 sums over the chunk's tiles -> fixed butterfly over the 8 lanes that share the
                 // chains (double) -> lanes 0..3 add the warp's value to its own slot: every step depends on the
                 // chunk only.
+                double* const out = cta_row();
+                double* const slots = out + 2 * (size_t)comm.n_vals;
 #pragma unroll
                 for (int s = 0; s < 2 * NJ; ++s) {
                     double lsum = (double)ll_acc[s], gsum = (double)gi_acc[s], dsum = (double)ds_acc[s];
@@ -994,7 +1036,7 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                     }
                     const int k = 8 * (s >> 1) + 2 * q + (s & 1);
                     if (lane < 4 && k < nch) {
-                        double* slot = ll_slots + 2 * ((((size_t)ew * NOUT + og) * KC + k) * NS1);
+                        double* slot = slots + 2 * ((((size_t)ew * NOUT + og) * KC + k) * NS1);
                         dd_accumulate(slot, lsum);
                         dd_accumulate(slot + 2 * (1 + seg_group), gsum);
                         if constexpr (DISP) dd_accumulate(slot + 2 * (1 + G), dsum);
@@ -1016,6 +1058,8 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
                             }
                     }
             }
+            setmaxnreg<kConsumerRegs, kRegs>();
+            named_sync(3, kThreads);
         }
 
         // ---------------- CTA partial: fold the per-warp LL slots and the intercept gradients ----------
@@ -1024,11 +1068,13 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
         if (threadIdx.x == 0) fed::stamp(comm, 5);
         // layout per (output block, chain): [LL, gi[G], g[P]] as (hi, lo) pairs (DISP: then dlog_dispersion);
         // g[] was accumulated in place, LL, gi[] (and dlog_dispersion) are the per-warp slots summed in warp order
+        double* const out = cta_row();
+        const double* const slots = ll_slots();
         for (int i = threadIdx.x; i < NOUT * nch * NS1; i += blockDim.x) {
             const int j = i % NS1, k = (i / NS1) % nch, o = i / (NS1 * nch);
             double hi = 0.0, lo = 0.0;
             for (int w = 0; w < kConsumerWarps; ++w) {
-                const double* slot = ll_slots + 2 * ((((size_t)w * NOUT + o) * KC + k) * NS1 + j);
+                const double* slot = slots + 2 * ((((size_t)w * NOUT + o) * KC + k) * NS1 + j);
                 fed::dd_add(hi, lo, slot[0], slot[1]);
             }
             const int jo = (DISP && j == 1 + G) ? 1 + G + P : j;   // slot 1 + G: the last value of the block
@@ -1042,7 +1088,9 @@ fed_glm_tc_kernel(FedComm comm, const GlmSegment* __restrict__ segs_g, GlmParams
     }
     __syncthreads();
     const unsigned long long status = *pipeline_fault() ? B200FED_ERR_PIPELINE : 0ull;
-    const bool fin = fed::epilogue_t<true>(comm, pro, status, row_doubles, comm.group_partials);
+    const fed::Prologue pro = s_pro;
+    // 12 (hi, lo) pairs of loads in flight in the final sums: 16 would not fit the 128 registers of the tail
+    const bool fin = fed::epilogue_t<true, 12>(comm, pro, status, row_doubles(), comm.group_partials);
     if (fin && threadIdx.x == 0) *work_counter = 0u;   // every CTA has stopped claiming: ready for the next launch
 }
 

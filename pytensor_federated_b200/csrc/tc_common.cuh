@@ -105,6 +105,23 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 // Named barrier over `count` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
+// v, as a value the compiler cannot prove equal to another copy of it: what is computed from it is recomputed where it
+// is used instead of being kept in a register from its first use on
+__device__ __forceinline__ int opaque(int v) {
+    asm volatile("" : "+r"(v));
+    return v;
+}
+
+// Register reallocation between warpgroups (setmaxnreg): the calling warpgroup's registers per thread go from `From`
+// to `To`, taken from the CTA's pool (inc, which blocks until the pool holds them) or given back to it (dec).  Every
+// thread of the warpgroup executes the same instruction, and ptxas allocates the code after it within `To` registers.
+template <int From, int To>
+__device__ __forceinline__ void setmaxnreg() {
+    static_assert(To % 8 == 0 && To >= 24 && To <= 256 && To != From, "setmaxnreg: a multiple of 8 in [24, 256]");
+    if constexpr (To > From) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(To));
+    else asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(To));
+}
+
 // ------------------------------------------------------------------ wgmma (sm_90a)
 // Warpgroup MMA: 128 threads (4 consecutive warps, the first a multiple of 4) issue together; the fp32
 // accumulator of an m64nN tile lives in registers, N / 2 per thread: d[4j + 2h + e] = (row 16 w + lane / 4 + 8 h,

@@ -46,7 +46,7 @@ LL_TERMS = {"tc": 64, "fp8": 60, "simt": 256, "generic": 512}
 # ------------------------------------------------------------------------------------------------ cases
 @dataclass
 class Seg:
-    X: np.ndarray               # int64 [n, P]: the stored design matrix times 2^xs
+    X: np.ndarray               # int64 or int16 [n, P]: the stored design matrix times 2^xs
     y: np.ndarray               # int64 [n], grid units (0 where the row is NaN)
     o: Optional[np.ndarray]     # int64 [n] grid units, or None
     w: Optional[np.ndarray]     # int64 [n], or None (weight 1)
@@ -55,13 +55,14 @@ class Seg:
     node: int
     xq: Optional[np.ndarray] = None   # fp8: e4m3 integers [n, P]
     sc: Optional[np.ndarray] = None   # fp8: UE8M0 scale bytes [4 ceil(n / 128), P / 32]
+    nz: Optional[np.ndarray] = None   # [m, 2] (row, feature) of zeros of X stored as -0.0
 
 
 @dataclass
 class Case:
     name: str
     kernel: str            # "tc", "fp8", "simt", "generic" or "custom" (CustomFamily on the general-shape kernel)
-    family: str            # "gaussian" or "gaussian_scale"
+    family: str            # "gaussian", "gaussian_scale" or "gaussian_location_scale" (its scale at 0)
     P: int
     K: int
     G: int
@@ -84,6 +85,15 @@ class Case:
         return self.family == "gaussian_scale"
 
     @property
+    def pair(self) -> bool:
+        """Chain k runs as kernel columns 2k (the mean: ic, beta) and 2k + 1 (the log scale: all coefficients 0)."""
+        return self.family == "gaussian_location_scale"
+
+    @property
+    def columns(self) -> int:
+        return 2 * self.K if self.pair else self.K
+
+    @property
     def n_rows(self) -> List[int]:
         return [s.X.shape[0] for s in self.segs]
 
@@ -91,6 +101,8 @@ class Case:
         ic = (self.ic * 2.0 ** -self.e).astype(np.float32)
         beta = (self.beta * 2.0 ** -self.ts).astype(np.float32)
         out = [ic[0], beta[0]] if self.K == 1 else [ic, beta]
+        if self.pair:
+            out += [np.zeros_like(v) for v in out]
         if self.disp:
             out.append(np.float32(0.0) if self.K == 1 else np.zeros(self.K, np.float32))
         return out
@@ -182,9 +194,24 @@ def e4m3_digits(wr: np.ndarray, unit: float):
     return raw, vals
 
 
+def imatmul(A: np.ndarray, B: np.ndarray, block: int = 1 << 16) -> np.ndarray:
+    """``A @ B`` of integer matrices as int64, through fp64 BLAS in blocks of ``block`` rows of A and of the inner
+    dimension.  fp64 is exact here: every partial sum of a block is an integer of magnitude at most inner x max|a| x
+    max|b|, asserted below 2^53, and the blocks add in int64."""
+    n, m = A.shape
+    out = np.zeros((n, B.shape[1]), np.int64)
+    for i in range(0, n, block):
+        for j in range(0, m, block):
+            a = A[i : i + block, j : j + block].astype(np.float64)
+            b = B[j : j + block].astype(np.float64)
+            assert np.abs(a).max(initial=0) * np.abs(b).max(initial=0) * a.shape[1] < 2.0 ** 53
+            out[i : i + block] += (a @ b).astype(np.int64)
+    return out
+
+
 def _eta(case: Case, seg: Seg, beta: np.ndarray, o: Optional[np.ndarray]) -> np.ndarray:
     """eta [n, K] in grid units from integer coefficients [K, P] (units 2^-ts)."""
-    eta = seg.X @ beta.T + case.ic[:, seg.group][None, :]
+    eta = imatmul(seg.X, beta.T) + case.ic[:, seg.group][None, :]
     return eta + (o[:, None] if o is not None else 0)
 
 
@@ -217,6 +244,36 @@ def _window_sums(A: np.ndarray, bounds) -> int:
     return max(np.abs(cs[b] - cs[a]).max() for a, b in bounds) if bounds else 0
 
 
+def _window_xsums(absX: np.ndarray, col: np.ndarray, bounds) -> int:
+    """``_window_sums(absX * |col|[:, None], bounds)`` without forming the product: one window per row of a matrix
+    product."""
+    if not bounds:
+        return 0
+    M = np.zeros((len(bounds), absX.shape[0]), np.int64)
+    for j, (a, b) in enumerate(bounds):
+        M[j, a:b] = np.abs(col[a:b])
+    return int(imatmul(M, absX).max())
+
+
+def _row_blocks(n: int, starts, rows: int = 1 << 16):
+    """``[r0, r1)`` covering ``[0, n)`` in blocks of about ``rows`` rows, cut only at the given window starts (a
+    window, a chunk of the segment, stays in the block its start is in)."""
+    cuts = [0]
+    for a in sorted(starts):
+        if a - cuts[-1] >= rows:
+            cuts.append(a)
+    if not starts:
+        cuts = list(range(0, n, rows)) or [0]
+    return list(zip(cuts, cuts[1:] + [n]))
+
+
+def seg_rows(s: Seg, r0: int, r1: int) -> Seg:
+    """Rows ``[r0, r1)`` of a segment, as a segment (views)."""
+    cut = lambda v: None if v is None else v[r0:r1]
+    return Seg(s.X[r0:r1], s.y[r0:r1], cut(s.o), cut(s.w), s.nan[r0:r1], s.group, s.node, cut(s.xq), s.sc,
+               None if s.nz is None else s.nz[(s.nz[:, 0] >= r0) & (s.nz[:, 0] < r1)] - [r0, 0])
+
+
 def _lowbit(v: np.ndarray) -> np.ndarray:
     return v & -v
 
@@ -235,67 +292,81 @@ def budget(case: Case, sm_count: int = SM_H100) -> None:
         beta_terms = [np.rint(t * 2.0 ** case.ts).astype(np.int64) for t in terms]
     else:
         beta_terms = [case.beta]
-    for s in case.segs:
-        Xv = s.X * 2.0 ** -case.xs
-        if case.storage == "bf16":
-            assert np.array_equal(torch.from_numpy(Xv).to(torch.bfloat16).double().numpy(), Xv), "X is not bf16"
-        if k8:
-            assert np.all(np.abs(s.xq) <= 16), "e4m3 integers are exact up to 16"
     table = None
     if case.kernel in ("tc", "fp8"):
         table = chunk_table(case.n_rows, sm_count, *(FP8_CHUNKS if k8 else TC_CHUNKS))
     tot_xwr = np.zeros((case.K, case.P), np.int64)
     tot_wr = np.zeros(case.K, np.int64)
     tot_ll = 0
-    for si, s in enumerate(case.segs):
-        absX = np.abs(s.X)
-        # eta: every partial dot product of every term, then the intercept and the offset
-        for bt in beta_terms:
-            assert (absX @ np.abs(bt).T).max() < LIMIT, f"{case.name}: x' beta term exceeds the eta budget"
-        eta_abs = absX @ np.abs(case.beta).T + np.abs(case.ic[:, s.group])[None, :]
-        if s.o is not None:
-            eta_abs = eta_abs + np.abs(s.o)[:, None]
-        assert eta_abs.max() < LIMIT and np.abs(s.y).max() < LIMIT, f"{case.name}: |eta| or |y| over budget"
-        d, w, wr = _wr(case, s)
-        assert np.abs(d).max() < LIMIT
+    for si, seg in enumerate(case.segs):
         bounds = []
         if table is not None:
-            bounds = [(f * TILE, min(s.X.shape[0], (f + t) * TILE)) for seg, f, t in table if seg == si]
-        for k in range(case.K):
-            if case.kernel == "tc":
-                hi, lo = (np.rint(t / unit).astype(np.int64) for t in bf16_split(wr[:, k] * unit, 2))
-                assert np.array_equal(hi + lo, wr[:, k]), f"{case.name}: w r is not hi + lo in bf16"
-                cols = [hi, lo, wr[:, k]]
-            elif k8:
-                raw, vals = e4m3_digits(wr[:, k], unit)
-                assert np.array_equal(vals, np.rint(vals)), f"{case.name}: an e4m3 term of w r is off the grid"
-                vals = vals.astype(np.int64)
-                assert np.array_equal(vals.sum(0), wr[:, k]), f"{case.name}: w r is not its 4-term e4m3 expansion"
-                cols = [*vals, wr[:, k]]
-                # MMA #2: one wgmma K step = 32 rows of x_q . t_k, accumulated with fewer bits than fp32
-                n = s.X.shape[0]
-                ng = -(-n // 32)
-                xq = np.zeros((ng * 32, case.P), np.int64)
-                xq[:n] = s.xq
-                for t in raw:
-                    ti = np.zeros(ng * 32, np.int64)
-                    ti[:n] = np.rint(t * 512)                      # e4m3 values are multiples of 2^-9
-                    p = np.abs(xq.reshape(ng, 32, case.P) * ti.reshape(ng, 32, 1))
-                    lb = np.where(p > 0, _lowbit(p), np.int64(1) << 62).min(1)   # finest product per column
-                    tot = p.sum(1)
-                    assert np.all((tot == 0) | (tot < KSTEP_LIMIT * lb)), f"{case.name}: e4m3 K step over budget"
-            else:
-                cols = [wr[:, k]]
-            if table is not None:   # fp32 accumulation windows: the chunks
-                for col in cols:
-                    assert _window_sums(absX * np.abs(col)[:, None], bounds) < LIMIT, f"{case.name}: x r over budget"
-                assert _window_sums(np.abs(wr[:, k]), bounds) < LIMIT, f"{case.name}: sum w r over budget"
-                if case.disp:
-                    q = w * np.abs(d[:, k] ** 2 - (1 << 2 * case.e))
-                    assert _window_sums(q, bounds) < LIMIT, f"{case.name}: sum w q over budget"
-            tot_xwr[k] += (absX * np.abs(wr[:, k])[:, None]).sum(0)
-            tot_wr[k] += np.abs(wr[:, k]).sum()
-        tot_ll += int((w[:, None] * d * d).sum())
+            bounds = sorted((f * TILE, min(seg.X.shape[0], (f + t) * TILE)) for sg, f, t in table if sg == si)
+        # a long segment in blocks of whole chunks: every check below is per row or per chunk
+        for r0, r1 in _row_blocks(seg.X.shape[0], [a for a, _ in bounds]):
+            s = seg_rows(seg, r0, r1)
+            win = [(a - r0, b - r0) for a, b in bounds if r0 <= a < r1]
+            Xv = s.X * 2.0 ** -case.xs
+            if case.storage == "bf16":
+                assert np.array_equal(torch.from_numpy(Xv).to(torch.bfloat16).double().numpy(), Xv), "X is not bf16"
+            if k8:
+                assert np.all(np.abs(s.xq) <= 16), "e4m3 integers are exact up to 16"
+            absX = np.abs(s.X)
+            # eta: every partial dot product of every term, then the intercept and the offset
+            for bt in beta_terms:
+                assert imatmul(absX, np.abs(bt).T).max() < LIMIT, f"{case.name}: x' beta term exceeds the eta budget"
+            eta_abs = imatmul(absX, np.abs(case.beta).T) + np.abs(case.ic[:, s.group])[None, :]
+            if s.o is not None:
+                eta_abs = eta_abs + np.abs(s.o)[:, None]
+            assert eta_abs.max() < LIMIT and np.abs(s.y).max() < LIMIT, f"{case.name}: |eta| or |y| over budget"
+            d, w, wr = _wr(case, s)
+            assert np.abs(d).max() < LIMIT
+            for k in range(case.K):
+                if case.kernel == "tc":
+                    hi, lo = (np.rint(t / unit).astype(np.int64) for t in bf16_split(wr[:, k] * unit, 2))
+                    assert np.array_equal(hi + lo, wr[:, k]), f"{case.name}: w r is not hi + lo in bf16"
+                    cols = [hi, lo, wr[:, k]]
+                elif k8:
+                    raw, vals = e4m3_digits(wr[:, k], unit)
+                    assert np.array_equal(vals, np.rint(vals)), f"{case.name}: an e4m3 term of w r is off the grid"
+                    vals = vals.astype(np.int64)
+                    assert np.array_equal(vals.sum(0), wr[:, k]), f"{case.name}: w r is not its 4-term e4m3 expansion"
+                    cols = [*vals, wr[:, k]]
+                    # MMA #2: one wgmma K step = 32 rows of x_q . t_k, accumulated with fewer bits than fp32
+                    n = s.X.shape[0]
+                    ng = -(-n // 32)
+                    xq = np.zeros((ng * 32, case.P), np.int64)
+                    xq[:n] = s.xq
+                    for t in raw:
+                        ti = np.zeros(ng * 32, np.int64)
+                        ti[:n] = np.rint(t * 512)                      # e4m3 values are multiples of 2^-9
+                        p = np.abs(xq.reshape(ng, 32, case.P) * ti.reshape(ng, 32, 1))
+                        lb = np.where(p > 0, _lowbit(p), np.int64(1) << 62).min(1)   # finest product per column
+                        tot = p.sum(1)
+                        assert np.all((tot == 0) | (tot < KSTEP_LIMIT * lb)), f"{case.name}: e4m3 K step over budget"
+                else:
+                    cols = [wr[:, k]]
+                if table is not None:   # fp32 accumulation windows: the chunks
+                    for col in cols:
+                        assert _window_xsums(absX, col, win) < LIMIT, f"{case.name}: x r over budget"
+                    assert _window_sums(np.abs(wr[:, k]), win) < LIMIT, f"{case.name}: sum w r over budget"
+                    if case.disp:
+                        q = w * np.abs(d[:, k] ** 2 - (1 << 2 * case.e))
+                        assert _window_sums(q, win) < LIMIT, f"{case.name}: sum w q over budget"
+                if case.pair:
+                    # column 2k + 1 at s = 0: the residual w (d^2 - 1), units 2^-2e, through the same (hi, lo) split
+                    # and chunk sums as the mean's (d^2 - 1 is exact in fp32 below 2^24)
+                    assert (d[:, k] ** 2).max() < 1 << 24, f"{case.name}: d^2 over budget"
+                    ws = w * (d[:, k] ** 2 - (1 << 2 * case.e))
+                    u2 = 2.0 ** (-2 * case.e)
+                    hi, lo = (np.rint(t / u2).astype(np.int64) for t in bf16_split(ws * u2, 2))
+                    assert np.array_equal(hi + lo, ws), f"{case.name}: w (d^2 - 1) is not hi + lo in bf16"
+                    for col in (hi, lo, ws):
+                        assert _window_xsums(absX, col, win) < LIMIT, f"{case.name}: x w (d^2 - 1) over budget"
+                    assert _window_sums(np.abs(ws), win) < LIMIT, f"{case.name}: sum w (d^2 - 1) over budget"
+                tot_xwr[k] += imatmul(np.abs(wr[:, k])[None, :], absX)[0]
+                tot_wr[k] += np.abs(wr[:, k]).sum()
+            tot_ll += int((w[:, None] * d * d).sum())
     if table is None:   # CUDA-core kernels: a warp's fp32 sums may run over the whole model
         assert tot_xwr.max() < LIMIT and tot_wr.max() < LIMIT, f"{case.name}: model-wide sums over budget"
         if case.kernel == "custom":   # -w d^2 / 2 in units of half the grid's square
@@ -309,11 +380,14 @@ BUGS = ["r_hi", "theta_hi", "offset_bf16", "weight_shift", "drop_last", "stale_t
 
 def oracle(case: Case, bug: Optional[str] = None):
     """The expected gradients in int64, in the kernel's layout: ``(gi [n_nodes, K, G] grid units, gb [n_nodes, K, P]
-    units 2^-xs of the grid, q [n_nodes, K] units of the grid squared)``.  ``bug`` applies one of :data:`BUGS`."""
+    units 2^-xs of the grid, q [n_nodes, K] units of the grid squared)``.  ``bug`` applies one of :data:`BUGS`.  A
+    pair case has 2K columns: 2k the mean's, as above, and 2k + 1 the scale's, in units of the grid squared (gi) and
+    2^-xs of it (gb)."""
     K, G, P = case.K, case.G, case.P
-    gi = np.zeros((case.n_nodes, K, G), np.int64)
-    gb = np.zeros((case.n_nodes, K, P), np.int64)
-    q = np.zeros((case.n_nodes, K), np.int64)
+    gi = np.zeros((case.n_nodes, case.columns, G), np.int64)
+    gb = np.zeros((case.n_nodes, case.columns, P), np.int64)
+    q = np.zeros((case.n_nodes, case.columns), np.int64)
+    mean = slice(0, None, 2) if case.pair else slice(None)
     unit = 2.0 ** -case.e
     beta = case.beta
     if bug == "theta_hi":
@@ -339,8 +413,12 @@ def oracle(case: Case, bug: Optional[str] = None):
             wr_b[TILE : TILE + m] = wr[:m]   # tile 1 multiplied with tile 0's residuals
         node = (s.node + 1) % case.n_nodes if bug == "wrong_node" and si == 0 else s.node
         grp = (s.group + 1) % G if bug == "wrong_group" and si == 0 else s.group
-        gi[node, :, grp] += wr.sum(0)
-        gb[node] += wr_b.T @ s.X
+        gi[node, mean, grp] += wr.sum(0)
+        gb[node, mean] += imatmul(wr_b.T, s.X)
+        if case.pair:   # the scale column at s = 0: dll/ds = z^2 - 1 with z = d
+            ws = ww[:, None] * (d * d - (1 << 2 * case.e))
+            gi[node, 1::2, grp] += ws.sum(0)
+            gb[node, 1::2] += imatmul(ws.T, s.X)
         if case.disp and bug != "drop_q":
             q[node] += (ww[:, None] * (d * d - (1 << 2 * case.e))).sum(0)
     if bug == "swap_chains":
@@ -349,9 +427,11 @@ def oracle(case: Case, bug: Optional[str] = None):
 
 
 def expected_raw(case: Case, ints, ll: np.ndarray) -> np.ndarray:
-    """``[n_nodes, K, 1 + G + P (+ 1)]`` float64 (exact) from the oracle's integers and a log-likelihood per block."""
+    """``[n_nodes, K, 1 + G + P (+ 1)]`` float64 (exact) from the oracle's integers and a log-likelihood per block
+    (pair cases: ``[n_nodes, 2K, 1 + G + P]``)."""
     gi, gb, q = ints
-    parts = [ll[..., None], gi * 2.0 ** -case.e, gb * 2.0 ** -(case.e + case.xs)]
+    e = np.tile([case.e, 2 * case.e], case.K)[None, :, None] if case.pair else case.e
+    parts = [ll[..., None], gi * 2.0 ** -e, gb * 2.0 ** -(e + case.xs)]
     if case.disp:
         parts.append((q * 2.0 ** (-2 * case.e))[..., None])
     return np.concatenate(parts, axis=2)
@@ -409,7 +489,9 @@ def build_model(case: Case, device) -> GlmShards:
         buf = torch.zeros(n * ld + 1, dtype=dt, device=device)
         first = 1 if case.misalign else 0
         X = buf[first : first + n * ld].view(n, ld)[:, : case.P]
-        X.copy_(torch.tensor(s.X * 2.0 ** -case.xs, dtype=torch.float32).to(dt))
+        X.copy_((torch.from_numpy(s.X).to(device, torch.float32) * 2.0 ** -case.xs).to(dt))
+        if s.nz is not None and len(s.nz):
+            X[torch.from_numpy(s.nz[:, 0]).to(device), torch.from_numpy(s.nz[:, 1]).to(device)] = -0.0
         Xs.append(X)
     kw = dict(groups=[s.group for s in case.segs], n_groups=case.G, n_chains=case.K,
               offsets=os_ if any(o is not None for o in os_) else None,
